@@ -48,8 +48,8 @@ __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefe
 
 template <int WARPS, int STAGES>
 __global__ void __launch_bounds__(WARPS * 32, 1)
-k1_ingest_tma(const __grid_constant__ CUtensorMap tmap, const agr_dev d, const uint32_t first_rid, const uint32_t n,
-              const uint32_t pf_dist) {
+k1_ingest_tma(const __grid_constant__ CUtensorMap tmap, const agr_dev d, const uint32_t first_rid, const unsigned long long first_log,
+              const uint32_t n, const uint32_t pf_dist) {
     extern __shared__ uint8_t smem_raw[];
     __shared__ uint64_t bars[WARPS * STAGES];
     __shared__ uint32_t s_ctr[K1_NLC];
@@ -167,7 +167,7 @@ k1_ingest_tma(const __grid_constant__ CUtensorMap tmap, const agr_dev d, const u
         }
         // this tile: agent loads have landed by now; classify and put the index CAS in flight.  pcx is dead here
         // (just consumed), so the CAS writes straight into the loop-carried registers.
-        if (valid) k1_begin(d, ap, h0, h1, h2, h3, h4, h5.x, AGR_REC - AGR_OFF_PAYLOAD, 0ULL, pcx);
+        if (valid) k1_begin(d, ap, h0, h1, h2, h3, h4, h5.x, AGR_REC - AGR_OFF_PAYLOAD, first_log, pcx);
         ph1 = h1; ph5y = h5.y; prid = rid; pvalid = valid; ptile = tile;
         if (s == STAGES - 1) phase ^= 1u;
     }
@@ -209,8 +209,8 @@ int agr_k1_tma_make_map(void* slab, unsigned long long rows, void* out_map /*128
 }
 
 template <int WARPS, int STAGES>
-static cudaError_t launch_tma(const void* map, const agr_dev& d, uint32_t first_rid, uint32_t n, uint32_t pf_dist, int sm_count,
-                              cudaStream_t st) {
+static cudaError_t launch_tma(const void* map, const agr_dev& d, uint32_t first_rid, unsigned long long first_log, uint32_t n,
+                              uint32_t pf_dist, int sm_count, cudaStream_t st) {
     const size_t smem = (size_t)WARPS * STAGES * TILE_BYTES + 1024;
     static bool attr_done = false;
     if (!attr_done) {
@@ -222,17 +222,17 @@ static cudaError_t launch_tma(const void* map, const agr_dev& d, uint32_t first_
     uint32_t blocks = (uint32_t)sm_count;
     const uint32_t need = (tiles + WARPS - 1) / WARPS;
     if (blocks > need) blocks = need;
-    k1_ingest_tma<WARPS, STAGES><<<blocks, WARPS * 32, smem, st>>>(*(const CUtensorMap*)map, d, first_rid, n, pf_dist);
+    k1_ingest_tma<WARPS, STAGES><<<blocks, WARPS * 32, smem, st>>>(*(const CUtensorMap*)map, d, first_rid, first_log, n, pf_dist);
     return cudaGetLastError();
 }
 
 // variant 1 (default TMA): 7 warps x 2 stages; 2: 6 x 2; 3: 4 x 3; 4: 14 x 1 (all: one persistent CTA per SM)
-cudaError_t agr_launch_k1_tma(uint32_t variant, const void* map, const agr_dev& d, uint32_t first_rid, uint32_t n, uint32_t pf_dist,
-                              int sm_count, cudaStream_t st) {
+cudaError_t agr_launch_k1_tma(uint32_t variant, const void* map, const agr_dev& d, uint32_t first_rid, unsigned long long first_log,
+                              uint32_t n, uint32_t pf_dist, int sm_count, cudaStream_t st) {
     switch (variant) {
-        case 2: return launch_tma<6, 2>(map, d, first_rid, n, pf_dist, sm_count, st);
-        case 3: return launch_tma<4, 3>(map, d, first_rid, n, pf_dist, sm_count, st);
-        case 4: return launch_tma<14, 1>(map, d, first_rid, n, pf_dist, sm_count, st);
-        default: return launch_tma<7, 2>(map, d, first_rid, n, pf_dist, sm_count, st);
+        case 2: return launch_tma<6, 2>(map, d, first_rid, first_log, n, pf_dist, sm_count, st);
+        case 3: return launch_tma<4, 3>(map, d, first_rid, first_log, n, pf_dist, sm_count, st);
+        case 4: return launch_tma<14, 1>(map, d, first_rid, first_log, n, pf_dist, sm_count, st);
+        default: return launch_tma<7, 2>(map, d, first_rid, first_log, n, pf_dist, sm_count, st);
     }
 }

@@ -98,16 +98,24 @@ __global__ void __launch_bounds__(256) k1_post(const agr_dev d, const uint32_t f
     const uint32_t stride = gridDim.x * blockDim.x;
     const int lane = threadIdx.x & 31;
     int delta[3] = {0, 0, 0};                                                     // dedupe hits, stored, queued
-    for (uint32_t i0 = blockIdx.x * blockDim.x; i0 < n; i0 += stride) {
-        const uint32_t i = i0 + threadIdx.x;
-        if (i >= n) continue;
-        // with the K1 kernel's row marks and nothing else to do for unmarked rows, 4 B per 32 rows decide who stays
-        const bool marked = marks && ((__ldg(&marks[i >> 5]) >> (i & 31u)) & 1u);
-        if (marks && !marked && dupfix == 0u && verdicts == nullptr && ids == nullptr) continue;
-        const uint32_t rid = first_rid + i;
-        const uint32_t r = k1_post_one(d, rid, dupfix, delta, marked);
-        if (verdicts) verdicts[i] = k1_verdict_word(r);
-        if (ids) ids[i] = k1_request_id(d, rid);
+    if (marks && dupfix == 0u && (d.cfg_flags & AGR_CFG_MINT_IDS) && verdicts == nullptr && ids == nullptr) {
+        // minted ids: K1 has decided every replay that names a row of an earlier batch, so the few rows left are far apart.  One
+        // thread per marks word (agr_launch_k1 sizes the grid for n / 32 threads) walks the word's set bits.
+        for (uint32_t w = blockIdx.x * blockDim.x + threadIdx.x; w < (n + 31u) / 32u; w += stride) {
+            for (uint32_t m = __ldg(&marks[w]); m != 0u; m &= m - 1u) k1_post_one(d, first_rid + w * 32u + (uint32_t)(__ffs(m) - 1), 0u, delta, true);
+        }
+    } else {
+        for (uint32_t i0 = blockIdx.x * blockDim.x; i0 < n; i0 += stride) {
+            const uint32_t i = i0 + threadIdx.x;
+            if (i >= n) continue;
+            // with the K1 kernel's row marks and nothing else to do for unmarked rows, 4 B per 32 rows decide who stays
+            const bool marked = marks && ((__ldg(&marks[i >> 5]) >> (i & 31u)) & 1u);
+            if (marks && !marked && dupfix == 0u && verdicts == nullptr && ids == nullptr) continue;
+            const uint32_t rid = first_rid + i;
+            const uint32_t r = k1_post_one(d, rid, dupfix, delta, marked);
+            if (verdicts) verdicts[i] = k1_verdict_word(r);
+            if (ids) ids[i] = k1_request_id(d, rid);
+        }
     }
     // counter corrections: one global atomic per CTA and counter (thousands of warps adding to the same three words would
     // serialise in L2 for longer than the pass itself takes)
@@ -443,23 +451,25 @@ static uint32_t k1_post_blocks(uint32_t n, int sm_count) {
     return b < cap ? b : cap;
 }
 
-cudaError_t agr_launch_k1_tma(uint32_t variant, const void* map, const agr_dev& d, uint32_t first_rid, uint32_t n, uint32_t pf_dist,
-                              int sm_count, cudaStream_t st);
+cudaError_t agr_launch_k1_tma(uint32_t variant, const void* map, const agr_dev& d, uint32_t first_rid, unsigned long long first_log,
+                              uint32_t n, uint32_t pf_dist, int sm_count, cudaStream_t st);
 
 void agr_launch_k1_post(const agr_dev& d, uint32_t first_rid, uint32_t n, int sm_count, cudaStream_t st, void* verdicts, void* ids,
                         const uint32_t* marks) {
     if (n) k1_post<<<k1_post_blocks(n, sm_count), 256, 0, st>>>(d, first_rid, n, (uint2*)verdicts, (uint4*)ids, marks);
 }
 
-void agr_launch_k1(const agr_dev& d, uint32_t first_rid, uint32_t n, uint32_t variant, const void* tmap, int sm_count,
-                   cudaStream_t st, cudaEvent_t ev0, cudaEvent_t ev1, void* verdicts, void* ids) {
+void agr_launch_k1(const agr_dev& d, uint32_t first_rid, unsigned long long first_log, uint32_t n, uint32_t variant, const void* tmap,
+                   int sm_count, cudaStream_t st, cudaEvent_t ev0, cudaEvent_t ev1, void* verdicts, void* ids) {
     if (n == 0) return;
     if (ev0) cudaEventRecord(ev0, st);
     if ((variant & 0xfu) != AGR_K1_LSU && tmap != nullptr) {
-        agr_launch_k1_tma(variant & 0xfu, tmap, d, first_rid, n, (variant >> 8) & 0xffu, sm_count, st);
+        agr_launch_k1_tma(variant & 0xfu, tmap, d, first_rid, first_log, n, (variant >> 8) & 0xffu, sm_count, st);
         if (ev1) cudaEventRecord(ev1, st);
         if ((d.cfg_flags & AGR_CFGI_SPLIT_INDEX) && !(d.cfg_flags & AGR_CFG_MINT_IDS)) k1_index<<<(n + 255u) / 256u, 256, 0, st>>>(d, first_rid, n);
-        k1_post<<<k1_post_blocks(n, sm_count), 256, 0, st>>>(d, first_rid, n, (uint2*)verdicts, (uint4*)ids, d.marks);
+        // minted ids never race for an id (dupfix stays 0): without verdicts or ids to write, k1_post visits the marked rows only
+        const bool sparse = d.marks && (d.cfg_flags & AGR_CFG_MINT_IDS) && verdicts == nullptr && ids == nullptr;
+        k1_post<<<k1_post_blocks(sparse ? (n + 31u) / 32u : n, sm_count), 256, 0, st>>>(d, first_rid, n, (uint2*)verdicts, (uint4*)ids, d.marks);
         return;
     }
     constexpr int WARPS = 8;

@@ -163,8 +163,10 @@ void agr_launch_k4_scatter(const agr_k4_params& p, cudaStream_t st);
 void agr_launch_k4_unpermute(const agr_k4_params& p, const void* local_res, const void* remote_res, void* out, uint32_t res_bytes,
                              cudaStream_t st);
 
-void agr_launch_k1(const agr_dev& d, uint32_t first_rid, uint32_t n, uint32_t variant, const void* tmap, int sm_count,
-                   cudaStream_t st, cudaEvent_t ev0 = nullptr, cudaEvent_t ev1 = nullptr,
+// first_log: arrival number of the batch's first row (= first_rid unless the slab is a ring).  With engine-minted ids the TMA
+// kernels decide a replay's dedupe hit on a row of an earlier batch themselves; k1_post resolves only the rest.
+void agr_launch_k1(const agr_dev& d, uint32_t first_rid, unsigned long long first_log, uint32_t n, uint32_t variant, const void* tmap,
+                   int sm_count, cudaStream_t st, cudaEvent_t ev0 = nullptr, cudaEvent_t ev1 = nullptr,
                    void* verdicts = nullptr /* device agr_verdict[n], written by k1_post */,
                    void* ids = nullptr /* device u8[n][16]: Request.ID per record, written by k1_post */);
 void agr_launch_expire(const agr_dev& d, unsigned long long rows, unsigned long long now, unsigned long long ttl,
