@@ -72,6 +72,7 @@ ABI_SYMBOLS = [
     "agr_agent_hash", "agr_agent_shard", "agr_comm_unique_id", "agr_comm_init", "agr_ingest_sharded", "agr_complete_sharded", "agr_snapshot", "agr_restore", "agr_verify", "agr_store_response_body", "agr_get_response_body",
     "agr_store_response", "agr_store_error_text", "agr_get_record_json", "agr_pending_json", "agr_rows_json", "agr_expire", "agr_reclaim", "agr_set_agent_states", "agr_json_decode",
     "agr_submit_ingest", "agr_submit_complete", "agr_poll", "agr_wait", "agr_ring_capacity", "agr_ingest_sharded_rows", "agr_fill_rows", "agr_reclaim_async",
+    "agr_complete_ex", "agr_submit_complete_ex",
 ]
 
 _lib = None
@@ -112,6 +113,10 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
         "agr_replay_scan_var": (i32, [vp, vp, vp, u64, vp, u32, C.POINTER(u32), C.POINTER(u64)]),
         "agr_get_record_var": (i32, [vp, C.c_char_p, vp, vp, u32, C.POINTER(u32)]),
         "agr_complete": (i32, [vp, vp, u32, vp]),
+        "agr_complete_ex": (i32, [vp, vp, u32, vp, vp, vp, vp]),
+        "agr_submit_complete_ex": (i32, [vp, vp, vp, u32, vp, u32, C.POINTER(u64)]),
+        "agr_submit_complete": (i32, [vp, vp, C.POINTER(u64)]),
+        "agr_wait": (i32, [vp, u64, vp]),
         "agr_replay_scan": (i32, [vp, vp, vp, u32, C.POINTER(u32)]),
         "agr_pending": (i32, [vp, C.c_char_p, vp, u32, C.POINTER(u32)]),
         "agr_get_record": (i32, [vp, C.c_char_p, vp, vp]),
@@ -458,6 +463,62 @@ class Engine:
         res = np.zeros(n, dtype=np.int32) if want_results else None
         _check(self.lib, self.lib.agr_complete(self.h, _ptr(outs), n, _ptr(res) if want_results else None))
         return res
+
+    def complete_ex(self, outs: np.ndarray, segments, hdr_lens: Optional[np.ndarray] = None, want_results: bool = True):
+        """agr_complete_ex: the outcomes with the bytes StoreResponse / MarkRequestFailed keep.  segments: one bytes object per
+        outcome (headers then body of a response, the text of an error, b"" otherwise), or a (uint8 blob, uint64 offsets[n + 1])
+        pair.  hdr_lens: uint32 per outcome, the leading header bytes of a response segment.  Returns (rc, results): rc is 0 or
+        AGR_ENOSPC (transitions applied, no byte of the batch stored); any other error raises."""
+        assert outs.dtype == outcome_dtype and outs.flags["C_CONTIGUOUS"]
+        n = len(outs)
+        if isinstance(segments, tuple):
+            blob, offs = segments
+        else:
+            assert len(segments) == n
+            offs = np.zeros(n + 1, dtype=np.uint64)
+            offs[1:] = np.cumsum([len(s) for s in segments], dtype=np.uint64)
+            blob = np.frombuffer(b"".join(segments) or b"\0", dtype=np.uint8)
+        assert blob.dtype == np.uint8 and offs.dtype == np.uint64 and len(offs) == n + 1
+        if hdr_lens is not None:
+            hdr_lens = np.ascontiguousarray(hdr_lens, dtype=np.uint32)
+            assert len(hdr_lens) == n
+        res = np.zeros(n, dtype=np.int32) if want_results else None
+        rc = self.lib.agr_complete_ex(self.h, _ptr(outs) if n else None, n, _ptr(blob), _ptr(offs),
+                                      _ptr(hdr_lens) if hdr_lens is not None else None, _ptr(res) if want_results and n else None)
+        if rc != K.AGR_ENOSPC:
+            _check(self.lib, rc)
+        return rc, res
+
+    # ---- tickets (AGR_CFG_COMBINE)
+    def submit_complete(self, outcome: np.ndarray) -> int:
+        assert outcome.dtype == outcome_dtype
+        o = np.ascontiguousarray(outcome.reshape(1))
+        t = C.c_uint64()
+        while True:
+            rc = self.lib.agr_submit_complete(self.h, _ptr(o), C.byref(t))
+            if rc != K.AGR_EAGAIN:
+                _check(self.lib, rc)
+                return int(t.value)
+
+    def submit_complete_ex(self, outcome: np.ndarray, headers: bytes, body: bytes) -> int:
+        """agr_submit_complete_ex: the outcome and its bytes (<= AGR_OUT_INLINE_BYTES) in one ticket; collect it with wait()."""
+        assert outcome.dtype == outcome_dtype
+        o = np.ascontiguousarray(outcome.reshape(1))
+        hb = (C.c_uint8 * max(1, len(headers))).from_buffer_copy(headers or b"\0")
+        bb = (C.c_uint8 * max(1, len(body))).from_buffer_copy(body or b"\0")
+        t = C.c_uint64()
+        while True:
+            rc = self.lib.agr_submit_complete_ex(self.h, _ptr(o), C.cast(hb, C.c_void_p), len(headers), C.cast(bb, C.c_void_p),
+                                                 len(body), C.byref(t))
+            if rc != K.AGR_EAGAIN:
+                _check(self.lib, rc)
+                return int(t.value)
+
+    def wait(self, ticket: int) -> int:
+        """agr_wait on an outcome's ticket: its result code (0, AGR_ENOTFOUND, AGR_ENOSPC)."""
+        out = (C.c_uint8 * 40)()
+        _check(self.lib, self.lib.agr_wait(self.h, C.c_uint64(ticket), C.cast(out, C.c_void_p)))
+        return int(np.frombuffer(bytes(out), dtype="<i4")[8])
 
     # ---- K3
     def replay_scan(self, with_records: bool = True, cap: int = 1 << 16):

@@ -358,6 +358,24 @@ __device__ __forceinline__ void k1_post_flush(const agr_dev& d, int* delta, cons
 }
 
 // ------------------------------------------------------------------------------------------------ K2
+// A warp copies len bytes from src (any alignment; global or shared memory) to the 16-byte aligned dst with 16-byte stores; the
+// last store fills the tail of dst's 16-byte rounded space.  Lane l reads the aligned 16-byte blocks around its output block
+// and funnel-shifts them into place; a block is read only if it holds a byte of the segment.
+__device__ __forceinline__ void warp_copy16(uint4* dst, const uint8_t* src, const uint32_t len, const uint32_t lane) {
+    const uint32_t sh = (uint32_t)reinterpret_cast<uintptr_t>(src) & 15u, q = sh >> 2, r = (sh & 3u) * 8u;
+    const uint4* as = reinterpret_cast<const uint4*>(src - sh);
+    const uint32_t chunks = (len + 15u) >> 4;
+    for (uint32_t c = lane; c < chunks; c += 32u) {
+        const uint4 lo = as[c];
+        uint4 hi = make_uint4(0u, 0u, 0u, 0u);
+        if (sh && sh + len > 16u * (c + 1u)) hi = as[c + 1u];
+        uint32_t w0 = lo.x, w1 = lo.y, w2 = lo.z, w3 = lo.w, w4 = hi.x, w5 = hi.y, w6 = hi.z, w7 = hi.w;
+        if (q & 2u) { w0 = w2; w1 = w3; w2 = w4; w3 = w5; w4 = w6; w5 = w7; }
+        if (q & 1u) { w0 = w1; w1 = w2; w2 = w3; w3 = w4; w4 = w5; }
+        dst[c] = make_uint4(__funnelshift_r(w0, w1, r), __funnelshift_r(w1, w2, r), __funnelshift_r(w2, w3, r), __funnelshift_r(w3, w4, r));
+    }
+}
+
 // One outcome (64 B agr_outcome as four 16 B words: request id | agent id[0..15] | agent id[16..31] | kind,http,seq):
 // resolve the agent in the device agent table (no per-outcome host work) and the request id to its row, write the 16 B op
 // and thread it onto its row's chain (head[row] = index of the last op linked + 1).
@@ -431,16 +449,29 @@ __device__ __forceinline__ uint32_t k2_apply_op(k2_row& r, const uint32_t kh, co
 // Op j applies its row's chain if it is the chain ROOT (the last op linked onto the row).  One outcome per row and batch is
 // the common case and takes no loop at all; short chains are sorted in registers (the walk order is the link order, which is
 // arbitrary); longer ones fall back to repeated minimum selection over the chain.
+// BYTES (agr_complete_ex): the ops carry bytes; the root also stores the segments of its row's last RESPONSE and last ERROR
+// op (the latest StoreResponse / MarkRequestFailed SET wins) and marks those ops K2_EFF_WIN for the copy.
 #define K2_SORT_MAX 8
-__device__ __forceinline__ void k2_apply_one(const agr_dev& d, const agr_k2_scratch& s, const uint32_t j, uint32_t* cnt) {
+template <bool BYTES>
+__device__ __forceinline__ void k2_note_bytes(const agr_k2_bytes* b, const uint32_t o, const uint32_t kh, int& wr, int& we) {
+    if (BYTES && b->dst[o] != K2_NO_BYTES) {                               // (plain outcomes of a service-kernel batch carry none)
+        if ((kh & 0xffu) == AGR_OUT_RESPONSE) wr = (int)o;
+        else if ((kh & 0xffu) == AGR_OUT_ERROR) we = (int)o;
+    }
+}
+template <bool BYTES = false>
+__device__ __forceinline__ void k2_apply_one(const agr_dev& d, const agr_k2_scratch& s, const uint32_t j, uint32_t* cnt,
+                                             const agr_k2_bytes* b = nullptr) {
     const agr_k2op me = s.ops[j];
     const uint32_t rid = me.rid;
     if (rid == AGR_RID_NONE) return;
     if (__ldcg(&d.head[rid]) != j + 1u) return;
     k2_row r{d.state[rid], d.aux[rid], 0ULL, 0ULL, false, false};
+    int wr = -1, we = -1;                                                  // BYTES: last RESPONSE / ERROR op of the row
     const uint32_t first = __ldcg(&s.nxt[j]);
     if (first == 0u) {
         s.eff[j] = (uint8_t)k2_apply_op(r, me.kh, me.seq, cnt);
+        k2_note_bytes<BYTES>(b, j, me.kh, wr, we);
     } else {
         uint32_t idx[K2_SORT_MAX];
         uint32_t len = 0;
@@ -459,7 +490,11 @@ __device__ __forceinline__ void k2_apply_one(const agr_dev& d, const agr_k2_scra
         if (len <= K2_SORT_MAX) {
 #pragma unroll
             for (int k = 0; k < K2_SORT_MAX; ++k) {
-                if ((uint32_t)k < len) { const agr_k2op op = s.ops[idx[k]]; s.eff[idx[k]] = (uint8_t)k2_apply_op(r, op.kh, op.seq, cnt); }
+                if ((uint32_t)k < len) {
+                    const agr_k2op op = s.ops[idx[k]];
+                    s.eff[idx[k]] = (uint8_t)k2_apply_op(r, op.kh, op.seq, cnt);
+                    k2_note_bytes<BYTES>(b, idx[k], op.kh, wr, we);
+                }
             }
         } else {
             long long last = -1;
@@ -473,7 +508,21 @@ __device__ __forceinline__ void k2_apply_one(const agr_dev& d, const agr_k2_scra
                 last = best;
                 const agr_k2op op = s.ops[best];
                 s.eff[best] = (uint8_t)k2_apply_op(r, op.kh, op.seq, cnt);
+                k2_note_bytes<BYTES>(b, best, op.kh, wr, we);
             }
+        }
+    }
+    if (BYTES) {
+        if (wr >= 0) {
+            b->resp_off[rid] = b->base + b->dst[wr];
+            b->resp_len[rid] = (uint32_t)(b->src_off[wr + 1] - b->src_off[wr]);
+            b->resp_hlen[rid] = b->hlen ? b->hlen[wr] : 0u;
+            s.eff[wr] |= (uint8_t)K2_EFF_WIN;
+        }
+        if (we >= 0) {
+            b->err_off[rid] = b->base + b->dst[we];
+            b->err_len[rid] = (uint32_t)(b->src_off[we + 1] - b->src_off[we]);
+            s.eff[we] |= (uint8_t)K2_EFF_WIN;
         }
     }
     d.state[rid] = r.st;

@@ -118,6 +118,10 @@ struct agr_handle {
     unsigned long long* d_resp_off = nullptr; uint32_t* d_resp_len = nullptr;
     uint32_t* d_resp_hlen = nullptr;           // leading bytes of the stored response that are its flattened headers
     unsigned long long* d_err_off = nullptr; uint32_t* d_err_len = nullptr;   // Request.Error text, same byte slab
+    // agr_complete_ex staging, allocated on first use: per-op offsets / slab places / header lengths, and the batch's bytes
+    unsigned long long *h_boff = nullptr, *d_boff = nullptr, *h_bdst = nullptr, *d_bdst = nullptr;
+    uint32_t *h_bhlen = nullptr, *d_bhlen = nullptr;
+    uint8_t *h_bsrc = nullptr, *d_bsrc = nullptr; size_t h_bsrc_cap = 0, d_bsrc_cap = 0;
     // K5 (JSON wire form) scratch
     uint32_t* d_jlen = nullptr; unsigned long long* d_joff = nullptr; unsigned long long* d_jchunk = nullptr; uint32_t j_cap = 0;
     uint8_t* d_json = nullptr; uint64_t json_cap = 0;
@@ -278,6 +282,7 @@ static void pack_agent_id(const char* id, unsigned long long w[4]) {
 // device-mapped memory, a release store publishes it, and the caller waits on a word the GPU writes.  One dispatcher thread
 // per handle turns the published prefix of the ring into batch descriptors; the resident service kernel (k_svc) does the rest.
 extern "C" { static int reserve_rows_locked(agr_handle* h, uint32_t n, uint64_t* first); }
+extern "C" { static int resp_reserve_locked(agr_handle* h, uint64_t need, uint64_t len, unsigned long long* off); }
 cudaError_t agr_launch_svc(const agr_dev& d, const svc_dev& v, const agr_k2_scratch& k2, unsigned long long next_seq, cudaStream_t st);
 unsigned long long agr_svc_desc_check(const svc_desc* dsc);
 
@@ -299,6 +304,7 @@ struct svc_host {
     std::chrono::steady_clock::time_point started;      // when it was launched
     agr_k2_scratch k2{};                                // K2 scratch of the service kernel (SVC_MAX_OPS ops)
     uint32_t* d_dupfix = nullptr;
+    unsigned long long *d_boff = nullptr, *d_bdst = nullptr; uint32_t* d_bhlen = nullptr;   // per-outcome byte places (svc_dev)
     std::atomic<uint64_t> batches{0}, ops{0};
     // diagnostics (AGR_SVC_DEBUG=1 prints them when the handle is destroyed)
     uint64_t starts = 0, stops = 0, sleeps = 0, flow_waits = 0;
@@ -339,6 +345,8 @@ static int svc_start_locked(agr_handle* h) {
     if (s->running) return 0;
     svc_dev v{};
     v.desc = s->desc; v.payload = s->payload; v.res = s->res; v.ctl = s->ctl; v.dupfix = s->d_dupfix;
+    v.resp = h->d_resp; v.resp_off = h->d_resp_off; v.resp_len = h->d_resp_len; v.resp_hlen = h->d_resp_hlen;
+    v.err_off = h->d_err_off; v.err_len = h->d_err_len; v.b_off = s->d_boff; v.b_dst = s->d_bdst; v.b_hlen = s->d_bhlen;
     v.idle_ns = 2000000000ULL;                                   // safety only: the dispatcher stops the kernel long before
     s->ctl->state = 1; s->ctl->stop = 0;
     std::atomic_thread_fence(std::memory_order_seq_cst);
@@ -389,10 +397,10 @@ static void svc_dispatcher(agr_handle* h) {
     // the contiguous published prefix [taken, to), grown INCREMENTALLY: a slot is looked at until it is published and never again
     // (re-reading the callers' ready words every iteration keeps pulling their cache lines away from the cores that write them)
     uint64_t to = s->taken;
-    uint32_t nrec = 0;
+    uint32_t nstaged = 0;                                        // records + outcomes with bytes: one 512 B stage slot of k_svc each
     uint32_t kinds[SVC_MAX_OPS / 16] = {0};
     while (!s->shutdown.load(std::memory_order_acquire)) {
-        svc_scan(s, s->taken, &to, &nrec, kinds, 128u);           // (csrc/agr_ring.hpp: shared with the CPU simulation of the ring)
+        svc_scan(s, s->taken, &to, &nstaged, kinds, 128u);        // (csrc/agr_ring.hpp: shared with the CPU simulation of the ring)
         const auto now = std::chrono::steady_clock::now();
         if (to == s->taken) {
             const auto idle = std::chrono::duration_cast<std::chrono::microseconds>(now - last_work).count();
@@ -423,13 +431,26 @@ static void svc_dispatcher(agr_handle* h) {
         }
         spins = 0;
         std::lock_guard<std::mutex> hl(h->mu);
-        if (s->fatal.load()) { svc_fail_ops(s, s->taken, to, s->fatal.load(), false); s->taken = to; nrec = 0; memset(kinds, 0, sizeof kinds); continue; }
+        if (s->fatal.load()) { svc_fail_ops(s, s->taken, to, s->fatal.load(), false); s->taken = to; nstaged = 0; memset(kinds, 0, sizeof kinds); continue; }
         if (s->running && s->ctl->state != 1u) {                // it left on its own (safety timeout): note it and start another
             cudaStreamSynchronize(h->stream);
             s->running = false;
         }
         // a resident kernel blocks device-wide synchronisations of other threads (cudaFree ...): let it go every 20 ms
         if (s->running && std::chrono::duration_cast<std::chrono::milliseconds>(now - s->started).count() > 20) svc_stop_locked(h);
+        // records, and the outcomes with bytes with their segments' region (16 B-rounded, in ring order)
+        uint32_t nrec = 0, nbytes = 0;
+        uint64_t byte_total = 0;
+        for (uint32_t k = 0; k < (uint32_t)(to - s->taken); ++k) {
+            const uint32_t kd = (kinds[k >> 4] >> ((k & 15u) * 2u)) & 3u;
+            if (kd == SVC_OP_RECORD) nrec++;
+            if (kd == SVC_OP_OUTCOME_BYTES) {                    // (the slot's payload is visible: its ready word was acquired)
+                uint32_t len;
+                memcpy(&len, s->payload + (size_t)((s->taken + k) & (SVC_SLOTS - 1u)) * SVC_PAYLOAD + SVC_BYTES_HDR + 4, 4);
+                byte_total += (std::min(len, SVC_BYTES_MAX) + 15u) & ~15u;
+                nbytes++;
+            }
+        }
         uint64_t first = 0;
         bool have_rows = true;
         if (nrec) {
@@ -440,6 +461,11 @@ static void svc_dispatcher(agr_handle* h) {
             uint32_t kd = (kinds[k >> 4] >> ((k & 15u) * 2u)) & 3u;
             if (kd == SVC_OP_RECORD && !have_rows) kd = SVC_OP_SKIP;
             dsc.kinds[k >> 4] |= kd << ((k & 15u) * 2u);
+        }
+        dsc.resp_base = SVC_NO_BYTES;
+        if (nbytes) {
+            unsigned long long off;
+            if (resp_reserve_locked(h, byte_total, byte_total, &off) == 0) dsc.resp_base = off;
         }
         dsc.from = s->taken; dsc.count = (uint32_t)(to - s->taken); dsc.n_records = have_rows ? nrec : 0u;
         dsc.first_l = first; dsc.first_p = (uint32_t)phys_row(h, first);
@@ -461,7 +487,7 @@ static void svc_dispatcher(agr_handle* h) {
         s->ops.fetch_add(dsc.count, std::memory_order_relaxed);
         h->k1_launches += nrec ? 1 : 0;                         // accounting: batches with records / with outcomes served by k_svc
         h->k2_launches += (dsc.count > nrec) ? 1 : 0;
-        nrec = 0; memset(kinds, 0, sizeof kinds);
+        nstaged = 0; memset(kinds, 0, sizeof kinds);
         if (!s->running && svc_start_locked(h) < 0) {
             // could not launch: nothing will ever process this batch — fail it from here
             svc_fail_ops(s, dsc.from, to, AGR_ECUDA, false);
@@ -507,6 +533,9 @@ static int svc_create(agr_handle* h) {
     TRY(dev_alloc(h, &s->k2.eff, (size_t)SVC_MAX_OPS + 8, false));
     TRY(dev_alloc(h, &s->k2.results, (size_t)SVC_MAX_OPS, false));
     TRY(dev_alloc(h, &s->d_dupfix, (size_t)4, true));
+    TRY(dev_alloc(h, &s->d_boff, (size_t)SVC_MAX_OPS + 1, false));
+    TRY(dev_alloc(h, &s->d_bdst, (size_t)SVC_MAX_OPS, false));
+    TRY(dev_alloc(h, &s->d_bhlen, (size_t)SVC_MAX_OPS, false));
     CK(cudaStreamSynchronize(h->stream));
     const uint32_t cpus = cpu_allowance();
     s->spin_cpus = cpus > 6 ? cpus - 6 : 1;             // leave room for the dispatcher, the driver's threads and the nappers' wake-ups
@@ -1125,7 +1154,12 @@ int agr_wait(agr_handle* h, agr_ticket ticket, agr_result* out) {
 }
 
 // ------------------------------------------------------------------------------------------ K2
-static int complete_locked(agr_handle* h, const agr_outcome* outs, uint32_t n, int32_t* results);
+static int complete_locked(agr_handle* h, const agr_outcome* outs, uint32_t n, int32_t* results, const agr_k2_bytes* bytes = nullptr,
+                           bool bytes_dropped = false);
+static int complete_ex_locked(agr_handle* h, const agr_outcome* outs, uint32_t n, const uint8_t* bytes, const uint64_t* offsets,
+                              const uint32_t* hdr_lens, int32_t* results);
+static int svc_complete_ex(agr_handle* h, const agr_outcome* outs, uint32_t n, const uint8_t* bytes, const uint64_t* offsets,
+                           const uint32_t* hdr_lens, int32_t* results);
 
 int agr_complete(agr_handle* h, const agr_outcome* outs, uint32_t n, int32_t* results) {
     if (!h || (n && !outs)) return fail(AGR_EINVAL, "NULL argument");
@@ -1135,7 +1169,23 @@ int agr_complete(agr_handle* h, const agr_outcome* outs, uint32_t n, int32_t* re
     return complete_locked(h, outs, n, results);
 }
 
-static int complete_locked(agr_handle* h, const agr_outcome* outs, uint32_t n, int32_t* results) {
+int agr_complete_ex(agr_handle* h, const agr_outcome* outs, uint32_t n, const uint8_t* bytes, const uint64_t* offsets,
+                    const uint32_t* hdr_lens, int32_t* results) {
+    if (!h || (n && (!outs || !offsets))) return fail(AGR_EINVAL, "NULL argument");
+    if (h->svc && n >= 1 && n <= SVC_MAX_CALL) {
+        bool fits = true;
+        for (uint32_t i = 0; i < n && fits; ++i) fits = offsets[i + 1] >= offsets[i] && offsets[i + 1] - offsets[i] <= AGR_OUT_INLINE_BYTES;
+        if (fits) return svc_complete_ex(h, outs, n, bytes, offsets, hdr_lens, results);
+    }
+    HLock lk(h);
+    CK(cudaSetDevice(h->device));
+    return complete_ex_locked(h, outs, n, bytes, offsets, hdr_lens, results);
+}
+
+// bytes (agr_complete_ex): the batch's bytes are staged on the device and have a region of the byte slab; bytes_dropped: they
+// have none (the transitions are applied all the same, and the call fails with AGR_ENOSPC)
+static int complete_locked(agr_handle* h, const agr_outcome* outs, uint32_t n, int32_t* results, const agr_k2_bytes* bytes,
+                           bool bytes_dropped) {
     if (n > h->cfg.max_batch) return fail(AGR_EINVAL, "n exceeds max_batch");
     if (n == 0) return 0;
     // outcomes go to the device as they are; k2_prepare resolves the agent ids in the device agent table
@@ -1151,8 +1201,8 @@ static int complete_locked(agr_handle* h, const agr_outcome* outs, uint32_t n, i
         for (auto& e : h->op_ev) if (!e) CK(cudaEventCreate(&e));
         CK(cudaEventRecord(h->op_ev[0], h->stream));
     }
-    agr_launch_k2(h->d, h->d_outs, h->k2, n, h->stream);
-    h->k2_launches += 3;
+    agr_launch_k2(h->d, h->d_outs, h->k2, n, h->stream, bytes);
+    h->k2_launches += bytes ? 4 : 3;
     CK(cudaGetLastError());
     if (timing) { CK(cudaEventRecord(h->op_ev[1], h->stream)); h->op_timed[0] = true; }
     CK(cudaMemcpyAsync(h->h_k2flag, h->k2.overflow, 4, cudaMemcpyDeviceToHost, h->stream));
@@ -1164,7 +1214,145 @@ static int complete_locked(agr_handle* h, const agr_outcome* outs, uint32_t n, i
         CK(cudaStreamSynchronize(h->stream));
     }
     // the state transitions were applied; list entries beyond the log capacity were dropped (agr_config.log_entries)
-    if (*h->h_k2flag) return fail(AGR_ENOSPC, "completed / failed log full: entries of this batch were dropped (raise agr_config.log_entries, or agr_reclaim)");
+    const char* log_full = "completed / failed log full: entries of this batch were dropped (raise agr_config.log_entries, or agr_reclaim)";
+    if (bytes_dropped)
+        return fail(AGR_ENOSPC, std::string("response byte slab full: the batch's outcomes were applied, none of its response / error bytes "
+                                            "were stored (raise agr_config.resp_bytes, or agr_reclaim with AGR_CFG_RING)") +
+                                    (*h->h_k2flag ? std::string("; also ") + log_full : std::string()));
+    if (*h->h_k2flag) return fail(AGR_ENOSPC, log_full);
+    return 0;
+}
+
+// ------------------------------------------------------------------------------------------ K2 with bytes (agr_complete_ex)
+// Places need bytes (a multiple of 16) in the response byte slab as one piece; len is the unrounded size the append-only check
+// uses.  With the ring a piece never wraps: the rest of the lap is skipped, and agr_reclaim moves resp_tail.
+static int resp_reserve_locked(agr_handle* h, uint64_t need, uint64_t len, unsigned long long* off) {
+    if (!is_ring(h)) {
+        if (h->resp_used + len > h->resp_cap) return fail(AGR_ENOSPC, "response slab full");
+        *off = h->resp_used;
+        h->resp_used += need;
+        return 0;
+    }
+    if (need > h->resp_cap / 2) return fail(AGR_ENOSPC, "response larger than half the response slab");
+    const uint64_t at = h->resp_used % h->resp_cap;
+    const uint64_t pad = (at + need > h->resp_cap) ? h->resp_cap - at : 0;
+    if (h->resp_used + pad + need - h->resp_tail > h->resp_cap)
+        return fail(AGR_ENOSPC, "response slab full: agr_reclaim releases the bytes of released rows");
+    h->resp_used += pad;
+    *off = h->resp_used % h->resp_cap;                           // the rows keep PHYSICAL offsets
+    h->resp_used += need;
+    return 0;
+}
+
+// Checks what agr_complete_ex got; *total = the size of the batch's region (every segment rounded up to 16 B), *max_len = the
+// longest segment.
+static int check_segments(const agr_outcome* outs, uint32_t n, const uint64_t* offsets, const uint32_t* hdr_lens, uint64_t* total,
+                          uint64_t* max_len) {
+    uint64_t t = 0, m = 0;
+    for (uint32_t i = 0; i < n; ++i) {
+        if (offsets[i + 1] < offsets[i]) return fail(AGR_EINVAL, "offsets must not decrease");
+        const uint64_t len = offsets[i + 1] - offsets[i];
+        if (len > 0xffffffffull) return fail(AGR_EINVAL, "a segment is longer than 4 GiB");
+        if (outs[i].kind == AGR_OUT_RESPONSE) {
+            if (hdr_lens && hdr_lens[i] > len) return fail(AGR_EINVAL, "hdr_lens[i] is longer than segment i");
+        } else if (outs[i].kind != AGR_OUT_ERROR && len) {
+            return fail(AGR_EINVAL, "only AGR_OUT_RESPONSE and AGR_OUT_ERROR outcomes carry bytes");
+        }
+        t += (len + 15u) & ~15ull;
+        m = std::max(m, len);
+    }
+    *total = t; *max_len = m;
+    return 0;
+}
+
+static int complete_ex_locked(agr_handle* h, const agr_outcome* outs, uint32_t n, const uint8_t* bytes, const uint64_t* offsets,
+                              const uint32_t* hdr_lens, int32_t* results) {
+    if (n > h->cfg.max_batch) return fail(AGR_EINVAL, "n exceeds max_batch");
+    if (n == 0) return 0;
+    uint64_t total = 0, max_len = 0;
+    TRY(check_segments(outs, n, offsets, hdr_lens, &total, &max_len));
+    const uint64_t nbytes = offsets[n] - offsets[0];
+    if (nbytes && !bytes) return fail(AGR_EINVAL, "NULL bytes");
+    if (!h->d_boff) {
+        const size_t mb = h->cfg.max_batch;
+        TRY(host_alloc(h, &h->h_boff, mb + 1)); TRY(dev_alloc(h, &h->d_boff, mb + 1, false));
+        TRY(host_alloc(h, &h->h_bdst, mb)); TRY(dev_alloc(h, &h->d_bdst, mb, false));
+        TRY(host_alloc(h, &h->h_bhlen, mb)); TRY(dev_alloc(h, &h->d_bhlen, mb, false));
+    }
+    // the batch's region: all or nothing
+    unsigned long long base = 0;
+    if (resp_reserve_locked(h, total, total, &base) < 0) return complete_locked(h, outs, n, results, nullptr, true);
+    // each segment's place in it, in array order (the host has the offsets: no device round trip)
+    uint64_t run = 0;
+    for (uint32_t i = 0; i < n; ++i) { h->h_bdst[i] = run; run += (offsets[i + 1] - offsets[i] + 15u) & ~15ull; }
+    CK(cudaMemcpyAsync(h->d_bdst, h->h_bdst, (size_t)n * 8, cudaMemcpyHostToDevice, h->stream));
+    const void* offs = offsets;
+    if (!is_pinned(offsets)) { memcpy(h->h_boff, offsets, ((size_t)n + 1) * 8); offs = h->h_boff; }
+    CK(cudaMemcpyAsync(h->d_boff, offs, ((size_t)n + 1) * 8, cudaMemcpyHostToDevice, h->stream));
+    if (hdr_lens) {
+        const uint32_t* hl = hdr_lens;
+        if (!is_pinned(hdr_lens)) { memcpy(h->h_bhlen, hdr_lens, (size_t)n * 4); hl = h->h_bhlen; }
+        CK(cudaMemcpyAsync(h->d_bhlen, hl, (size_t)n * 4, cudaMemcpyHostToDevice, h->stream));
+    }
+    if (nbytes) {
+        // (+ 16: warp_copy16 reads whole aligned 16-byte blocks around a segment)
+        if (nbytes + 16 > h->d_bsrc_cap) { TRY(dev_regrow(h, &h->d_bsrc, (size_t)(nbytes + nbytes / 4 + 16), false)); h->d_bsrc_cap = nbytes + nbytes / 4 + 16; }
+        const uint8_t* src = bytes + offsets[0];
+        if (!is_pinned(src)) {
+            if (nbytes > h->h_bsrc_cap) { TRY(host_regrow(h, &h->h_bsrc, (size_t)(nbytes + nbytes / 4))); h->h_bsrc_cap = nbytes + nbytes / 4; }
+            par_memcpy(h->h_bsrc, src, nbytes);
+            src = h->h_bsrc;
+        }
+        CK(cudaMemcpyAsync(h->d_bsrc, src, nbytes, cudaMemcpyHostToDevice, h->stream));
+    }
+    agr_k2_bytes b{};
+    b.src = h->d_bsrc; b.src_off = h->d_boff; b.dst = h->d_bdst; b.hlen = hdr_lens ? h->d_bhlen : nullptr; b.base = base;
+    b.slab = h->d_resp; b.resp_off = h->d_resp_off; b.resp_len = h->d_resp_len; b.resp_hlen = h->d_resp_hlen;
+    b.err_off = h->d_err_off; b.err_len = h->d_err_len;
+    return complete_locked(h, outs, n, results, &b, false);
+}
+
+// agr_complete_ex through the single-request ring: every outcome goes as SVC_OP_OUTCOME_BYTES with its segment inline
+static int svc_complete_ex(agr_handle* h, const agr_outcome* outs, uint32_t n, const uint8_t* bytes, const uint64_t* offsets,
+                           const uint32_t* hdr_lens, int32_t* results) {
+    uint64_t total = 0, max_len = 0;
+    TRY(check_segments(outs, n, offsets, hdr_lens, &total, &max_len));
+    if (total && !bytes) return fail(AGR_EINVAL, "NULL bytes");
+    svc_host* s = h->svc;
+    uint64_t pos[SVC_MAX_CALL];
+    for (uint32_t i = 0; i < n; ++i) {
+        const uint32_t len = (uint32_t)(offsets[i + 1] - offsets[i]);
+        const uint32_t hl = (hdr_lens && outs[i].kind == AGR_OUT_RESPONSE) ? hdr_lens[i] : 0u;
+        while (!svc_submit_outcome_bytes(s, &outs[i], hl, len ? bytes + offsets[i] : nullptr, len, nullptr, 0u, &pos[i])) {}
+    }
+    int rc = 0;
+    for (uint32_t i = 0; i < n; ++i) {
+        svc_answer r; svc_wait(s, pos[i], &r);
+        int32_t res = (int32_t)r.w0;
+        if (res == AGR_ENOSPC) { res = 0; if (rc == 0) rc = AGR_ENOSPC; }
+        else if (res < 0 && res != AGR_ENOTFOUND) rc = res;
+        if (results) results[i] = res;
+        svc_release(s, pos[i]);
+    }
+    if (rc == AGR_ENOSPC)
+        return fail(rc, "response byte slab full: the outcomes were applied, their response / error bytes were not stored "
+                        "(raise agr_config.resp_bytes, or agr_reclaim with AGR_CFG_RING)");
+    if (rc < 0) return fail(rc, "single-request front end: CUDA error");
+    return 0;
+}
+
+int agr_submit_complete_ex(agr_handle* h, const agr_outcome* outcome, const uint8_t* headers, uint32_t hdr_len,
+                           const uint8_t* body, uint32_t body_len, agr_ticket* ticket) {
+    if (!h || !outcome || !ticket || (hdr_len && !headers) || (body_len && !body)) return fail(AGR_EINVAL, "NULL argument");
+    if (!h->svc) return fail(AGR_EINVAL, "engine was not created with AGR_CFG_COMBINE");
+    if ((uint64_t)hdr_len + body_len > AGR_OUT_INLINE_BYTES)
+        return fail(AGR_EINVAL, "headers + body exceed AGR_OUT_INLINE_BYTES: use agr_complete_ex(n = 1)");
+    if (outcome->kind != AGR_OUT_RESPONSE && outcome->kind != AGR_OUT_ERROR && hdr_len + body_len)
+        return fail(AGR_EINVAL, "only AGR_OUT_RESPONSE and AGR_OUT_ERROR outcomes carry bytes");
+    uint64_t a = 0;
+    if (!svc_submit_outcome_bytes(h->svc, outcome, outcome->kind == AGR_OUT_RESPONSE ? hdr_len : 0u, headers, hdr_len, body, body_len, &a))
+        return AGR_EAGAIN;                                       // collect outstanding tickets (agr_poll) and come again
+    *ticket = a | TICKET_OUTCOME;
     return 0;
 }
 
@@ -1512,20 +1700,7 @@ static int store_bytes_locked(agr_handle* h, const char* agent_id, const uint8_t
     const uint32_t len = alen + blen;
     const uint64_t need = ((uint64_t)len + 15u) & ~15ull;
     unsigned long long off;
-    if (!is_ring(h)) {
-        if (h->resp_used + len > h->resp_cap) return fail(AGR_ENOSPC, "response slab full");
-        off = h->resp_used;
-        h->resp_used += need;
-    } else {                                                     // byte ring: a blob never wraps; agr_reclaim advances resp_tail
-        if (need > h->resp_cap / 2) return fail(AGR_ENOSPC, "response larger than half the response slab");
-        const uint64_t at = h->resp_used % h->resp_cap;
-        const uint64_t pad = (at + need > h->resp_cap) ? h->resp_cap - at : 0;
-        if (h->resp_used + pad + need - h->resp_tail > h->resp_cap)
-            return fail(AGR_ENOSPC, "response slab full: agr_reclaim releases the bytes of released rows");
-        h->resp_used += pad;
-        off = h->resp_used % h->resp_cap;                        // the rows keep PHYSICAL offsets
-        h->resp_used += need;
-    }
+    TRY(resp_reserve_locked(h, need, len, &off));
     if (alen) CK(cudaMemcpyAsync(h->d_resp + off, a, alen, cudaMemcpyHostToDevice, h->stream));
     if (blen) CK(cudaMemcpyAsync(h->d_resp + off + alen, b, blen, cudaMemcpyHostToDevice, h->stream));
     if (which == 0) {

@@ -2,7 +2,7 @@
 //
 //   K1  k1_ingest_v0 (LSU variant; the default TMA kernel is in agr_k1_tma.cu, the variable-length one in
 //       agr_k1_var.cu), k1_index (split mode), k1_post          (requests.go:64-117, server.go:493-557)
-//   K2  k2_prepare / k2_link / k2_apply / k2_offsets / k2_append / k2_tail
+//   K2  k2_link / k2_apply / k2_append; with bytes (agr_complete_ex) k2_apply_bytes and k2_copy_bytes
 //                                                                 (requests.go:120-194,228-275, server.go:583-615)
 //   K3  k3_pass<count|scatter> / k3_scan_groups / k3_scan_total / k3_gather, k_resolve, k_verify, k_drop_*
 //                                                                 (replay_worker.go:58-117, requests.go:197-225)
@@ -514,14 +514,15 @@ void agr_launch_resolve(const agr_dev& d, const agr_dop* ops, uint32_t* hrid, ui
     if (n) k_resolve<<<(n + 255u) / 256u, 256, 0, st>>>(d, ops, hrid, n);
 }
 
-__global__ void __launch_bounds__(256) k2_apply(const agr_dev d, const agr_k2_scratch s, const uint32_t n) {
+template <bool BYTES>
+__device__ __forceinline__ void k2_apply_body(const agr_dev& d, const agr_k2_scratch& s, const uint32_t n, const agr_k2_bytes* b) {
     __shared__ uint32_t s_cnt[3];
     const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
     const int lane = threadIdx.x & 31;
     if (threadIdx.x < 3) s_cnt[threadIdx.x] = 0u;
     __syncthreads();
     uint32_t cnt[3] = {0u, 0u, 0u};                                  // completions, errors, dead-lettered
-    if (j < n) k2_apply_one(d, s, j, cnt);
+    if (j < n) k2_apply_one<BYTES>(d, s, j, cnt, b);
     // one global atomic per CTA and counter: a million outcomes are 32 K warps, and that many adds to one word serialise in L2
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
@@ -534,6 +535,21 @@ __global__ void __launch_bounds__(256) k2_apply(const agr_dev d, const agr_k2_sc
         if (s_cnt[1]) atomicAdd(&d.ctr[C_FAILURES], (unsigned long long)s_cnt[1]);
         if (s_cnt[2]) atomicAdd(&d.ctr[C_DEAD_LETTERED], (unsigned long long)s_cnt[2]);
     }
+}
+__global__ void __launch_bounds__(256) k2_apply(const agr_dev d, const agr_k2_scratch s, const uint32_t n) {
+    k2_apply_body<false>(d, s, n, nullptr);
+}
+__global__ void __launch_bounds__(256) k2_apply_bytes(const agr_dev d, const agr_k2_scratch s, const uint32_t n, const agr_k2_bytes b) {
+    k2_apply_body<true>(d, s, n, &b);
+}
+
+// One warp per op: copies the segments of the ops k2_apply_bytes marked K2_EFF_WIN from the staged batch into their 16-byte
+// aligned places in the byte slab (losers' places stay unused).
+__global__ void __launch_bounds__(256) k2_copy_bytes(const agr_k2_scratch s, const agr_k2_bytes b, const uint32_t n) {
+    const uint32_t j = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31u;
+    if (j >= n || !(s.eff[j] & K2_EFF_WIN)) return;
+    const unsigned long long o = b.src_off[j];
+    warp_copy16(reinterpret_cast<uint4*>(b.slab + b.base + b.dst[j]), b.src + (o - b.src_off[0]), (uint32_t)(b.src_off[j + 1] - o), lane);
 }
 
 // Order-preserving append of the batch's completed / failed pushes.  Tiles of K2_TILE ops are claimed through a ticket (so a
@@ -623,13 +639,15 @@ __global__ void __launch_bounds__(256) k2_append(const agr_dev d, const agr_k2_s
 }
 
 uint32_t agr_k2_tiles(uint32_t n) { return (n + K2_TILE - 1u) / K2_TILE; }
-void agr_launch_k2(const agr_dev& d, const void* outs, const agr_k2_scratch& s, uint32_t n, cudaStream_t st) {
+void agr_launch_k2(const agr_dev& d, const void* outs, const agr_k2_scratch& s, uint32_t n, cudaStream_t st, const agr_k2_bytes* bytes) {
     if (n == 0) return;
     const uint32_t blocks = (n + 255u) / 256u, ntiles = agr_k2_tiles(n);
     cudaMemsetAsync(s.ticket, 0, (size_t)(ntiles + 1u) * 8u, st);   // {ticket, overflow}, then the batch's tile words
     k2_link<<<blocks, 256, 0, st>>>(d, (const uint8_t*)outs, s, n);
-    k2_apply<<<blocks, 256, 0, st>>>(d, s, n);
+    if (bytes) k2_apply_bytes<<<blocks, 256, 0, st>>>(d, s, n, *bytes);
+    else k2_apply<<<blocks, 256, 0, st>>>(d, s, n);
     k2_append<<<ntiles, 256, 0, st>>>(d, s, n);
+    if (bytes) k2_copy_bytes<<<(n + 7u) / 8u, 256, 0, st>>>(s, *bytes, n);
 }
 
 // ------------------------------------------------------------------------------------------------ K3

@@ -87,6 +87,22 @@ struct agr_k2_scratch {
     unsigned long long* tiles; // [tiles] k2_append's look-back words
 };
 
+// agr_complete_ex: the bytes a batch's outcomes carry (StoreResponse's response, MarkRequestFailed's error text).  The chain
+// root of a row writes the stored-response / error words of its last applied RESPONSE / ERROR op and marks that op's eff
+// byte with K2_EFF_WIN; only marked ops' segments are copied into the byte slab.
+#define K2_EFF_WIN 4u
+#define K2_NO_BYTES (~0ULL)   // dst[j] of an op that carries no bytes (a plain outcome in a batch of the service kernel)
+struct agr_k2_bytes {
+    const uint8_t* src;                  // the batch's bytes on the device
+    const unsigned long long* src_off;   // [n + 1] the caller's offsets: segment j = src + (src_off[j] - src_off[0]), src_off[j+1] - src_off[j] bytes
+    const unsigned long long* dst;       // [n] where segment j goes, relative to base (16-byte rounded running sum of the lengths)
+    const uint32_t* hlen;                // [n] leading bytes of a RESPONSE segment that are its flattened headers; nullptr = none
+    unsigned long long base;             // physical offset of the batch's region in the byte slab (a multiple of 16)
+    uint8_t* slab;                       // the byte slab
+    unsigned long long* resp_off; uint32_t* resp_len; uint32_t* resp_hlen;   // per-row words of the stored response
+    unsigned long long* err_off; uint32_t* err_len;                           // and of the stored error text
+};
+
 // K3 select modes
 enum { K3_TICK = 0, K3_AGENT_PENDING = 1, K3_LOG_AGENT = 2, K3_AGENT_PENDING_IDS = 3 /* LRANGE: expired records' ids included */ };
 struct agr_k3_params {
@@ -188,7 +204,8 @@ void agr_launch_k1_post(const agr_dev& d, uint32_t first_rid, uint32_t n, int sm
                         const uint32_t* marks = nullptr);
 int agr_k1_tma_make_map(void* slab, unsigned long long rows, void* out_map /*128 B, 64 B aligned*/);
 uint32_t agr_k2_tiles(uint32_t n);
-void agr_launch_k2(const agr_dev& d, const void* outs /*device agr_outcome[n]*/, const agr_k2_scratch& s, uint32_t n, cudaStream_t st);
+void agr_launch_k2(const agr_dev& d, const void* outs /*device agr_outcome[n]*/, const agr_k2_scratch& s, uint32_t n, cudaStream_t st,
+                   const agr_k2_bytes* bytes = nullptr /* agr_complete_ex: apply with bytes, then copy the winners' segments */);
 void agr_launch_resolve(const agr_dev& d, const agr_dop* ops, uint32_t* hrid, uint32_t n, cudaStream_t st);
 void agr_launch_k3_select(const agr_dev& d, const agr_k3_params& p, int sm_count, cudaStream_t st);
 void agr_launch_k3_gather(const agr_dev& d, const uint32_t* rids, const uint32_t* slots, uint32_t n,

@@ -1,7 +1,7 @@
 // agr_ring.hpp — the CALLERS' side of the single-request ring (AGR_CFG_COMBINE; layout and protocol: agr_svc.h).
 //
 // Everything a calling thread does to hand one operation over and to collect its answer, as templates over the host-side ring
-// object H (agr_engine.cu's svc_host; tests/ring_sim.cpp's stand-in).  H provides:
+// object H (agr_engine.cu's svc_host; the stand-ins of tests/ring_sim.cpp and tests/ring_sim_bytes.cpp).  H provides:
 //   svc_res* res; uint8_t* payload; std::atomic<uint32_t>* ready;          pinned, device-mapped in the engine
 //   std::atomic<uint64_t> head, scanned; std::atomic<uint32_t> waiters; uint32_t spin_cpus;
 //   std::atomic<bool> sleeping; std::mutex smu; std::condition_variable scv;   the dispatcher's sleep / wake-up
@@ -78,6 +78,21 @@ static bool svc_submit_one(H* s, uint32_t kind, const void* item, size_t item_by
     *abs = a;
     return ok;
 }
+// hands over ONE outcome with its bytes (SVC_OP_OUTCOME_BYTES): the 64 B outcome, hdr_len, the segment's length and the segment
+// a | b; only the 16 B-rounded part of the slot that is used is written.  a_len + b_len <= SVC_BYTES_MAX (the caller checks).
+template <class H>
+static bool svc_submit_outcome_bytes(H* s, const void* outcome, uint32_t hdr_len, const uint8_t* a, uint32_t a_len, const uint8_t* b,
+                                     uint32_t b_len, uint64_t* abs) {
+    alignas(16) uint8_t item[SVC_PAYLOAD];
+    const uint32_t len = a_len + b_len, used = (SVC_BYTES_DATA + len + 15u) & ~15u;
+    memcpy(item, outcome, SVC_BYTES_HDR);
+    memcpy(item + SVC_BYTES_HDR, &hdr_len, 4);
+    memcpy(item + SVC_BYTES_HDR + 4, &len, 4);
+    if (a_len) memcpy(item + SVC_BYTES_DATA, a, a_len);
+    if (b_len) memcpy(item + SVC_BYTES_DATA + a_len, b, b_len);
+    memset(item + SVC_BYTES_DATA + len, 0, used - SVC_BYTES_DATA - len);
+    return svc_submit_one(s, SVC_OP_OUTCOME_BYTES, item, used, abs);
+}
 struct svc_answer { uint32_t w0, w1; uint64_t rid; };
 template <class H>
 static inline bool svc_try(H* s, uint64_t a, svc_answer* out) {
@@ -112,17 +127,18 @@ static inline void svc_release(H* s, uint64_t a) {       // everything of the an
 
 // ---- the dispatcher's side of the ready words
 // Grows the contiguous published prefix [taken, *to) by whatever has been published since: at most SVC_MAX_OPS operations and
-// max_records records per batch.  A slot is looked at until it is published and never again (re-reading the callers' ready words
-// every iteration keeps pulling their cache lines away from the cores that write them), and an operation's kind is noted in
-// kinds[] (2 bits each, the batch descriptor's form) AT THAT MOMENT: a no-op slot may be published again, for the next lap, as soon
-// as `scanned` has passed it.  Publishes the new scan position.
+// max_staged records plus outcomes with bytes per batch (*nstaged counts those: each takes a whole 512 B slot of the kernel's
+// stage; the dispatcher tells the two apart by kinds[]).  A slot is looked at until it is published and never again (re-reading
+// the callers' ready words every iteration keeps pulling their cache lines away from the cores that write them), and an
+// operation's kind is noted in kinds[] (2 bits each, the batch descriptor's form) AT THAT MOMENT: a no-op slot may be published
+// again, for the next lap, as soon as `scanned` has passed it.  Publishes the new scan position.
 template <class H>
-static inline void svc_scan(H* s, const uint64_t taken, uint64_t* to, uint32_t* nrec, uint32_t* kinds, const uint32_t max_records) {
+static inline void svc_scan(H* s, const uint64_t taken, uint64_t* to, uint32_t* nstaged, uint32_t* kinds, const uint32_t max_staged) {
     while (*to - taken < SVC_MAX_OPS) {
         const uint32_t slot = (uint32_t)(*to & (SVC_SLOTS - 1u));
         const uint32_t rw = s->ready[slot].load(std::memory_order_acquire);
         if ((rw >> 2) != (uint32_t)(*to / SVC_SLOTS) + 1u) break;
-        if ((rw & 3u) == SVC_OP_RECORD) { if (*nrec == max_records) break; (*nrec)++; }
+        if ((rw & 3u) == SVC_OP_RECORD || (rw & 3u) == SVC_OP_OUTCOME_BYTES) { if (*nstaged == max_staged) break; (*nstaged)++; }
         kinds[(*to - taken) >> 4] |= (rw & 3u) << (((*to - taken) & 15u) * 2u);
         (*to)++;
     }

@@ -55,9 +55,12 @@ extern "C" __global__ void __launch_bounds__(SVC_THREADS, 1)
 k_svc(const agr_dev d0, const svc_dev v, const agr_k2_scratch k2, const unsigned long long first_seq) {
     extern __shared__ __align__(128) uint8_t smem[];
     __shared__ __align__(16) uint32_t s_dw[2][64];           // the accepted descriptors, as words
-    __shared__ uint32_t s_go[2], s_nout[2];
+    __shared__ uint32_t s_go[2], s_nout[2], s_nbyt[2];
+    // s_rec_op: the ops whose whole slot is pulled into the stage — records, then the outcomes with bytes
     __shared__ uint16_t s_rec_op[2][SVC_MAX_RECS], s_out_op[2][SVC_MAX_OPS];
+    __shared__ uint16_t s_out_stage[2][SVC_MAX_OPS];         // outcome -> its stage slot (outcomes with bytes), 0xffff = none
     __shared__ uint32_t s_wc[12], s_wf[12];
+    __shared__ unsigned long long s_wsum[12];
     __shared__ unsigned long long s_logbase[2];
     __shared__ long long s_cyc[2];                           // loader's clock64 accounting: waiting for a batch, pulling payloads
     const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
@@ -103,25 +106,33 @@ k_svc(const agr_dev d0, const svc_dev v, const agr_k2_scratch k2, const unsigned
                     }
                 }
                 __syncwarp();
-                uint32_t nout = 0;
+                uint32_t nout = 0, nbyt = 0;
                 if (go == 1u) {
-                    // op -> (record i | outcome j) maps: thirty-two ops per step, running offsets
+                    // op -> (record i | outcome j, and stage slot of an outcome with bytes) maps: thirty-two ops per step, running offsets
                     const svc_desc& D = *reinterpret_cast<const svc_desc*>(s_dw[st]);
-                    uint32_t br = 0, bo = 0;
+                    uint32_t br = 0, bo = 0, bb = 0;
                     const uint32_t lt = (1u << lane) - 1u;
                     for (uint32_t base = 0; base < D.count; base += 32u) {
                         const uint32_t op = base + lane;
                         const uint32_t kind = (op < D.count) ? ((D.kinds[op >> 4] >> ((op & 15u) * 2u)) & 3u) : 0u;
-                        const uint32_t mr = __ballot_sync(FULL, kind == SVC_OP_RECORD), mo = __ballot_sync(FULL, kind == SVC_OP_OUTCOME);
+                        const bool is_out = kind == SVC_OP_OUTCOME || kind == SVC_OP_OUTCOME_BYTES;
+                        const uint32_t mr = __ballot_sync(FULL, kind == SVC_OP_RECORD), mo = __ballot_sync(FULL, is_out);
+                        const uint32_t mb = __ballot_sync(FULL, kind == SVC_OP_OUTCOME_BYTES);
                         if (kind == SVC_OP_RECORD) s_rec_op[st][br + __popc(mr & lt)] = (uint16_t)op;
-                        if (kind == SVC_OP_OUTCOME) s_out_op[st][bo + __popc(mo & lt)] = (uint16_t)op;
-                        br += __popc(mr); bo += __popc(mo);
+                        if (is_out) {
+                            const uint32_t oi = bo + __popc(mo & lt);
+                            uint16_t sp = 0xffffu;
+                            if (kind == SVC_OP_OUTCOME_BYTES) { sp = (uint16_t)(D.n_records + bb + __popc(mb & lt)); s_rec_op[st][sp] = (uint16_t)op; }
+                            s_out_op[st][oi] = (uint16_t)op;
+                            s_out_stage[st][oi] = sp;
+                        }
+                        br += __popc(mr); bo += __popc(mo); bb += __popc(mb);
                     }
-                    nout = bo;
+                    nout = bo; nbyt = bb;
                     last_work = globaltimer_ns();
                 }
                 if (lane == 0) {
-                    s_go[st] = go; s_nout[st] = nout;
+                    s_go[st] = go; s_nout[st] = nout; s_nbyt[st] = nbyt;
                     if (go != 1u) v.ctl->heartbeat = polls;
                     const long long c = clock64(); c_wait += c - c0; c0 = c;
                 }
@@ -131,7 +142,7 @@ k_svc(const agr_dev d0, const svc_dev v, const agr_k2_scratch k2, const unsigned
             if (go == 1u) {
                 // pull the payloads out of host memory: eight 16-byte loads in flight per thread
                 const svc_desc& D = *reinterpret_cast<const svc_desc*>(s_dw[st]);
-                const uint32_t rec_chunks = D.n_records * 32u, total = rec_chunks + s_nout[st] * 4u;
+                const uint32_t rec_chunks = (D.n_records + s_nbyt[st]) * 32u, total = rec_chunks + s_nout[st] * 4u;
                 const unsigned long long from = D.from;
                 for (uint32_t cb = tid; cb < total; cb += SVC_LOADERS * 8u) {
                     uint4 val[8];
@@ -240,14 +251,44 @@ k_svc(const agr_dev d0, const svc_dev v, const agr_k2_scratch k2, const unsigned
 
         // ------------------------------------------------------------------ outcomes: link, apply, ordered append
         if (nout) {                                                               // nout is uniform over the workers
+            const uint32_t nbyt = s_nbyt[st];
+            const bool bytes_in = nbyt != 0u && D.resp_base != SVC_NO_BYTES;     // outcomes with bytes, and room for them
             if (wt < nout) {
                 const uint8_t* o = s_out + (size_t)wt * 64u;
                 k2_link_one(d, k2, wt, lds_v4(o), lds_v4(o + 16), lds_v4(o + 32), lds_v4(o + 48));
             }
+            agr_k2_bytes b{};
+            if (bytes_in) {
+                // the segments' places: a block prefix sum of their 16 B-rounded lengths in ring order (the dispatcher reserved the
+                // same total), carried together with the plain lengths in one 64-bit word
+                uint32_t len = 0u, hl = 0u, sp = 0xffffu;
+                if (wt < nout && (sp = s_out_stage[st][wt]) != 0xffffu) {
+                    const uint8_t* p = s_rec + (size_t)sp * 512u;
+                    len = min(*reinterpret_cast<const uint32_t*>(p + SVC_BYTES_HDR + 4), SVC_BYTES_MAX);
+                    hl = min(*reinterpret_cast<const uint32_t*>(p + SVC_BYTES_HDR), len);
+                }
+                const unsigned long long x = ((unsigned long long)((len + 15u) & ~15u) << 32) | len;
+                unsigned long long incl = x;
+#pragma unroll
+                for (int o = 1; o < 32; o <<= 1) { const unsigned long long y = __shfl_up_sync(FULL, incl, o); if ((int)lane >= o) incl += y; }
+                if (lane == 31u) s_wsum[wwarp] = incl;
+                bar_sync(BAR_WORK, SVC_WORKERS);
+                unsigned long long pre = 0, tot = 0;
+#pragma unroll
+                for (int w = 0; w < (int)(SVC_WORKERS / 32u); ++w) { if ((uint32_t)w < wwarp) pre += s_wsum[w]; tot += s_wsum[w]; }
+                const unsigned long long ex = pre + incl - x;
+                if (wt < nout) { v.b_off[wt] = ex & 0xffffffffULL; v.b_dst[wt] = (sp != 0xffffu) ? (ex >> 32) : K2_NO_BYTES; v.b_hlen[wt] = hl; }
+                if (wt == 0) v.b_off[nout] = tot & 0xffffffffULL;
+                b.src_off = v.b_off; b.dst = v.b_dst; b.hlen = v.b_hlen; b.base = D.resp_base; b.slab = v.resp;
+                b.resp_off = v.resp_off; b.resp_len = v.resp_len; b.resp_hlen = v.resp_hlen; b.err_off = v.err_off; b.err_len = v.err_len;
+            }
             __threadfence_block();
             bar_sync(BAR_WORK, SVC_WORKERS);
             uint32_t cnt[3] = {0u, 0u, 0u};
-            if (wt < nout) k2_apply_one(d, k2, wt, cnt);
+            if (wt < nout) {
+                if (bytes_in) k2_apply_one<true>(d, k2, wt, cnt, &b);
+                else k2_apply_one(d, k2, wt, cnt);
+            }
 #pragma unroll
             for (int k = 0; k < 3; ++k) cnt[k] = __reduce_add_sync(FULL, cnt[k]);
             if (lane == 0) {
@@ -279,10 +320,22 @@ k_svc(const agr_dev d0, const svc_dev v, const agr_k2_scratch k2, const unsigned
                 }
                 d.log_len[0] = nc; d.log_len[1] = nf;
             }
-            // the outcomes' result codes (the records' verdicts went out as soon as they were final)
+            // the winners' segments, from the stage into their places (warp per segment)
+            if (bytes_in) {
+                for (uint32_t i = wwarp; i < nout; i += SVC_WORKERS / 32u) {
+                    if (!(__ldcg(&k2.eff[i]) & K2_EFF_WIN)) continue;
+                    const unsigned long long o = __ldcg(&v.b_off[i]);
+                    warp_copy16(reinterpret_cast<uint4*>(v.resp + D.resp_base + __ldcg(&v.b_dst[i])),
+                                s_rec + (size_t)s_out_stage[st][i] * 512u + SVC_BYTES_DATA, (uint32_t)(__ldcg(&v.b_off[i + 1]) - o), lane);
+                }
+            }
+            // the outcomes' result codes (the records' verdicts went out as soon as they were final); an outcome whose bytes found
+            // no room was applied all the same and says so with AGR_ENOSPC
             if (wt < nout) {
                 const unsigned long long slot_abs = from + s_out_op[st][wt];
-                st_res(v.res + (slot_abs & (SVC_SLOTS - 1u)), (uint32_t)k2.results[wt], 0u, 0u, svc_tag(slot_abs) << 16);
+                int32_t res = k2.results[wt];
+                if (res == 0 && nbyt && !bytes_in && s_out_stage[st][wt] != 0xffffu) res = AGR_ENOSPC;
+                st_res(v.res + (slot_abs & (SVC_SLOTS - 1u)), (uint32_t)res, 0u, 0u, svc_tag(slot_abs) << 16);
             }
         }
         bar_sync(BAR_WORK, SVC_WORKERS);                                         // everything of the stage has been read

@@ -23,8 +23,14 @@
 #define SVC_MAX_CALL 32u          // records / outcomes per call that go through the ring
 #define SVC_DESCS 64u             // descriptor ring entries
 #define SVC_PAYLOAD 512u          // bytes per slot: an agr_record, or an agr_outcome in the first 64 B
+// SVC_OP_OUTCOME_BYTES (agr_submit_complete_ex, agr_complete_ex): the 64 B outcome, then u32 hdr_len, u32 len, then the len
+// bytes of its segment (response headers + body, or the error text); the caller writes only the 16 B-rounded part it uses
+#define SVC_BYTES_HDR 64u         // offset of hdr_len (len follows)
+#define SVC_BYTES_DATA 72u        // offset of the segment
+#define SVC_BYTES_MAX (SVC_PAYLOAD - SVC_BYTES_DATA)   // 440 = AGR_OUT_INLINE_BYTES
+#define SVC_NO_BYTES (~0ULL)      // svc_desc.resp_base when the batch's bytes found no room in the response byte slab
 
-enum { SVC_OP_SKIP = 0, SVC_OP_RECORD = 1, SVC_OP_OUTCOME = 2 };
+enum { SVC_OP_SKIP = 0, SVC_OP_RECORD = 1, SVC_OP_OUTCOME = 2, SVC_OP_OUTCOME_BYTES = 3 };
 
 // batch descriptor (256 B = 64 words), written by the dispatcher (host), polled by the kernel: sixteen lanes read 16 B each
 // in ONE poll; the kernel accepts it when the batch number matches and the check word agrees with the other 62 words (a poll
@@ -39,7 +45,9 @@ struct __attribute__((aligned(64))) svc_desc {
     uint32_t tail_phys;                   // live window of the slab after this batch's rows were reserved
     uint64_t tail, head_l;
     uint64_t idx_base;
-    uint64_t reserved[15];
+    uint64_t resp_base;                   // SVC_OP_OUTCOME_BYTES ops: physical offset of the batch's region of the response byte
+                                          // slab (their 16 B-rounded segments in ring order), or SVC_NO_BYTES
+    uint64_t reserved[14];
     uint64_t check;                       // words 60..61: XOR of svc_mix_word over words 0..59 and 62..63
     uint64_t seq;                         // words 62..63: batch number; the kernel waits for desc[seq % SVC_DESCS].seq == seq
 };
@@ -81,4 +89,10 @@ struct svc_dev {                          // device-visible addresses of the pin
     svc_ctl* ctl;
     uint32_t* dupfix;                     // device word for in-batch duplicate ids (hash-id mode)
     unsigned long long idle_ns;           // safety: leave after this long without a batch even if nobody said stop
+    // SVC_OP_OUTCOME_BYTES: the response byte slab and its per-row words, and per-outcome scratch [SVC_MAX_OPS (+ 1)]
+    uint8_t* resp;
+    unsigned long long *resp_off, *err_off;
+    uint32_t *resp_len, *resp_hlen, *err_len;
+    unsigned long long *b_off, *b_dst;    // running sums of the segments' lengths / of their 16 B-rounded lengths
+    uint32_t* b_hlen;
 };

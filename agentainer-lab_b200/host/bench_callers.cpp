@@ -6,7 +6,11 @@
 // With <inflight> > 0 every thread keeps that many requests in flight through the ticket calls (agr_submit_ingest ->
 // agr_poll -> agr_submit_complete -> agr_poll): the goroutine-per-request pattern of a Go host, where a request parks instead
 // of pinning an OS thread (INTEGRATION.md).  Every request is still handed over one at a time.
-//   bench_callers <threads> <seconds> [device] [mint|hash] [agents] [inflight per thread, 0 = blocking calls]
+// With <bytes> = store | fused every StoreResponse keeps a response of 64 B of flattened headers plus <body> bytes of body
+// (requests.go:134-175): store = today's pattern, the completion (blocking call or ticket) and then agr_store_response;
+// fused = the bytes travel with the completion, agr_submit_complete_ex (tickets) or agr_complete_ex(n = 1) (blocking), and a
+// body above AGR_OUT_INLINE_BYTES falls back to the locked agr_complete_ex(n = 1).
+//   bench_callers <threads> <seconds> [device] [mint|hash] [agents] [inflight per thread, 0 = blocking calls] [none|store|fused] [body]
 #include <atomic>
 #include <chrono>
 #include <cstdio>
@@ -32,10 +36,21 @@ int main(int argc, char** argv) {
     const bool mint = !(argc > 4 && strcmp(argv[4], "hash") == 0);
     const int n_agents = argc > 5 ? atoi(argv[5]) : 256;
     const int inflight = argc > 6 ? atoi(argv[6]) : 0;
+    const int bytes_mode = argc > 7 ? (strcmp(argv[7], "store") == 0 ? 1 : strcmp(argv[7], "fused") == 0 ? 2 : 0) : 0;
+    const uint32_t body_len = argc > 8 ? (uint32_t)atoi(argv[8]) : 256u;
+    static constexpr char kHdr[] = "Content-Type: application/json\nX-Trace-Id: 0123456789abcdef0123\n";
+    static_assert(sizeof kHdr - 1 == 64, "64 B of headers");
+    const std::string hdr = kHdr;
+    const std::vector<uint8_t> body(body_len, (uint8_t)'x');
+    std::string seg = hdr; seg.append(body.begin(), body.end());
+    const uint64_t seg_off[2] = {0, seg.size()};
+    const uint32_t seg_hlen = (uint32_t)hdr.size();
+    const bool inline_fits = seg.size() <= AGR_OUT_INLINE_BYTES;
     agr_config cfg; memset(&cfg, 0, sizeof cfg);
     cfg.device = device;
     cfg.slab_rows = 1ull << 26;                         // 64 Mi rows = 32 GiB of slab (~43 GB with the per-row arrays)
-    cfg.max_agents = 1024; cfg.max_batch = 1u << 16; cfg.log_entries = cfg.slab_rows; cfg.resp_bytes = 1 << 20;
+    cfg.max_agents = 1024; cfg.max_batch = 1u << 16; cfg.log_entries = cfg.slab_rows;
+    cfg.resp_bytes = bytes_mode ? 8ull << 30 : 1 << 20;               // append-only: room for a few seconds of stored responses
     cfg.flags = AGR_CFG_PERSISTENCE | AGR_CFG_COMBINE | (mint ? AGR_CFG_MINT_IDS : 0u);
     agr_handle* h = nullptr;
     if (agr_create(&cfg, &h) < 0) { fprintf(stderr, "agr_create: %s\n", agr_last_error()); return 2; }
@@ -61,7 +76,7 @@ int main(int argc, char** argv) {
         if (inflight > 0) {
             // Tickets are answered in hand-over order (batch by batch), so the thread keeps its requests in a FIFO and polls only
             // the OLDEST one: a poll that says "not yet" means nothing younger is ready either.
-            struct flight { int stage; agr_ticket t; std::chrono::steady_clock::time_point t0; uint32_t rec; };
+            struct flight { int stage; agr_ticket t; std::chrono::steady_clock::time_point t0; uint32_t rec; uint8_t rid[16]; };
             std::vector<flight> q((size_t)inflight);
             size_t head = 0, count = 0;                                   // FIFO over q: [head, head + count)
             auto push = [&](const flight& f) { q[(head + count) % q.size()] = f; count++; };
@@ -90,14 +105,26 @@ int main(int argc, char** argv) {
                         agr_outcome o; memset(&o, 0, sizeof o);
                         memcpy(o.request_id, res.request_id, 16); memcpy(o.agent_id, recs[f.rec].agent_id, AGR_AGENT_ID_BYTES);
                         o.kind = AGR_OUT_RESPONSE; o.http_status = 200; o.seq = n;
+                        if (bytes_mode == 2 && !inline_fits) {                // too big for a ticket: the locked batch call, n = 1
+                            int32_t r1 = -1;
+                            if (agr_complete_ex(h, &o, 1, (const uint8_t*)seg.data(), seg_off, &seg_hlen, &r1) < 0 || r1 != 0) { bad++; stop.store(true); break; }
+                            const auto t1 = std::chrono::steady_clock::now();
+                            if (my.size() < my.capacity()) my.push_back((uint32_t)std::chrono::duration_cast<std::chrono::nanoseconds>(t1 - f.t0).count());
+                            continue;
+                        }
                         int rc2;
                         // AGR_EAGAIN: the slot drawn still holds somebody's uncollected answer; the next draw is another slot
-                        while ((rc2 = agr_submit_complete(h, &o, &f.t)) == AGR_EAGAIN && !stop.load(std::memory_order_relaxed)) {}
+                        while ((rc2 = (bytes_mode == 2 ? agr_submit_complete_ex(h, &o, (const uint8_t*)hdr.data(), seg_hlen, body.data(), body_len, &f.t)
+                                                       : agr_submit_complete(h, &o, &f.t))) == AGR_EAGAIN && !stop.load(std::memory_order_relaxed)) {}
                         if (rc2 == AGR_EAGAIN) break;                      // the run is over: this request stays forwarded-but-uncompleted
                         if (rc2 < 0) { bad++; stop.store(true); break; }
                         f.stage = 1;
+                        memcpy(&f.rid, o.request_id, 16);
                         push(f);
                     } else {
+                        if (bytes_mode == 1 && agr_store_response(h, recs[f.rec].agent_id, f.rid, (const uint8_t*)hdr.data(), seg_hlen, body.data(), body_len) < 0) {
+                            bad++; stop.store(true); break;
+                        }
                         const auto t1 = std::chrono::steady_clock::now();
                         if (my.size() < my.capacity()) my.push_back((uint32_t)std::chrono::duration_cast<std::chrono::nanoseconds>(t1 - f.t0).count());
                     }
@@ -118,7 +145,12 @@ int main(int argc, char** argv) {
             memcpy(o.request_id, id[0], 16); memcpy(o.agent_id, r.agent_id, AGR_AGENT_ID_BYTES);
             o.kind = AGR_OUT_RESPONSE; o.http_status = 200; o.seq = n + 1;
             int32_t res = -1;
-            if (agr_complete(h, &o, 1, &res) < 0 || res != 0) { bad++; break; }
+            if (bytes_mode == 2) {
+                if (agr_complete_ex(h, &o, 1, (const uint8_t*)seg.data(), seg_off, &seg_hlen, &res) < 0 || res != 0) { bad++; break; }
+            } else {
+                if (agr_complete(h, &o, 1, &res) < 0 || res != 0) { bad++; break; }
+                if (bytes_mode == 1 && agr_store_response(h, r.agent_id, id[0], (const uint8_t*)hdr.data(), seg_hlen, body.data(), body_len) < 0) { bad++; break; }
+            }
             const auto t1 = std::chrono::steady_clock::now();
             if (my.size() < my.capacity()) my.push_back((uint32_t)std::chrono::duration_cast<std::chrono::nanoseconds>(t1 - t0).count());
             n++;
@@ -146,10 +178,11 @@ int main(int argc, char** argv) {
     agr_stats s2; agr_stats_get(h, &s2);
     printf("{\"threads\": %d, \"seconds\": %.3f, \"round_trips\": %.0f, \"round_trips_per_s\": %.1f, \"ops_per_s\": %.1f, "
            "\"p50_us\": %.2f, \"p99_us\": %.2f, \"latency_samples\": %zu, \"svc_batches\": %llu, \"ops_per_batch\": %.1f, "
-           "\"id_mode\": \"%s\", \"agents\": %d, \"inflight_per_thread\": %d, \"errors\": %llu, \"stored\": %llu, \"completions\": %llu, \"host_cpus\": %u}\n",
+           "\"id_mode\": \"%s\", \"agents\": %d, \"inflight_per_thread\": %d, \"response_bytes\": \"%s\", \"hdr_bytes\": %u, \"body_bytes\": %u, \"errors\": %llu, \"stored\": %llu, \"completions\": %llu, \"host_cpus\": %u}\n",
            threads, secs, rt, rt / secs, 2.0 * rt / secs, pct(0.50), pct(0.99), all.size(),
            (unsigned long long)(s1.svc_batches - s0.svc_batches), (double)(s1.svc_ops - s0.svc_ops) / std::max<double>(1.0, (double)(s1.svc_batches - s0.svc_batches)),
-           mint ? "mint" : "hash", n_agents, inflight, (unsigned long long)bad.load(), (unsigned long long)s2.stored, (unsigned long long)s2.completions,
+           mint ? "mint" : "hash", n_agents, inflight, bytes_mode == 0 ? "none" : bytes_mode == 1 ? "store" : "fused",
+           bytes_mode ? seg_hlen : 0u, bytes_mode ? body_len : 0u, (unsigned long long)bad.load(), (unsigned long long)s2.stored, (unsigned long long)s2.completions,
            std::thread::hardware_concurrency());
     agr_destroy(h);
     return bad.load() ? 1 : 0;

@@ -158,23 +158,30 @@ static std::string flatten(const std::map<std::string, std::string>& h) {      /
     for (const auto& kv : h) out += kv.first + ": " + kv.second + "\n";
     return out;
 }
-Error Manager::StoreResponse(const std::string& agentID, const std::string& requestID, const Response& resp) {
-    Error e = complete(agentID, requestID, AGR_OUT_RESPONSE, resp.StatusCode);
-    if (!e.empty()) return e;
-    if (resp.Headers.empty() && resp.Body.empty()) return "";               // nothing besides the status code to keep
-    uint8_t id[16]; ParseUUID(requestID, id);
-    const std::string hdr = flatten(resp.Headers);                          // requests.go:134-147
-    if (agr_store_response(h_, agentID.c_str(), id, (const uint8_t*)hdr.data(), (uint32_t)hdr.size(), resp.Body.data(), (uint32_t)resp.Body.size()) < 0)
-        return std::string("failed to update request: ") + agr_last_error();
+Error Manager::complete_ex(const std::string& agentID, const std::string& requestID, uint8_t kind, int http, const std::string& seg,
+                           uint32_t hdr_len) {
+    agr_outcome o; memset(&o, 0, sizeof o);
+    if (!ParseUUID(requestID, o.request_id)) return "failed to get request: malformed id";
+    strncpy(o.agent_id, agentID.c_str(), AGR_AGENT_ID_BYTES - 1);
+    o.kind = kind; o.http_status = (uint16_t)http; o.seq = now();
+    const uint64_t offs[2] = {0, seg.size()};
+    int32_t res = 0;
+    // one call: the transition and the bytes (through the single-request ring when they fit a ticket)
+    const int rc = agr_complete_ex(h_, &o, 1, (const uint8_t*)seg.data(), offs, &hdr_len, &res);
+    if (rc < 0 && rc != AGR_ENOSPC) return std::string("failed to update request: ") + agr_last_error();
+    if (res == AGR_ENOTFOUND) return "failed to get request: redis: nil";                  // requests.go:153-156,232-235
+    if (rc == AGR_ENOSPC) return std::string("failed to update request: ") + agr_last_error();
     return "";
 }
+Error Manager::StoreResponse(const std::string& agentID, const std::string& requestID, const Response& resp) {
+    if (resp.Headers.empty() && resp.Body.empty()) return complete(agentID, requestID, AGR_OUT_RESPONSE, resp.StatusCode);   // only the status to keep
+    std::string seg = flatten(resp.Headers);                                // requests.go:134-147
+    const uint32_t hdr_len = (uint32_t)seg.size();
+    seg.append(resp.Body.begin(), resp.Body.end());
+    return complete_ex(agentID, requestID, AGR_OUT_RESPONSE, resp.StatusCode, seg, hdr_len);
+}
 Error Manager::MarkRequestFailed(const std::string& agentID, const std::string& requestID, const std::string& err) {
-    Error e = complete(agentID, requestID, AGR_OUT_ERROR, 0);
-    if (!e.empty()) return e;
-    uint8_t id[16]; ParseUUID(requestID, id);
-    if (agr_store_error_text(h_, agentID.c_str(), id, err.data(), (uint32_t)err.size()) < 0)   // request.Error = err.Error(), requests.go:244
-        return std::string("failed to update request: ") + agr_last_error();
-    return "";
+    return complete_ex(agentID, requestID, AGR_OUT_ERROR, 0, err, 0);       // request.Error = err.Error(), requests.go:244
 }
 Error Manager::GetRequestJSON(const std::string& agentID, const std::string& requestID, std::string* out) {
     uint8_t id[16];

@@ -94,6 +94,9 @@ class Manager {
 
   private:
     Error complete(const std::string& agentID, const std::string& requestID, uint8_t kind, int http);
+    // the same with the bytes the record keeps (agr_complete_ex): seg = flattened headers (hdr_len bytes) + body, or the error text
+    Error complete_ex(const std::string& agentID, const std::string& requestID, uint8_t kind, int http, const std::string& seg,
+                      uint32_t hdr_len);
     agr_handle* h_;
     bool mint_;
     std::atomic<uint64_t> seq_{0};

@@ -217,6 +217,27 @@ typedef struct agr_outcome {
  * (t.requestID == "", server.go:588,597). */
 int agr_complete(agr_handle* h, const agr_outcome* outs, uint32_t n, int32_t* results);
 
+/* agr_complete with the bytes StoreResponse / MarkRequestFailed keep (requests.go:134-175,244), in the same call.  Segment i =
+ * bytes[offsets[i] .. offsets[i+1]) (offsets[0..n], non-decreasing; bytes and offsets may be pageable or pinned):
+ *   AGR_OUT_RESPONSE  its first hdr_lens[i] bytes are the flattened "Key: Value\n" headers, the rest the body (hdr_lens
+ *                     nullable = no headers; read only for responses)
+ *   AGR_OUT_ERROR     the segment is Request.Error
+ *   any other kind    the segment must be empty (AGR_EINVAL)
+ * The result equals, outcome by outcome in array order, agr_complete(&outs[i], 1, &r) followed, when r == 0, by
+ * agr_store_response(headers, body) for a response or agr_store_error_text(segment) for an error: of several outcomes of one
+ * record in a batch the last response's bytes and the last error's text are the ones kept; an empty response segment clears
+ * the stored response; misses, dial errors and all-zero request ids store nothing.
+ * Space is all or nothing: the batch takes ONE region of the response byte slab (every segment rounded up to 16 B; with
+ * AGR_CFG_RING it does not wrap).  If it does not fit, the transitions are applied and results filled all the same, no byte of
+ * the batch is stored, and the call returns AGR_ENOSPC ("response byte slab full", told apart from a full completed / failed
+ * log by agr_last_error).  Segments that lose to a later one of the same record keep their place unused: agr_reclaim gives it
+ * back with AGR_CFG_RING; in an append-only slab it is lost.
+ * With AGR_CFG_COMBINE, n <= 32 and every segment <= AGR_OUT_INLINE_BYTES, the call goes through the single-request ring like
+ * agr_complete does; otherwise it is one locked batch. */
+int agr_complete_ex(agr_handle* h, const agr_outcome* outs, uint32_t n, const uint8_t* bytes, const uint64_t* offsets,
+                    const uint32_t* hdr_lens, int32_t* results);
+#define AGR_OUT_INLINE_BYTES 440u   /* largest segment a ticket carries: 512 B ring slot - 64 B outcome - 8 B lengths */
+
 /* ------------------------------------------------- single requests without a blocked thread (AGR_CFG_COMBINE) */
 /* The reference handles every HTTP request on its own goroutine (server.go:493); goroutines are not OS threads, and a cgo call
  * that blocks until the verdict is back would pin one OS thread per in-flight request.  These calls are the same single-request
@@ -239,6 +260,12 @@ typedef struct agr_result {
 } agr_result;                  /* 40 B */
 int agr_submit_ingest(agr_handle* h, const agr_record* rec, agr_ticket* ticket);
 int agr_submit_complete(agr_handle* h, const agr_outcome* outcome, agr_ticket* ticket);
+/* agr_submit_complete with the outcome's bytes in the ticket (agr_complete_ex(n = 1) semantics): headers then body for a
+ * response, the error text in body for an error (hdr_len 0).  hdr_len + body_len <= AGR_OUT_INLINE_BYTES, else AGR_EINVAL:
+ * the caller then uses agr_complete_ex(n = 1).  The ticket's result is AGR_ENOSPC when the transition was applied but the
+ * bytes found no room in the response byte slab. */
+int agr_submit_complete_ex(agr_handle* h, const agr_outcome* outcome, const uint8_t* headers, uint32_t hdr_len,
+                           const uint8_t* body, uint32_t body_len, agr_ticket* ticket);
 int agr_poll(agr_handle* h, agr_ticket ticket, agr_result* out);
 int agr_wait(agr_handle* h, agr_ticket ticket, agr_result* out);
 uint32_t agr_ring_capacity(void);
