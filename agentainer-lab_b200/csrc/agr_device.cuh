@@ -104,7 +104,10 @@ struct k1_ctx {
     uint32_t slot, astatus;
     bool replay, want_store, cas_issued, deferred, bad, hole;
     uint32_t known;            // replay-flagged + tracked: 0 n/a, 1 target row's words are in o_route / o_state, 2 resolve in the post pass,
-    uint32_t o_route, o_state; //                           3 the id names no live row (cannot be a dedupe hit)
+    uint32_t o_route, o_state; //                           3 cannot be a dedupe hit (no live row, or not an earlier one),
+                               //                           4 earlier row of the same batch: its header words are in t_*
+    uint4 t_agent0, t_agent1, r_agent0, r_agent1;   // known == 4: the target's agent id and this row's
+    uint32_t t_flags, t_lens, t_body;               //             the target's flags, path_len | hdr_len << 16, body_len
 };
 
 __device__ __forceinline__ ag_probe agent_probe_load(const agr_dev& d, uint32_t idx) {
@@ -130,13 +133,19 @@ __device__ __forceinline__ void agent_resolve(const agr_dev& d, ag_probe p, cons
 
 // body_len = the record's body_len field, payload_cap = the payload bytes the record form can hold (416 for the fixed
 // stride, stored length - 96 for a variable-length record): a record whose lengths do not fit is never persisted.
-// first_log: arrival number of the batch's first row, or 0.  With engine-minted ids the row a replay-flagged request names is a
-// pure function of the id; if it arrived BEFORE this batch its words are final, so the dedupe hit (AGR_VF_KNOWN) is decided
-// right here (two 4-byte loads in flight behind the tile's checksum) and only requests naming a row of the SAME batch — or, with
-// first_log == 0 / caller-supplied ids, every tracked replay — are left to the post pass.
+// decide (fixed-stride batch kernels only): first_log is the arrival number of the batch's first row and my_log this row's.  With
+// engine-minted ids the row a replay-flagged request names is a pure function of the id, so the dedupe hit (AGR_VF_KNOWN) is
+// decided here and nothing is left to the post pass:
+//   - a target that arrived BEFORE this batch: its route and state words are final (two 4-byte loads);
+//   - an earlier target of the SAME batch: it is stored, with this row's slot, exactly when its agent id equals this row's (slots
+//     are never reused, so equal slots mean equal ids), persistence is on and it is neither replay-flagged, a hole, nor too long
+//     for its row.  Its header bytes 32..83 are loaded instead of its words, which this launch may not have written yet;
+//   - any other row (this one, a later one) is not a dedupe hit.
+// The loads are issued here and consumed by k1_finish, one tile later.  Without `decide`, or with caller-supplied ids, every
+// tracked replay is left to the post pass.
 __device__ __forceinline__ void k1_begin(const agr_dev& d, const ag_probe& ap, const uint4& h0, const uint4& h1, const uint4& h2, const uint4& h3,
-                                         const uint4& h4, const uint32_t body_len, const uint32_t payload_cap, const unsigned long long first_log,
-                                         k1_ctx& c) {
+                                         const uint4& h4, const uint32_t body_len, const uint32_t payload_cap, const bool decide,
+                                         const unsigned long long first_log, const unsigned long long my_log, k1_ctx& c) {
     c.id_lo = pack64(h0.x, h0.y); c.id_hi = pack64(h0.z, h0.w);
     c.replay = (h4.z & AGR_F_REPLAY) != 0;                                                // server.go:506
     c.hole = (d.cfg_flags & AGR_CFGI_HOLES) && (h4.z & AGR_FI_HOLE);                       // row emptied by the exchange (K4)
@@ -153,10 +162,20 @@ __device__ __forceinline__ void k1_begin(const agr_dev& d, const ag_probe& ap, c
     c.known = 0u; c.o_route = 0u; c.o_state = 0u;
     if (c.replay && found && (h1.x | h1.y | h1.z | h1.w) != 0u) {
         c.known = 2u;
-        if ((d.cfg_flags & AGR_CFG_MINT_IDS) && first_log) {
+        if ((d.cfg_flags & AGR_CFG_MINT_IDS) && decide) {
             const uint32_t orid = lookup_rid(d, pack64(h1.x, h1.y), pack64(h1.z, h1.w));
-            if (orid == AGR_RID_NONE) c.known = 3u;
-            else if (row_logical(d, orid) < first_log) { c.o_route = __ldcg(&d.route[orid]); c.o_state = __ldcg(&d.state[orid]); c.known = 1u; }
+            const unsigned long long olog = orid == AGR_RID_NONE ? ~0ULL : row_logical(d, orid);
+            if (olog < first_log) { c.o_route = __ldcg(&d.route[orid]); c.o_state = __ldcg(&d.state[orid]); c.known = 1u; }
+            else if (olog < my_log) {
+                const uint8_t* t = rec_ptr(d, orid);
+                c.t_agent0 = __ldcg(reinterpret_cast<const uint4*>(t + AGR_OFF_AGENT_ID));
+                c.t_agent1 = __ldcg(reinterpret_cast<const uint4*>(t + AGR_OFF_AGENT_ID + 16));
+                const uint2 fl = __ldcg(reinterpret_cast<const uint2*>(t + AGR_OFF_FLAGS));
+                c.t_flags = fl.x; c.t_lens = fl.y;
+                c.t_body = __ldcg(reinterpret_cast<const uint32_t*>(t + AGR_OFF_BODY_LEN));
+                c.r_agent0 = h2; c.r_agent1 = h3;
+                c.known = 4u;
+            } else c.known = 3u;
         }
     }
     if (c.cas_issued) {
@@ -216,6 +235,14 @@ __device__ __forceinline__ k1_result k1_finish(const agr_dev& d, uint32_t rid, c
             vflags |= AGR_VF_TRACKED;
             if (c.known == 1u) {                                                          // dedupe hit decided here (see k1_begin)
                 if (rt_slot(c.o_route) == c.slot && (c.o_state & ST_STORED)) { vflags |= AGR_VF_KNOWN; lc[C_DEDUPE_HITS]++; }
+            } else if (c.known == 4u) {                                                   // the same-batch target's store condition
+                const uint4 x0 = make_uint4(c.t_agent0.x ^ c.r_agent0.x, c.t_agent0.y ^ c.r_agent0.y, c.t_agent0.z ^ c.r_agent0.z, c.t_agent0.w ^ c.r_agent0.w);
+                const uint4 x1 = make_uint4(c.t_agent1.x ^ c.r_agent1.x, c.t_agent1.y ^ c.r_agent1.y, c.t_agent1.z ^ c.r_agent1.z, c.t_agent1.w ^ c.r_agent1.w);
+                const bool same_agent = (x0.x | x0.y | x0.z | x0.w | x1.x | x1.y | x1.z | x1.w) == 0u;
+                const bool stored = (d.cfg_flags & AGR_CFG_PERSISTENCE) && !(c.t_flags & AGR_F_REPLAY) &&
+                                    !((d.cfg_flags & AGR_CFGI_HOLES) && (c.t_flags & AGR_FI_HOLE)) &&
+                                    (unsigned long long)(c.t_lens & 0xffffu) + (c.t_lens >> 16) + c.t_body <= AGR_REC - AGR_OFF_PAYLOAD;
+                if (same_agent && stored) { vflags |= AGR_VF_KNOWN; lc[C_DEDUPE_HITS]++; }
             } else if (c.known == 2u) {
                 vflags |= AGR_VF_DUP_ID;                                                  // marker "resolve me in the post pass" (never
                 lc[K1_NLC]++;                                                             // a real flag of a replay-flagged row)

@@ -957,9 +957,8 @@ static int launch_k1_locked(agr_handle* h, uint64_t first, uint32_t n, agr_verdi
         const uint64_t k = h->tev_next++ % AGR_TIMING_RING;
         e0 = h->tev[2 * k]; e1 = h->tev[2 * k + 1];
     }
-    agr_launch_k1(h->d, (uint32_t)phys_row(h, first), first, n, h->cfg.k1_variant, (h->cfg.k1_variant & 0xfu) != AGR_K1_LSU ? h->tmap : nullptr,
-                  h->sm_count, h->stream, e0, e1, d_out, d_ids);
-    h->k1_launches += agr_k1_launches_per_batch(h->cfg.k1_variant);
+    h->k1_launches += agr_launch_k1(h->d, (uint32_t)phys_row(h, first), first, n, h->cfg.k1_variant,
+                                    (h->cfg.k1_variant & 0xfu) != AGR_K1_LSU ? h->tmap : nullptr, h->sm_count, h->stream, e0, e1, d_out, d_ids);
     CK(cudaGetLastError());
     return 0;
 }

@@ -46,7 +46,9 @@ __device__ __forceinline__ uint4 lds128(uint32_t addr) {
 }
 __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 
-template <int WARPS, int STAGES>
+// MINT: the engine mints ids (AGR_CFG_MINT_IDS), so k1_begin decides every replay's dedupe hit; the hash-id instantiation carries
+// none of that code (the index CAS loop is latency-bound, and the larger loop body cost it ~1.6 us a C2 step on H100).
+template <int WARPS, int STAGES, bool MINT>
 __global__ void __launch_bounds__(WARPS * 32, 1)
 k1_ingest_tma(const __grid_constant__ CUtensorMap tmap, const agr_dev d, const uint32_t first_rid, const unsigned long long first_log,
               const uint32_t n, const uint32_t pf_dist) {
@@ -58,8 +60,14 @@ k1_ingest_tma(const __grid_constant__ CUtensorMap tmap, const agr_dev d, const u
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     if (threadIdx.x < K1_NLC) s_ctr[threadIdx.x] = 0;
     if (threadIdx.x < WARPS * STAGES) mbar_init(smem_u32(&bars[threadIdx.x]), 1);
+    if (threadIdx.x == 0) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap) : "memory");
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     __syncthreads();
+    // Programmatic dependent launch (launch_tma): nothing above touches global memory, and the wait returns once the previous
+    // kernel of the stream has completed and its writes are visible (at once when the launch was not programmatic).
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    // the previous batch is done with the other set of per-batch words: zero it for the next one (k1_post, when it runs, does too)
+    if (blockIdx.x == 0 && threadIdx.x < 4) d.dupfix_next[threadIdx.x] = 0;
 
     uint32_t lc[K1_NLC + 1];
 #pragma unroll
@@ -162,15 +170,21 @@ k1_ingest_tma(const __grid_constant__ CUtensorMap tmap, const agr_dev d, const u
                 d.route[prid] = r.route;
             }
             // one bit per row the post pass has to visit (tracked replays): it then reads 4 B per 32 rows instead of every route word
-            const uint32_t mk = __ballot_sync(FULL, pvalid && (rt_flags(r.route) & (AGR_VF_REPLAY | AGR_VF_DUP_ID)) == (AGR_VF_REPLAY | AGR_VF_DUP_ID));
-            if (lane == 0 && d.marks) d.marks[ptile] = mk;
+            if (d.marks) {
+                const uint32_t mk = __ballot_sync(FULL, pvalid && (rt_flags(r.route) & (AGR_VF_REPLAY | AGR_VF_DUP_ID)) == (AGR_VF_REPLAY | AGR_VF_DUP_ID));
+                if (lane == 0) d.marks[ptile] = mk;
+            }
         }
         // this tile: agent loads have landed by now; classify and put the index CAS in flight.  pcx is dead here
         // (just consumed), so the CAS writes straight into the loop-carried registers.
-        if (valid) k1_begin(d, ap, h0, h1, h2, h3, h4, h5.x, AGR_REC - AGR_OFF_PAYLOAD, first_log, pcx);
+        if (valid) k1_begin(d, ap, h0, h1, h2, h3, h4, h5.x, AGR_REC - AGR_OFF_PAYLOAD, MINT, first_log, first_log + i, pcx);
         ph1 = h1; ph5y = h5.y; prid = rid; pvalid = valid; ptile = tile;
         if (s == STAGES - 1) phase ^= 1u;
     }
+    // The next K1 on the stream may start once every CTA of this one has streamed its tiles: its launch is processed during this
+    // launch's drain, and its CTAs take each SM the moment this launch's CTA leaves it.  (Measured on H100: ~0.5 us a step
+    // better than triggering at the start.)
+    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     if ((blockIdx.x * WARPS + warp) < tiles) {                    // this warp had at least one tile: flush its last one
         k1_result r{0u, 0u};
         if (pvalid) {
@@ -179,8 +193,10 @@ k1_ingest_tma(const __grid_constant__ CUtensorMap tmap, const agr_dev d, const u
             d.state[prid] = r.state;
             d.route[prid] = r.route;
         }
-        const uint32_t mk = __ballot_sync(FULL, pvalid && (rt_flags(r.route) & (AGR_VF_REPLAY | AGR_VF_DUP_ID)) == (AGR_VF_REPLAY | AGR_VF_DUP_ID));
-        if (lane == 0 && d.marks) d.marks[ptile] = mk;
+        if (d.marks) {
+            const uint32_t mk = __ballot_sync(FULL, pvalid && (rt_flags(r.route) & (AGR_VF_REPLAY | AGR_VF_DUP_ID)) == (AGR_VF_REPLAY | AGR_VF_DUP_ID));
+            if (lane == 0) d.marks[ptile] = mk;
+        }
     }
     k1_flush_counters(d, lc, s_ctr);
 }
@@ -208,13 +224,13 @@ int agr_k1_tma_make_map(void* slab, unsigned long long rows, void* out_map /*128
     return r == CUDA_SUCCESS ? 0 : -2;
 }
 
-template <int WARPS, int STAGES>
-static cudaError_t launch_tma(const void* map, const agr_dev& d, uint32_t first_rid, unsigned long long first_log, uint32_t n,
+template <int WARPS, int STAGES, bool MINT>
+static cudaError_t launch_tma_k(const void* map, const agr_dev& d, uint32_t first_rid, unsigned long long first_log, uint32_t n,
                               uint32_t pf_dist, int sm_count, cudaStream_t st) {
     const size_t smem = (size_t)WARPS * STAGES * TILE_BYTES + 1024;
     static bool attr_done = false;
     if (!attr_done) {
-        cudaError_t e = cudaFuncSetAttribute(k1_ingest_tma<WARPS, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        cudaError_t e = cudaFuncSetAttribute(k1_ingest_tma<WARPS, STAGES, MINT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
         attr_done = true;
     }
@@ -222,8 +238,21 @@ static cudaError_t launch_tma(const void* map, const agr_dev& d, uint32_t first_
     uint32_t blocks = (uint32_t)sm_count;
     const uint32_t need = (tiles + WARPS - 1) / WARPS;
     if (blocks > need) blocks = need;
-    k1_ingest_tma<WARPS, STAGES><<<blocks, WARPS * 32, smem, st>>>(*(const CUtensorMap*)map, d, first_rid, first_log, n, pf_dist);
-    return cudaGetLastError();
+    // programmatic stream serialization: the launch may start during the tail of the kernel before it on the stream (the kernel
+    // waits for that one to complete before it touches global memory)
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(blocks); cfg.blockDim = dim3(WARPS * 32); cfg.dynamicSmemBytes = smem; cfg.stream = st;
+    cfg.attrs = attr; cfg.numAttrs = 1;
+    return cudaLaunchKernelEx(&cfg, k1_ingest_tma<WARPS, STAGES, MINT>, *(const CUtensorMap*)map, d, first_rid, first_log, n, pf_dist);
+}
+template <int WARPS, int STAGES>
+static cudaError_t launch_tma(const void* map, const agr_dev& d, uint32_t first_rid, unsigned long long first_log, uint32_t n,
+                              uint32_t pf_dist, int sm_count, cudaStream_t st) {
+    return (d.cfg_flags & AGR_CFG_MINT_IDS) ? launch_tma_k<WARPS, STAGES, true>(map, d, first_rid, first_log, n, pf_dist, sm_count, st)
+                                            : launch_tma_k<WARPS, STAGES, false>(map, d, first_rid, first_log, n, pf_dist, sm_count, st);
 }
 
 // variant 1 (default TMA): 7 warps x 2 stages; 2: 6 x 2; 3: 4 x 3; 4: 14 x 1 (all: one persistent CTA per SM)

@@ -40,7 +40,7 @@ __global__ void __launch_bounds__(WARPS * 32) k1_ingest_v0(const agr_dev d, cons
         // ---- long-latency chain first: agent probe -> classification -> first index CAS in flight
         const ag_probe ap = k1_agent_issue(d, h2, h3);
         k1_ctx cx;
-        if (valid) k1_begin(d, ap, h0, h1, h2, h3, h4, h5.x, AGR_REC - AGR_OFF_PAYLOAD, 0ULL, cx);
+        if (valid) k1_begin(d, ap, h0, h1, h2, h3, h4, h5.x, AGR_REC - AGR_OFF_PAYLOAD, false, 0ULL, 0ULL, cx);
         // ---- pass 2 (pure streaming, independent of the decision chain): payload checksum
         uint32_t c0 = 0, c1 = 0;
         {
@@ -445,7 +445,6 @@ void agr_launch_reindex(const agr_dev& d, uint32_t rows, cudaStream_t st) {
     if (rows) k1_index<<<(rows + 255u) / 256u, 256, 0, st>>>(d, 0u, rows);
 }
 
-int agr_k1_launches_per_batch(uint32_t variant) { return (variant & 0x10u) ? 3 : 2; }
 static uint32_t k1_post_blocks(uint32_t n, int sm_count) {
     uint32_t b = (n + 255u) / 256u, cap = (uint32_t)sm_count * 16u;
     return b < cap ? b : cap;
@@ -459,18 +458,28 @@ void agr_launch_k1_post(const agr_dev& d, uint32_t first_rid, uint32_t n, int sm
     if (n) k1_post<<<k1_post_blocks(n, sm_count), 256, 0, st>>>(d, first_rid, n, (uint2*)verdicts, (uint4*)ids, marks);
 }
 
-void agr_launch_k1(const agr_dev& d, uint32_t first_rid, unsigned long long first_log, uint32_t n, uint32_t variant, const void* tmap,
-                   int sm_count, cudaStream_t st, cudaEvent_t ev0, cudaEvent_t ev1, void* verdicts, void* ids) {
-    if (n == 0) return;
+int agr_launch_k1(const agr_dev& d, uint32_t first_rid, unsigned long long first_log, uint32_t n, uint32_t variant, const void* tmap,
+                  int sm_count, cudaStream_t st, cudaEvent_t ev0, cudaEvent_t ev1, void* verdicts, void* ids) {
+    if (n == 0) return 0;
     if (ev0) cudaEventRecord(ev0, st);
     if ((variant & 0xfu) != AGR_K1_LSU && tmap != nullptr) {
-        agr_launch_k1_tma(variant & 0xfu, tmap, d, first_rid, first_log, n, (variant >> 8) & 0xffu, sm_count, st);
+        // minted ids never race for an id (dupfix stays 0) and the TMA kernel decides every replay's dedupe hit itself: without
+        // verdicts or ids to write there is nothing left for k1_post, and the kernel neither marks rows nor needs the pass
+        const bool post = !(d.cfg_flags & AGR_CFG_MINT_IDS) || (d.cfg_flags & AGR_CFGI_SPLIT_INDEX) || verdicts != nullptr || ids != nullptr;
+        agr_dev dk = d;
+        if (!post) dk.marks = nullptr;
+        agr_launch_k1_tma(variant & 0xfu, tmap, dk, first_rid, first_log, n, (variant >> 8) & 0xffu, sm_count, st);
         if (ev1) cudaEventRecord(ev1, st);
-        if ((d.cfg_flags & AGR_CFGI_SPLIT_INDEX) && !(d.cfg_flags & AGR_CFG_MINT_IDS)) k1_index<<<(n + 255u) / 256u, 256, 0, st>>>(d, first_rid, n);
+        if (!post) return 1;
+        int launched = 2;
+        if ((d.cfg_flags & AGR_CFGI_SPLIT_INDEX) && !(d.cfg_flags & AGR_CFG_MINT_IDS)) {
+            k1_index<<<(n + 255u) / 256u, 256, 0, st>>>(d, first_rid, n);
+            launched = 3;
+        }
         // minted ids never race for an id (dupfix stays 0): without verdicts or ids to write, k1_post visits the marked rows only
         const bool sparse = d.marks && (d.cfg_flags & AGR_CFG_MINT_IDS) && verdicts == nullptr && ids == nullptr;
         k1_post<<<k1_post_blocks(sparse ? (n + 31u) / 32u : n, sm_count), 256, 0, st>>>(d, first_rid, n, (uint2*)verdicts, (uint4*)ids, d.marks);
-        return;
+        return launched;
     }
     constexpr int WARPS = 8;
     const uint32_t tiles = (n + 31u) / 32u;
@@ -479,8 +488,13 @@ void agr_launch_k1(const agr_dev& d, uint32_t first_rid, unsigned long long firs
     if (blocks > maxb) blocks = maxb;
     k1_ingest_v0<WARPS><<<blocks, WARPS * 32, 0, st>>>(d, first_rid, n);
     if (ev1) cudaEventRecord(ev1, st);
-    if ((d.cfg_flags & AGR_CFGI_SPLIT_INDEX) && !(d.cfg_flags & AGR_CFG_MINT_IDS)) k1_index<<<(n + 255u) / 256u, 256, 0, st>>>(d, first_rid, n);
+    int launched = 2;
+    if ((d.cfg_flags & AGR_CFGI_SPLIT_INDEX) && !(d.cfg_flags & AGR_CFG_MINT_IDS)) {
+        k1_index<<<(n + 255u) / 256u, 256, 0, st>>>(d, first_rid, n);
+        launched = 3;
+    }
     k1_post<<<k1_post_blocks(n, sm_count), 256, 0, st>>>(d, first_rid, n, (uint2*)verdicts, (uint4*)ids, nullptr);
+    return launched;
 }
 
 // ------------------------------------------------------------------------------------------------ K2

@@ -39,7 +39,7 @@ struct agr_dev {
     unsigned long long* log_len;   // [0] completed, [1] failed
     unsigned long long log_cap;
     uint32_t* dupfix;          // per-batch words: [0] in-batch duplicate-id races (see k1_post), [1] spare, [2] replay-flagged records
-    uint32_t* dupfix_next;     // the other copy of those words: k1_post clears it for the next batch (no memset between batches)
+    uint32_t* dupfix_next;     // the other copy of those words: the TMA K1 and k1_post clear it for the next batch (no memset between batches)
     uint32_t* marks;           // K1 (TMA kernel) -> k1_post: one bit per row of the batch that the post pass must visit; nullptr = visit all
     uint32_t* head;            // [rows] K2 per-batch chain head of a row (op index + 1, 0 when idle)
     unsigned long long* ptime; // [rows] time.Now() of the latest StoreResponse (requests.go:146,164), the outcome's seq
@@ -180,8 +180,9 @@ void agr_launch_k4_unpermute(const agr_k4_params& p, const void* local_res, cons
                              cudaStream_t st);
 
 // first_log: arrival number of the batch's first row (= first_rid unless the slab is a ring).  With engine-minted ids the TMA
-// kernels decide a replay's dedupe hit on a row of an earlier batch themselves; k1_post resolves only the rest.
-void agr_launch_k1(const agr_dev& d, uint32_t first_rid, unsigned long long first_log, uint32_t n, uint32_t variant, const void* tmap,
+// kernels decide every replay's dedupe hit themselves, and k1_post is launched only to write verdicts or ids.
+// Returns the number of kernels launched.
+int agr_launch_k1(const agr_dev& d, uint32_t first_rid, unsigned long long first_log, uint32_t n, uint32_t variant, const void* tmap,
                    int sm_count, cudaStream_t st, cudaEvent_t ev0 = nullptr, cudaEvent_t ev1 = nullptr,
                    void* verdicts = nullptr /* device agr_verdict[n], written by k1_post */,
                    void* ids = nullptr /* device u8[n][16]: Request.ID per record, written by k1_post */);
@@ -214,4 +215,3 @@ void agr_launch_k3_gather(const agr_dev& d, const uint32_t* rids, const uint32_t
 void agr_launch_drop_agent(const agr_dev& d, uint32_t slot, unsigned long long rows, unsigned long long max_log_len,
                            cudaStream_t st);
 void agr_launch_synth(uint8_t* dst, agr_synth_dev s, unsigned long long first_index, uint32_t n, cudaStream_t st);
-int  agr_k1_launches_per_batch(uint32_t variant);
