@@ -671,6 +671,15 @@ void agr_launch_k2(const agr_dev& d, const void* outs, const agr_k2_scratch& s, 
 // give the stable rank — the warp-ballot agent-id partition.
 struct k3_item { bool sel; uint32_t rid; uint32_t slot; bool inq; };
 
+// q = pb + offset within a warp's run (< 2 * ring_rows + 2) back into the ring
+__device__ __forceinline__ uint32_t k3_wrap(const agr_dev& d, uint32_t q) {
+    if (d.ring_rows && q >= d.ring_rows) {
+        q -= d.ring_rows;
+        if (q >= d.ring_rows) q -= d.ring_rows;
+    }
+    return q;
+}
+
 // `st` = the row's state word (row modes; prefetched by the caller) — unused in log mode
 // `prow` = the physical row of item `it` (row modes)
 __device__ __forceinline__ k3_item k3_eval(const agr_dev& d, const agr_k3_params& p, unsigned long long it, uint32_t prow, uint32_t st, uint32_t rt) {
@@ -726,13 +735,10 @@ __global__ void __launch_bounds__(256) k3_mark(const agr_dev d, const agr_k3_par
     uint32_t mininq = AGR_RID_NONE;
     const bool rows = (p.mode != K3_LOG_AGENT);
     uint32_t* mask = p.selmask + (size_t)w * (p.per_warp >> 5);
-    // physical row of item k: the warp's run is contiguous in the ring and wraps at most once
+    // physical row of item k: the warp's run is contiguous in the ring.  The window is [lo & ~3, hi) with hi - lo <= ring_rows,
+    // so a run holds at most ring_rows + 3 items; one that starts at pb >= ring_rows - 2 (only when ring_rows % 4 != 0) wraps twice
     const uint32_t pb = rows ? row_physical(d, b) : 0u;
-    auto prow_of = [&](unsigned long long k) -> uint32_t {
-        uint32_t q = pb + (uint32_t)(k - b);
-        if (d.ring_rows && q >= d.ring_rows) q -= d.ring_rows;
-        return q;
-    };
+    auto prow_of = [&](unsigned long long k) -> uint32_t { return k3_wrap(d, pb + (uint32_t)(k - b)); };
     // Row modes, aligned run (the host rounds `lo` down to a multiple of 4; ring sizes that are not one take the scalar path): a lane
     // owns FOUR consecutive rows, so the row words arrive as two 16-byte loads per 128-row group instead of eight 4-byte ones;
     // the groups of 512 rows are in flight at once.  The selection bits are put together from the lanes' nibbles (three xor-shuffles).
@@ -855,7 +861,7 @@ __global__ void __launch_bounds__(256) k3_place(const agr_dev d, const agr_k3_pa
     uint16_t* list = s_list[threadIdx.x >> 5];
     auto fetch = [&](const uint32_t blk_first, const uint32_t i, uint32_t& rid, uint32_t& rt) {
         const unsigned long long k = b + blk_first + list[i];
-        if (rows) { rid = pb + (uint32_t)(k - b); if (d.ring_rows && rid >= d.ring_rows) rid -= d.ring_rows; }
+        if (rows) rid = k3_wrap(d, pb + (uint32_t)(k - b));
         else rid = p.log[k];
         rt = __ldg(&d.route[rid]);
     };
