@@ -375,8 +375,9 @@ class Engine:
         return ms.value
 
     def debug_read(self, which: str, first_rid: int, n: int) -> np.ndarray:
-        sel = {"state": 0, "route": 1, "aux": 2, "cksum": 3, "verdict": 4}[which]
-        out = np.zeros(n, dtype=verdict_dtype if sel == 4 else np.uint64 if sel == 3 else np.uint32)
+        """Per-row words of logical rows [first_rid, +n); "cmin": the TTL sweep's time bounds of physical chunks [first_rid, +n)."""
+        sel = {"state": 0, "route": 1, "aux": 2, "cksum": 3, "verdict": 4, "mtime": 5, "cmin": 6}[which]
+        out = np.zeros(n, dtype=verdict_dtype if sel == 4 else np.uint64 if sel in (3, 5, 6) else np.uint32)
         _check(self.lib, self.lib.agr_debug_read(self.h, sel, first_rid, n, _ptr(out)))
         return out
 

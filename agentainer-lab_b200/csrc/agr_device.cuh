@@ -273,6 +273,7 @@ __device__ __forceinline__ void k1_note_time(const agr_dev& d, const uint32_t fi
     if ((threadIdx.x & 31) == 0 && count) {
         unsigned long long t = pack64(lmin, hmin);
         if (t == 0ULL) t = 1ULL;                                                          // 0 means "unknown"
+        if (t == ~0ULL) t = ~0ULL - 1ULL;                                                 // ~0 means "no stored row"
         const uint32_t c0 = first / AGR_CHUNK_ROWS, c1 = (first + count - 1u) / AGR_CHUNK_ROWS;
         atomicMin(d.cmin + c0, t);
         if (c1 != c0) atomicMin(d.cmin + c1, t);
@@ -556,10 +557,12 @@ __device__ __forceinline__ void k2_apply_one(const agr_dev& d, const agr_k2_scra
     d.aux[rid] = r.aux;
     if (r.responded) d.ptime[rid] = r.ptime;
     if (r.written) {
-        d.mtime[rid] = r.mtime;
+        // mtime 0 reads "K2 never SET this row" in the sweep (it then takes created_at): a SET at time 0 counts as one at 1 ns
+        const unsigned long long t = r.mtime ? r.mtime : 1ULL;
+        d.mtime[rid] = t;
         unsigned long long* cm = d.cmin + rid / AGR_CHUNK_ROWS;             // the TTL sweep's bound must stay a lower bound
-        const unsigned long long cur = __ldcg(cm), t = r.mtime ? r.mtime : 1ULL;
-        if (cur != 0ULL && cur != ~0ULL && t < cur) atomicMin(cm, t);   // (0: unknown, ~0: never swept / empty — both are recomputed)
+        const unsigned long long cur = __ldcg(cm), b = t < ~0ULL ? t : ~0ULL - 1ULL;  // (~0 means "no stored row")
+        if (cur != 0ULL && cur != ~0ULL && b < cur) atomicMin(cm, b);   // (0: unknown, ~0: never swept / empty — both are recomputed)
     }
     d.head[rid] = 0;
 }

@@ -2431,6 +2431,13 @@ int agr_debug_read(agr_handle* h, int which, uint64_t first_rid, uint32_t n, voi
     if (!h || (n && !out)) return fail(AGR_EINVAL, "NULL argument");
     HLock lk(h);
     CK(cudaSetDevice(h->device));
+    if (which == AGR_DBG_CMIN) {                              // per physical chunk, not per row
+        const uint64_t chunks = h->cfg.slab_rows / AGR_CHUNK_ROWS + 1;
+        if (first_rid > chunks || n > chunks - first_rid) return fail(AGR_EINVAL, "chunk range out of bounds");
+        if (n) CK(cudaMemcpyAsync(out, h->d.cmin + first_rid, (size_t)n * 8, cudaMemcpyDeviceToHost, h->stream));
+        CK(cudaStreamSynchronize(h->stream));
+        return 0;
+    }
     if (!is_ring(h) && first_rid + n > h->cfg.slab_rows) return fail(AGR_EINVAL, "row range out of bounds");
     if (is_ring(h) && (first_rid + n > h->rows_used || n > h->cfg.slab_rows)) return fail(AGR_EINVAL, "row range out of bounds");
     const uint8_t* base = nullptr; size_t w = 4;
@@ -2442,6 +2449,7 @@ int agr_debug_read(agr_handle* h, int which, uint64_t first_rid, uint32_t n, voi
         case AGR_DBG_ROUTE: case AGR_DBG_VERDICT: base = (const uint8_t*)h->d.route; break;
         case AGR_DBG_AUX: base = (const uint8_t*)h->d.aux; break;
         case AGR_DBG_CKSUM: base = (const uint8_t*)h->d.cksum; w = 8; break;
+        case AGR_DBG_MTIME: base = (const uint8_t*)h->d.mtime; w = 8; break;
         default: return fail(AGR_EINVAL, "bad array selector");
     }
     const uint64_t p0 = phys_row(h, first_rid);

@@ -234,14 +234,17 @@ __global__ void __launch_bounds__(256) k_expire(const agr_dev d, const unsigned 
         const unsigned long long rid = r0 + threadIdx.x + q * 256u;
         if ((st[q] & ST_STORED) && t[q] == 0ULL) t[q] = __ldcs(reinterpret_cast<const unsigned long long*>(rec_ptr(d, (uint32_t)rid) + AGR_OFF_SEQ));
     }
+    // a SET at time 0 counts as one at 1 ns everywhere (0 is "never SET" in mtime and "unknown" in the bound), and a row kept
+    // at time ~0 enters the bound as ~0 - 1 (~0 is "no stored row", which would let k_first_live skip the chunk)
     unsigned long long lmin = ~0ULL;
     uint32_t gone = 0;
 #pragma unroll
     for (uint32_t q = 0; q < EXP_PER_THREAD; ++q) {
         if (!(st[q] & ST_STORED)) continue;
         const unsigned long long rid = r0 + threadIdx.x + q * 256u;
-        if (now >= t[q] && now - t[q] >= ttl) { d.state[rid] = st[q] & ~ST_STORED; gone++; }
-        else if (t[q] < lmin) lmin = t[q];
+        const unsigned long long tq = t[q] ? t[q] : 1ULL;
+        if (now >= tq && now - tq >= ttl) { d.state[rid] = st[q] & ~ST_STORED; gone++; }
+        else lmin = min(lmin, min(tq, ~0ULL - 1ULL));
     }
 #pragma unroll
     for (int o = 16; o; o >>= 1) { const unsigned long long y = __shfl_xor_sync(FULL, lmin, o); if (y < lmin) lmin = y; }
@@ -252,7 +255,7 @@ __global__ void __launch_bounds__(256) k_expire(const agr_dev d, const unsigned 
 #pragma unroll
         for (int w = 1; w < 8; ++w) if (s_min[w] < lmin) lmin = s_min[w];
         if (s_cnt && expired) atomicAdd(expired, (unsigned long long)s_cnt);
-        d.cmin[c] = (lmin == 0ULL) ? 1ULL : lmin;               // exact now (~0: the chunk holds no stored row any more)
+        d.cmin[c] = lmin;                                       // exact now (~0: the chunk holds no stored row any more)
     }
 }
 void agr_launch_expire(const agr_dev& d, unsigned long long rows, unsigned long long now, unsigned long long ttl,
@@ -371,7 +374,12 @@ __global__ void __launch_bounds__(256) k_log_count(const agr_dev d, const uint32
     __syncthreads();
     if (threadIdx.x == 0) chunk_cnt[blockIdx.x] = s_cnt;
 }
-__global__ void __launch_bounds__(1024) k_log_scan(uint32_t* chunk_cnt, const uint32_t nchunks, unsigned long long* new_len) {   // exclusive; total -> *new_len
+// exclusive scan of the chunk counts; the new length goes to *log_len.  Entries K2 pushed after the first `len` (agr_reclaim_async
+// compacts what its scan saw one step later) name rows that were stored when they were pushed, never released ones: they are
+// copied after the kept ones as they are.
+__global__ void __launch_bounds__(1024) k_log_scan(uint32_t* chunk_cnt, const uint32_t nchunks, const uint32_t* __restrict__ log,
+                                                   const unsigned long long len, uint32_t* __restrict__ out,
+                                                   unsigned long long* log_len) {
     __shared__ uint32_t s_w[32];
     __shared__ uint32_t s_carry;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -392,7 +400,10 @@ __global__ void __launch_bounds__(1024) k_log_scan(uint32_t* chunk_cnt, const ui
         if (threadIdx.x == 1023) s_carry = pre + x;
         __syncthreads();
     }
-    if (threadIdx.x == 0) { chunk_cnt[nchunks] = s_carry; *new_len = s_carry; }
+    const unsigned long long cur = *reinterpret_cast<volatile unsigned long long*>(log_len), kept = s_carry;
+    for (unsigned long long i = len + threadIdx.x; i < cur; i += 1024) out[kept + (i - len)] = log[i];
+    __syncthreads();
+    if (threadIdx.x == 0) { chunk_cnt[nchunks] = s_carry; *log_len = kept + (cur - len); }
 }
 // one warp per chunk keeps the order: 32 entries per step, ballot + popc
 __global__ void __launch_bounds__(32) k_log_scatter(const agr_dev d, const uint32_t* __restrict__ log, const unsigned long long len,
@@ -414,7 +425,7 @@ void agr_launch_log_compact(const agr_dev& d, const uint32_t* log, unsigned long
     if (!len) return;
     const uint32_t nch = (uint32_t)((len + LC_CHUNK - 1) / LC_CHUNK);
     k_log_count<<<nch, 256, 0, st>>>(d, log, len, released, chunk_cnt);
-    k_log_scan<<<1, 1024, 0, st>>>(chunk_cnt, nch, new_len);
+    k_log_scan<<<1, 1024, 0, st>>>(chunk_cnt, nch, log, len, out, new_len);
     k_log_scatter<<<nch, 32, 0, st>>>(d, log, len, released, chunk_cnt, out);
 }
 

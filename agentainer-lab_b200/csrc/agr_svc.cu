@@ -223,7 +223,7 @@ k_svc(const agr_dev d0, const svc_dev v, const agr_k2_scratch k2, const unsigned
             d.route[rid] = r.route;
             if ((r.state & ST_STORED) && (d.cfg_flags & AGR_CFG_RING)) {         // TTL bookkeeping (see k1_note_time)
                 unsigned long long t = pack64(h4.x, h4.y);
-                atomicMin(d.cmin + rid / AGR_CHUNK_ROWS, t ? t : 1ULL);
+                atomicMin(d.cmin + rid / AGR_CHUNK_ROWS, t == 0ULL ? 1ULL : t == ~0ULL ? ~0ULL - 1ULL : t);   // 0 unknown, ~0 empty
                 d.mtime[rid] = t;
             }
         }

@@ -120,7 +120,7 @@ typedef struct agr_config {
     uint64_t table_slots;    /* dedupe-index slots, power of two >= 2*slab_rows; 0 = auto */
     uint32_t max_agents;     /* agent-table capacity; 0 = 4096 */
     uint32_t max_batch;      /* largest n accepted by one agr_ingest / agr_complete; 0 = 1<<20 */
-    uint64_t log_entries;    /* capacity of the completed and failed logs; 0 = 2*slab_rows */
+    uint64_t log_entries;    /* capacity of the completed and failed logs; 0 = 3*slab_rows */
     uint64_t id_secret;      /* AGR_CFG_MINT_IDS: key of the id permutation; 0 = drawn from the OS CSPRNG at agr_create */
     uint64_t vslab_bytes;    /* AGR_CFG_VARLEN: capacity of the byte slab; 0 = 1024 * slab_rows */
     uint64_t resp_bytes;     /* capacity of the stored-response byte slab; 0 = 64 * slab_rows */
@@ -480,9 +480,12 @@ int agr_ingest_sharded_rows(agr_handle* h, uint64_t first_rid, uint32_t n, agr_v
 int agr_complete_sharded(agr_handle* h, const agr_outcome* outs, uint32_t n, int32_t* results, agr_exchange_info* info);
 
 /* Diagnostic read-back of the per-row SoA words (tests, snapshot tooling): which = 0 state (u32), 1 route (u32),
- * 2 aux (u32), 3 checksum (u64), 4 verdict (agr_verdict: what agr_ingest_rows returned for the row).  out must hold
- * n elements of that width. */
-enum { AGR_DBG_STATE = 0, AGR_DBG_ROUTE = 1, AGR_DBG_AUX = 2, AGR_DBG_CKSUM = 3, AGR_DBG_VERDICT = 4 };
+ * 2 aux (u32), 3 checksum (u64), 4 verdict (agr_verdict: what agr_ingest_rows returned for the row), 5 mtime (u64: the
+ * last-SET time K2 wrote, or — rings — K1; 0 = the TTL sweep takes the record's created_at).  6 cmin (u64) is per physical
+ * 4096-row chunk instead: first_rid is a chunk index and first_rid + n <= slab_rows / 4096 + 1; the value is a lower bound of
+ * the last-SET times of the chunk's stored rows (0 = unknown, ~0 = no stored row).  out must hold n elements of that width. */
+enum { AGR_DBG_STATE = 0, AGR_DBG_ROUTE = 1, AGR_DBG_AUX = 2, AGR_DBG_CKSUM = 3, AGR_DBG_VERDICT = 4, AGR_DBG_MTIME = 5,
+       AGR_DBG_CMIN = 6 };
 int agr_debug_read(agr_handle* h, int which, uint64_t first_rid, uint32_t n, void* out);
 
 /* -------------------------------------------------- synthetic stream (bench) */

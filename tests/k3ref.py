@@ -6,7 +6,8 @@ It is computed from what a test did to an engine, never from the engine's output
   * the outcomes applied, in call order,
   * the agent statuses at scan time, dropped agents,
   * rows expired by agr_expire and rows released by agr_reclaim,
-  * rows reserved but not filled yet (they bound every scan).
+  * rows reserved but not filled yet (they bound every scan),
+  * the time of every record and outcome (for the TTL sweep).
 
 The rules are the reference's (oracle/model.py):
   * every stored fresh record joins its agent's pending list, whatever the agent's status;
@@ -16,6 +17,9 @@ The rules are the reference's (oracle/model.py):
     onto the failed list, again on every later ERROR;
   * DIAL_ERR changes nothing; an outcome for a record that is not stored (expired, released, unknown) changes nothing;
   * an expired record stays in the pending list's ids but is not returned or replayed;
+  * a row's last-SET time is its record's created_at, then the time of every RESPONSE or ERROR applied to it while it is stored
+    (SET ... EX restarts the TTL, Q11); sweep(now, ttl) drops a stored row when now >= t and now - t >= ttl (MiniRedis.get,
+    model.py:74-80: the key expires at t + ttl; a clock behind t expires nothing);
   * a tick selects the pending, stored records of running agents with retry_count < max_retries, ordered by
     (agent slot, row) (model.py:353-376, the canonical cross-agent order Q9).
 """
@@ -44,6 +48,7 @@ class K3Ref:
         self.maxr = np.zeros(cap, dtype=np.uint8)
         self.resp = np.zeros(cap, dtype=np.uint16)
         self.ids = np.zeros((cap, 16), dtype=np.uint8)
+        self.mtime = np.zeros(cap, dtype=np.uint64)          # last-SET time
         self.logs = ([], [])                             # completed, failed: rows in push order
         self.resv = []                                   # [first, end) reserved, not filled
         self.agent_status = {}                           # slot -> status code
@@ -55,7 +60,7 @@ class K3Ref:
         if end <= cap:
             return
         new = max(end, 2 * cap)
-        for name in ("slot", "stored", "inq", "status", "retry", "err", "maxr", "resp", "ids"):
+        for name in ("slot", "stored", "inq", "status", "retry", "err", "maxr", "resp", "ids", "mtime"):
             a = getattr(self, name)
             b = np.zeros((new,) + a.shape[1:], dtype=a.dtype)
             if name == "slot":
@@ -95,8 +100,9 @@ class K3Ref:
         self.n = first + count
         self.resv.append((first, first + count))
 
-    def add_rows(self, first: int, slots, ids, max_retries=None) -> None:
-        """Rows [first, first + len(slots)) were ingested; slot -1 = not stored (unknown or dropped agent)."""
+    def add_rows(self, first: int, slots, ids, max_retries=None, created=None) -> None:
+        """Rows [first, first + len(slots)) were ingested; slot -1 = not stored (unknown or dropped agent); created: the
+        records' created_at (default 0)."""
         slots = np.asarray(slots, dtype=np.int64)
         end = first + len(slots)
         if first >= self.n:
@@ -119,12 +125,17 @@ class K3Ref:
         self.maxr[first:end] = self.max_retries if max_retries is None else max_retries
         self.resp[first:end] = 0
         self.ids[first:end] = ids
+        self.mtime[first:end] = 0 if created is None else np.asarray(created, dtype=np.uint64)
 
-    def complete(self, rows, kinds, https) -> None:
-        """Outcomes in call order (row = the record the outcome names, or -1 when it names none)."""
-        for r, k, h in zip(np.asarray(rows).tolist(), np.asarray(kinds).tolist(), np.asarray(https).tolist()):
+    def complete(self, rows, kinds, https, times=None) -> None:
+        """Outcomes in call order (row = the record the outcome names, or -1 when it names none); times: the outcomes' times
+        (default: the rows' times stay as they are)."""
+        times = [None] * len(rows) if times is None else np.asarray(times, dtype=np.uint64).tolist()
+        for r, k, h, t in zip(np.asarray(rows).tolist(), np.asarray(kinds).tolist(), np.asarray(https).tolist(), times):
             if r < self.tail or r >= self.n or not self.stored[r]:
                 continue                                  # the key does not exist: the call fails, nothing changes
+            if t is not None and k in (OUT_RESPONSE, OUT_ERROR):
+                self.mtime[r] = t                         # StoreResponse / MarkRequestFailed SET the record again
             if k == OUT_RESPONSE:
                 self.status[r] = ST_COMPLETED
                 self.resp[r] = h
@@ -148,15 +159,30 @@ class K3Ref:
         self.stored[rows] = False
         return len(rows)
 
+    def due(self, rows, now: int, ttl: int) -> np.ndarray:
+        """Which of these rows' last SET is ttl or more before now (the model's expiry rule; Python ints: no wrap-around)."""
+        t = self.mtime[np.asarray(rows, dtype=np.int64)].tolist()
+        return np.array([now >= x and now - x >= ttl for x in t], dtype=bool)
+
+    def sweep(self, now: int, ttl: int) -> int:
+        """agr_expire(now, ttl): every stored row whose last SET is due is dropped.  Returns how many."""
+        rows = np.flatnonzero(self.stored[self.tail:self.n]) + self.tail
+        rows = rows[self.due(rows, now, ttl)]
+        self.stored[rows] = False
+        return len(rows)
+
     def bound(self) -> int:
         """Every scan stops at the first reserved row K1 has not filled."""
         return min([self.n] + [r[0] for r in self.resv])
 
-    def reclaim(self) -> int:
-        """agr_reclaim: release the rows at the tail that hold no record, up to the first stored one (or the bound)."""
-        hi = self.bound()
-        live = np.flatnonzero(self.stored[self.tail:hi])
-        count = int(live[0]) if len(live) else hi - self.tail
+    def reclaim(self, count=None) -> int:
+        """agr_reclaim: release the rows at the tail that hold no record, up to the first stored one (or the bound).
+        count: release that many instead (what an earlier scan found: agr_reclaim_async)."""
+        if count is None:
+            hi = self.bound()
+            live = np.flatnonzero(self.stored[self.tail:hi])
+            count = int(live[0]) if len(live) else hi - self.tail
+        assert not self.stored[self.tail: self.tail + count].any()
         end = self.tail + count
         self.inq[self.tail:end] = False
         self.logs = tuple([r for r in log if r >= end] for log in self.logs)

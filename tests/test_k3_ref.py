@@ -94,3 +94,71 @@ def test_k3ref_equals_oracle(seed):
     for a, p in pend.items():
         assert p == o.lists[a]["pending"]
     assert sum(len(t) for t in ticks) > 0
+
+
+U64 = (1 << 64) - 1
+
+
+@pytest.mark.parametrize("seed", range(6))
+def test_k3ref_sweep_equals_the_model_clock(seed):
+    """K3Ref.sweep against MiniRedis's key expiry (SET ... EX at the SET's clock, GET at the sweep's clock): random records and
+    outcomes whose times run backwards (clock skew), sweeps at exactly t + ttl and t + ttl - 1 of some live row, sweeps behind
+    every time, time 0 and times up to UINT64_MAX.  After every sweep the set of stored rows is the set of live keys."""
+    from oracle.model import MiniRedis, RedisNil
+    rng = np.random.default_rng(900 + seed)
+    ttl = [1, 1000, 10**9, 1 << 40, 7, 12345][seed]
+    redis = MiniRedis()
+    redis.ticks_per_second = ttl                        # SET ... EX 1 = ttl of the stream's unit
+    ref = K3Ref()
+    ref.set_agents([0], [1])
+
+    def some_time(base):
+        c = rng.random()
+        if c < 0.05:
+            return 0
+        if c < 0.10:
+            return U64 - int(rng.integers(0, 3))
+        return max(0, min(U64, base + int(rng.integers(-3 * ttl, 3 * ttl + 1))))
+
+    base = int(rng.choice([0, 5 * ttl, U64 - 50 * ttl if ttl < 1 << 40 else 1 << 60]))
+    swept = 0
+    for step in range(60):
+        base = max(0, min(U64, base + int(rng.integers(0, 2 * ttl + 1))))
+        n = int(rng.integers(1, 20))
+        times = [some_time(base) for _ in range(n)]
+        first = ref.n
+        ref.add_rows(first, np.zeros(n, np.int64), np.zeros((n, 16), np.uint8), created=times)
+        for r, t in zip(range(first, first + n), times):
+            redis.now = t
+            redis.set(f"k{r}", r, ttl_s=1)
+        rows = rng.integers(0, ref.n, size=int(rng.integers(0, 12)))
+        kinds = rng.choice([OUT_RESPONSE, OUT_ERROR, OUT_DIAL_ERR], size=len(rows))
+        otimes = [some_time(base) for _ in rows]
+        for r, k, t in zip(rows.tolist(), kinds.tolist(), otimes):
+            if ref.stored[r] and k != OUT_DIAL_ERR:     # a SET of a key that exists (not swept yet)
+                assert f"k{r}" in redis.strings
+                redis.now = t
+                redis.set(f"k{r}", r, ttl_s=1)
+        ref.complete(rows, kinds, np.zeros(len(rows), np.int64), times=otimes)
+        live = np.flatnonzero(ref.stored[: ref.n])
+        c = rng.random()
+        if c < 0.6 and len(live):                       # exactly at a live row's expiry, or 1 ns before it
+            t = int(ref.mtime[int(rng.choice(live))])
+            now = t + ttl - int(rng.integers(0, 2))
+        elif c < 0.8:
+            now = max(0, base - int(rng.integers(0, 4 * ttl)))   # the clock behind most times
+        else:
+            now = int(rng.integers(0, 1 << 63)) * 2 + int(rng.integers(0, 2))
+        now = min(now, U64)
+        before = set(live.tolist())
+        swept += ref.sweep(now, ttl)
+        redis.now = now
+        alive = set()
+        for r in before:
+            try:
+                redis.get(f"k{r}")
+                alive.add(r)
+            except RedisNil:
+                pass
+        assert alive == set(np.flatnonzero(ref.stored[: ref.n]).tolist()), f"step {step}: now {now}"
+    assert swept > 0
