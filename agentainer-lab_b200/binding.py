@@ -72,7 +72,7 @@ ABI_SYMBOLS = [
     "agr_agent_hash", "agr_agent_shard", "agr_comm_unique_id", "agr_comm_init", "agr_ingest_sharded", "agr_complete_sharded", "agr_snapshot", "agr_restore", "agr_verify", "agr_store_response_body", "agr_get_response_body",
     "agr_store_response", "agr_store_error_text", "agr_get_record_json", "agr_pending_json", "agr_rows_json", "agr_expire", "agr_reclaim", "agr_set_agent_states", "agr_json_decode",
     "agr_submit_ingest", "agr_submit_complete", "agr_poll", "agr_wait", "agr_ring_capacity", "agr_ingest_sharded_rows", "agr_fill_rows", "agr_reclaim_async",
-    "agr_complete_ex", "agr_submit_complete_ex",
+    "agr_complete_ex", "agr_submit_complete_ex", "agr_submit_complete_large",
 ]
 
 _lib = None
@@ -115,6 +115,7 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
         "agr_complete": (i32, [vp, vp, u32, vp]),
         "agr_complete_ex": (i32, [vp, vp, u32, vp, vp, vp, vp]),
         "agr_submit_complete_ex": (i32, [vp, vp, vp, u32, vp, u32, C.POINTER(u64)]),
+        "agr_submit_complete_large": (i32, [vp, vp, vp, u32, vp, u32, C.POINTER(u64)]),
         "agr_submit_complete": (i32, [vp, vp, C.POINTER(u64)]),
         "agr_wait": (i32, [vp, u64, vp]),
         "agr_replay_scan": (i32, [vp, vp, vp, u32, C.POINTER(u32)]),
@@ -503,14 +504,21 @@ class Engine:
 
     def submit_complete_ex(self, outcome: np.ndarray, headers: bytes, body: bytes) -> int:
         """agr_submit_complete_ex: the outcome and its bytes (<= AGR_OUT_INLINE_BYTES) in one ticket; collect it with wait()."""
+        return self._submit_bytes(self.lib.agr_submit_complete_ex, outcome, headers, body)
+
+    def submit_complete_large(self, outcome: np.ndarray, headers: bytes, body: bytes) -> int:
+        """agr_submit_complete_large: the outcome and its bytes (<= AGR_OUT_TICKET_MAX_BYTES) in one ticket, spread over
+        consecutive ring slots above AGR_OUT_INLINE_BYTES; collect it with wait()."""
+        return self._submit_bytes(self.lib.agr_submit_complete_large, outcome, headers, body)
+
+    def _submit_bytes(self, fn, outcome: np.ndarray, headers: bytes, body: bytes) -> int:
         assert outcome.dtype == outcome_dtype
         o = np.ascontiguousarray(outcome.reshape(1))
         hb = (C.c_uint8 * max(1, len(headers))).from_buffer_copy(headers or b"\0")
         bb = (C.c_uint8 * max(1, len(body))).from_buffer_copy(body or b"\0")
         t = C.c_uint64()
         while True:
-            rc = self.lib.agr_submit_complete_ex(self.h, _ptr(o), C.cast(hb, C.c_void_p), len(headers), C.cast(bb, C.c_void_p),
-                                                 len(body), C.byref(t))
+            rc = fn(self.h, _ptr(o), C.cast(hb, C.c_void_p), len(headers), C.cast(bb, C.c_void_p), len(body), C.byref(t))
             if rc != K.AGR_EAGAIN:
                 _check(self.lib, rc)
                 return int(t.value)

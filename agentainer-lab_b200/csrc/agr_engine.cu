@@ -314,7 +314,7 @@ struct svc_host {
 };
 
 
-static void svc_fail_ops(svc_host* s, uint64_t from, uint64_t to, int rc, bool records_only);
+static void svc_fail_ops(svc_host* s, uint64_t from, uint64_t to, int rc, bool records_only, const uint32_t* conts);
 // stops the resident kernel; the caller holds h->mu, so no new batch can be published meanwhile
 static int svc_stop_locked(agr_handle* h) {
     svc_host* s = h->svc;
@@ -333,7 +333,7 @@ static int svc_stop_locked(agr_handle* h) {
         // whoever waits for an operation of those batches gets an error instead of waiting for ever
         for (uint64_t q = s->ctl->done_seq + 1; q <= s->seq; ++q) {
             const svc_desc* dsc = s->desc + (q % SVC_DESCS);
-            if (dsc->seq == q) svc_fail_ops(s, dsc->from, dsc->from + dsc->count, AGR_ECUDA, false);
+            if (dsc->seq == q) svc_fail_ops(s, dsc->from, dsc->from + dsc->count, AGR_ECUDA, false, dsc->cont);
         }
         s->fatal = AGR_ECUDA;
         return fail(AGR_ECUDA, "service kernel left with batches unprocessed");
@@ -374,18 +374,19 @@ struct HLock {
     HLock(const HLock&) = delete; HLock& operator=(const HLock&) = delete;
 };
 
-// answers every op of [from, to) from the host side (slab full, CUDA error): the callers see rc
-static void svc_fail_ops(svc_host* s, uint64_t from, uint64_t to, int rc, bool records_only) {
+// answers every op of [from, to) from the host side (slab full, CUDA error): the callers see rc.  conts: the batch's
+// continuation bits (relative to from), answered as already collected (nobody waits for them)
+static void svc_fail_ops(svc_host* s, uint64_t from, uint64_t to, int rc, bool records_only, const uint32_t* conts) {
     for (uint64_t a = from; a < to; ++a) {
         const uint32_t slot = (uint32_t)(a & (SVC_SLOTS - 1u));
         const uint32_t rw = s->ready[slot].load(std::memory_order_relaxed), kd = rw & 3u;
-        const bool rec = kd == SVC_OP_RECORD;
+        const bool rec = kd == SVC_OP_RECORD, cont = (conts[(a - from) >> 5] >> ((a - from) & 31u)) & 1u;
         // (a skipped slot has no waiter and keeps its old answer; it may even have been published again for the NEXT lap already)
         if ((rw >> 2) != (uint32_t)(a / SVC_SLOTS) + 1u || kd == SVC_OP_SKIP || (records_only && !rec)) continue;
         svc_res* r = s->res + slot;
-        r->w[0] = rec ? 0u : (uint32_t)rc; r->w[1] = rec ? (uint32_t)rc : 0u; r->w[2] = 0;
+        r->w[0] = rec ? 0u : cont ? 0u : (uint32_t)rc; r->w[1] = rec ? (uint32_t)rc : 0u; r->w[2] = 0;
         std::atomic_thread_fence(std::memory_order_release);
-        r->w[3] = svc_tag(a) << 16;
+        r->w[3] = (svc_tag(a) | (cont ? SVC_COLLECTED : 0u)) << 16;
     }
 }
 
@@ -398,9 +399,9 @@ static void svc_dispatcher(agr_handle* h) {
     // (re-reading the callers' ready words every iteration keeps pulling their cache lines away from the cores that write them)
     uint64_t to = s->taken;
     uint32_t nstaged = 0;                                        // records + outcomes with bytes: one 512 B stage slot of k_svc each
-    uint32_t kinds[SVC_MAX_OPS / 16] = {0};
+    uint32_t kinds[SVC_MAX_OPS / 16] = {0}, conts[SVC_MAX_OPS / 32] = {0};
     while (!s->shutdown.load(std::memory_order_acquire)) {
-        svc_scan(s, s->taken, &to, &nstaged, kinds, 128u);        // (csrc/agr_ring.hpp: shared with the CPU simulation of the ring)
+        svc_scan(s, s->taken, &to, &nstaged, kinds, 128u, conts); // (csrc/agr_ring.hpp: shared with the CPU simulation of the ring)
         const auto now = std::chrono::steady_clock::now();
         if (to == s->taken) {
             const auto idle = std::chrono::duration_cast<std::chrono::microseconds>(now - last_work).count();
@@ -431,30 +432,37 @@ static void svc_dispatcher(agr_handle* h) {
         }
         spins = 0;
         std::lock_guard<std::mutex> hl(h->mu);
-        if (s->fatal.load()) { svc_fail_ops(s, s->taken, to, s->fatal.load(), false); s->taken = to; nstaged = 0; memset(kinds, 0, sizeof kinds); continue; }
+        if (s->fatal.load()) {
+            svc_fail_ops(s, s->taken, to, s->fatal.load(), false, conts);
+            s->taken = to; nstaged = 0; memset(kinds, 0, sizeof kinds); memset(conts, 0, sizeof conts);
+            continue;
+        }
         if (s->running && s->ctl->state != 1u) {                // it left on its own (safety timeout): note it and start another
             cudaStreamSynchronize(h->stream);
             s->running = false;
         }
         // a resident kernel blocks device-wide synchronisations of other threads (cudaFree ...): let it go every 20 ms
         if (s->running && std::chrono::duration_cast<std::chrono::milliseconds>(now - s->started).count() > 20) svc_stop_locked(h);
-        // records, and the outcomes with bytes with their segments' region (16 B-rounded, in ring order)
-        uint32_t nrec = 0, nbytes = 0;
+        // records, and the outcomes with bytes with their segments' region (16 B-rounded, in ring order; a span's length is
+        // clamped to the slots the batch holds of it, as the kernel does)
+        const uint32_t count = (uint32_t)(to - s->taken);
+        uint32_t nrec = 0, nbytes = 0, ncont = 0;
         uint64_t byte_total = 0;
-        for (uint32_t k = 0; k < (uint32_t)(to - s->taken); ++k) {
+        for (uint32_t k = 0; k < count; ++k) {
             const uint32_t kd = (kinds[k >> 4] >> ((k & 15u) * 2u)) & 3u;
             if (kd == SVC_OP_RECORD) nrec++;
+            if ((conts[k >> 5] >> (k & 31u)) & 1u) { ncont++; continue; }
             if (kd == SVC_OP_OUTCOME_BYTES) {                    // (the slot's payload is visible: its ready word was acquired)
                 uint32_t len;
                 memcpy(&len, s->payload + (size_t)((s->taken + k) & (SVC_SLOTS - 1u)) * SVC_PAYLOAD + SVC_BYTES_HDR + 4, 4);
-                byte_total += (std::min(len, SVC_BYTES_MAX) + 15u) & ~15u;
+                byte_total += (svc_span_len(len, svc_conts_after(conts, k, count)) + 15u) & ~15u;
                 nbytes++;
             }
         }
         uint64_t first = 0;
         bool have_rows = true;
         if (nrec) {
-            if (reserve_rows_locked(h, nrec, &first) < 0) { svc_fail_ops(s, s->taken, to, AGR_ENOSPC, true); have_rows = false; }
+            if (reserve_rows_locked(h, nrec, &first) < 0) { svc_fail_ops(s, s->taken, to, AGR_ENOSPC, true, conts); have_rows = false; }
         }
         svc_desc dsc{};
         for (uint32_t k = 0; k < (uint32_t)(to - s->taken); ++k) {
@@ -462,12 +470,13 @@ static void svc_dispatcher(agr_handle* h) {
             if (kd == SVC_OP_RECORD && !have_rows) kd = SVC_OP_SKIP;
             dsc.kinds[k >> 4] |= kd << ((k & 15u) * 2u);
         }
+        memcpy(dsc.cont, conts, sizeof conts);
         dsc.resp_base = SVC_NO_BYTES;
         if (nbytes) {
             unsigned long long off;
             if (resp_reserve_locked(h, byte_total, byte_total, &off) == 0) dsc.resp_base = off;
         }
-        dsc.from = s->taken; dsc.count = (uint32_t)(to - s->taken); dsc.n_records = have_rows ? nrec : 0u;
+        dsc.from = s->taken; dsc.count = count; dsc.n_records = have_rows ? nrec : 0u;
         dsc.first_l = first; dsc.first_p = (uint32_t)phys_row(h, first);
         dsc.tail = h->tail; dsc.head_l = h->rows_used; dsc.tail_phys = is_ring(h) ? (uint32_t)(h->tail % h->cfg.slab_rows) : 0u;
         dsc.idx_base = h->d.idx_base;
@@ -484,13 +493,13 @@ static void svc_dispatcher(agr_handle* h) {
         s->seq = dsc.seq;
         s->taken = to;
         s->batches.fetch_add(1, std::memory_order_relaxed);
-        s->ops.fetch_add(dsc.count, std::memory_order_relaxed);
+        s->ops.fetch_add(dsc.count - ncont, std::memory_order_relaxed);     // operations: a span counts once
         h->k1_launches += nrec ? 1 : 0;                         // accounting: batches with records / with outcomes served by k_svc
         h->k2_launches += (dsc.count > nrec) ? 1 : 0;
-        nstaged = 0; memset(kinds, 0, sizeof kinds);
+        nstaged = 0; memset(kinds, 0, sizeof kinds); memset(conts, 0, sizeof conts);
         if (!s->running && svc_start_locked(h) < 0) {
             // could not launch: nothing will ever process this batch — fail it from here
-            svc_fail_ops(s, dsc.from, to, AGR_ECUDA, false);
+            svc_fail_ops(s, dsc.from, to, AGR_ECUDA, false, dsc.cont);
         }
     }
     std::lock_guard<std::mutex> hl(h->mu);
@@ -1340,19 +1349,30 @@ static int svc_complete_ex(agr_handle* h, const agr_outcome* outs, uint32_t n, c
     return 0;
 }
 
-int agr_submit_complete_ex(agr_handle* h, const agr_outcome* outcome, const uint8_t* headers, uint32_t hdr_len,
-                           const uint8_t* body, uint32_t body_len, agr_ticket* ticket) {
+// one outcome with its bytes in one ticket, hdr_len + body_len <= max_len (agr_submit_complete_ex: one slot;
+// agr_submit_complete_large: a span of slots above AGR_OUT_INLINE_BYTES)
+static int submit_outcome_bytes(agr_handle* h, const agr_outcome* outcome, const uint8_t* headers, uint32_t hdr_len, const uint8_t* body,
+                                uint32_t body_len, agr_ticket* ticket, uint32_t max_len, const char* too_long) {
     if (!h || !outcome || !ticket || (hdr_len && !headers) || (body_len && !body)) return fail(AGR_EINVAL, "NULL argument");
     if (!h->svc) return fail(AGR_EINVAL, "engine was not created with AGR_CFG_COMBINE");
-    if ((uint64_t)hdr_len + body_len > AGR_OUT_INLINE_BYTES)
-        return fail(AGR_EINVAL, "headers + body exceed AGR_OUT_INLINE_BYTES: use agr_complete_ex(n = 1)");
+    if ((uint64_t)hdr_len + body_len > max_len) return fail(AGR_EINVAL, too_long);
     if (outcome->kind != AGR_OUT_RESPONSE && outcome->kind != AGR_OUT_ERROR && hdr_len + body_len)
         return fail(AGR_EINVAL, "only AGR_OUT_RESPONSE and AGR_OUT_ERROR outcomes carry bytes");
     uint64_t a = 0;
-    if (!svc_submit_outcome_bytes(h->svc, outcome, outcome->kind == AGR_OUT_RESPONSE ? hdr_len : 0u, headers, hdr_len, body, body_len, &a))
+    if (!svc_submit_outcome_span(h->svc, outcome, outcome->kind == AGR_OUT_RESPONSE ? hdr_len : 0u, headers, hdr_len, body, body_len, &a))
         return AGR_EAGAIN;                                       // collect outstanding tickets (agr_poll) and come again
     *ticket = a | TICKET_OUTCOME;
     return 0;
+}
+int agr_submit_complete_ex(agr_handle* h, const agr_outcome* outcome, const uint8_t* headers, uint32_t hdr_len,
+                           const uint8_t* body, uint32_t body_len, agr_ticket* ticket) {
+    return submit_outcome_bytes(h, outcome, headers, hdr_len, body, body_len, ticket, AGR_OUT_INLINE_BYTES,
+                                "headers + body exceed AGR_OUT_INLINE_BYTES: use agr_submit_complete_large or agr_complete_ex(n = 1)");
+}
+int agr_submit_complete_large(agr_handle* h, const agr_outcome* outcome, const uint8_t* headers, uint32_t hdr_len,
+                              const uint8_t* body, uint32_t body_len, agr_ticket* ticket) {
+    return submit_outcome_bytes(h, outcome, headers, hdr_len, body, body_len, ticket, AGR_OUT_TICKET_MAX_BYTES,
+                                "headers + body exceed AGR_OUT_TICKET_MAX_BYTES: use agr_complete_ex(n = 1)");
 }
 
 // ------------------------------------------------------------------------------------------ K3

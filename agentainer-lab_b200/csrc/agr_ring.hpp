@@ -1,7 +1,8 @@
 // agr_ring.hpp — the CALLERS' side of the single-request ring (AGR_CFG_COMBINE; layout and protocol: agr_svc.h).
 //
 // Everything a calling thread does to hand one operation over and to collect its answer, as templates over the host-side ring
-// object H (agr_engine.cu's svc_host; the stand-ins of tests/ring_sim.cpp and tests/ring_sim_bytes.cpp).  H provides:
+// object H (agr_engine.cu's svc_host; the stand-ins of tests/ring_sim.cpp, tests/ring_sim_bytes.cpp and tests/ring_sim_span.cpp).
+// H provides:
 //   svc_res* res; uint8_t* payload; std::atomic<uint32_t>* ready;          pinned, device-mapped in the engine
 //   std::atomic<uint64_t> head, scanned; std::atomic<uint32_t> waiters; uint32_t spin_cpus;
 //   std::atomic<bool> sleeping; std::mutex smu; std::condition_variable scv;   the dispatcher's sleep / wake-up
@@ -93,6 +94,67 @@ static bool svc_submit_outcome_bytes(H* s, const void* outcome, uint32_t hdr_len
     memset(item + SVC_BYTES_DATA + len, 0, used - SVC_BYTES_DATA - len);
     return svc_submit_one(s, SVC_OP_OUTCOME_BYTES, item, used, abs);
 }
+// item_bytes (a multiple of 16) into a slot's payload, with streaming stores as in svc_submit_one
+template <class H>
+static inline void svc_stream_slot(H* s, uint32_t slot, const void* item, size_t item_bytes) {
+    __m128i* dst = reinterpret_cast<__m128i*>(s->payload + (size_t)slot * SVC_PAYLOAD);
+    const __m128i* src = reinterpret_cast<const __m128i*>(item);
+    for (size_t k = 0; k < item_bytes / 16; ++k) _mm_stream_si128(dst + k, _mm_loadu_si128(src + k));
+}
+// bytes [off, off + n) of the segment a | b
+static inline void svc_copy_seg(uint8_t* dst, const uint8_t* a, uint32_t a_len, const uint8_t* b, uint32_t off, uint32_t n) {
+    if (off < a_len) {
+        const uint32_t m = a_len - off < n ? a_len - off : n;
+        memcpy(dst, a + off, m);
+        dst += m; off += m; n -= m;
+    }
+    if (n) memcpy(dst, b + (off - a_len), n);
+}
+// hands over ONE outcome whose segment a | b may be longer than a slot holds (agr_submit_complete_large).  Up to SVC_BYTES_MAX
+// bytes it is svc_submit_outcome_bytes; above that a SPAN (agr_svc.h) of 1 + svc_span_conts(len) consecutive slots, claimed with
+// one fetch_add (slot numbers wrap past the ring's end like any other).  It is handed over only if every slot of it is free;
+// otherwise all of them go out as no-ops and the result is false, as for svc_submit_one.  a_len + b_len <=
+// AGR_OUT_TICKET_MAX_BYTES (the caller checks).
+template <class H>
+static bool svc_submit_outcome_span(H* s, const void* outcome, uint32_t hdr_len, const uint8_t* a, uint32_t a_len, const uint8_t* b,
+                                    uint32_t b_len, uint64_t* abs) {
+    const uint32_t len = a_len + b_len;
+    if (len <= SVC_BYTES_MAX) return svc_submit_outcome_bytes(s, outcome, hdr_len, a, a_len, b, b_len, abs);
+    const uint32_t n = 1u + svc_span_conts(len);
+    const uint64_t a0 = s->head.fetch_add(n, std::memory_order_relaxed);
+    // every slot is looked at, also after one that is not free: a slot's ready word may be written again only once the
+    // dispatcher has consumed its previous lap (svc_slot_free waits for that before it answers false)
+    bool ok = true;
+    for (uint32_t j = 0; j < n; ++j) {
+        const uint64_t x = a0 + j;
+        ok = svc_slot_free(s, x, (uint32_t)(x & (SVC_SLOTS - 1u)), (uint32_t)(x / SVC_SLOTS)) && ok;
+    }
+    if (ok) {
+        alignas(16) uint8_t item[SVC_PAYLOAD];
+        memcpy(item, outcome, SVC_BYTES_HDR);                         // head: outcome, hdr_len, len, the first SVC_BYTES_MAX bytes
+        memcpy(item + SVC_BYTES_HDR, &hdr_len, 4);
+        memcpy(item + SVC_BYTES_HDR + 4, &len, 4);
+        svc_copy_seg(item + SVC_BYTES_DATA, a, a_len, b, 0u, SVC_BYTES_MAX);
+        svc_stream_slot(s, (uint32_t)(a0 & (SVC_SLOTS - 1u)), item, SVC_PAYLOAD);
+        for (uint32_t j = 1; j < n; ++j) {                            // continuations: SVC_PAYLOAD bytes each, the last one 16 B-rounded
+            const uint32_t off = SVC_BYTES_MAX + (j - 1u) * SVC_PAYLOAD, m = len - off < SVC_PAYLOAD ? len - off : SVC_PAYLOAD;
+            const uint32_t used = (m + 15u) & ~15u;
+            svc_copy_seg(item, a, a_len, b, off, m);
+            memset(item + m, 0, used - m);
+            svc_stream_slot(s, (uint32_t)((a0 + j) & (SVC_SLOTS - 1u)), item, used);
+        }
+        _mm_sfence();
+    }
+    // the continuations first, the head last: the dispatcher, which consumes slots in order, finds a published head complete
+    const uint32_t kind = ok ? (uint32_t)SVC_OP_OUTCOME_BYTES : (uint32_t)SVC_OP_SKIP;
+    for (uint32_t j = n; j-- > 0;) {
+        const uint64_t x = a0 + j;
+        s->ready[x & (SVC_SLOTS - 1u)].store(((uint32_t)(x / SVC_SLOTS) + 1u) << 2 | kind, std::memory_order_release);
+    }
+    if (s->sleeping.load(std::memory_order_seq_cst)) { std::lock_guard<std::mutex> lk(s->smu); s->scv.notify_one(); }
+    *abs = a0;
+    return ok;
+}
 struct svc_answer { uint32_t w0, w1; uint64_t rid; };
 template <class H>
 static inline bool svc_try(H* s, uint64_t a, svc_answer* out) {
@@ -132,15 +194,35 @@ static inline void svc_release(H* s, uint64_t a) {       // everything of the an
 // the callers' ready words every iteration keeps pulling their cache lines away from the cores that write them), and an
 // operation's kind is noted in kinds[] (2 bits each, the batch descriptor's form) AT THAT MOMENT: a no-op slot may be published
 // again, for the next lap, as soon as `scanned` has passed it.  Publishes the new scan position.
+// A span (agr_svc.h) is taken whole or not at all: its head's len word (visible: the head's ready word was acquired, and the
+// continuations were published before it) says how many continuation slots follow; they count against both budgets, take the
+// head's kind in kinds[] and are marked in conts[] (1 bit per op, svc_desc.cont).  Callers that never hand over spans may pass
+// no conts.
 template <class H>
-static inline void svc_scan(H* s, const uint64_t taken, uint64_t* to, uint32_t* nstaged, uint32_t* kinds, const uint32_t max_staged) {
+static inline void svc_scan(H* s, const uint64_t taken, uint64_t* to, uint32_t* nstaged, uint32_t* kinds, const uint32_t max_staged,
+                            uint32_t* conts = nullptr) {
     while (*to - taken < SVC_MAX_OPS) {
         const uint32_t slot = (uint32_t)(*to & (SVC_SLOTS - 1u));
-        const uint32_t rw = s->ready[slot].load(std::memory_order_acquire);
+        const uint32_t rw = s->ready[slot].load(std::memory_order_acquire), kind = rw & 3u;
         if ((rw >> 2) != (uint32_t)(*to / SVC_SLOTS) + 1u) break;
-        if ((rw & 3u) == SVC_OP_RECORD || (rw & 3u) == SVC_OP_OUTCOME_BYTES) { if (*nstaged == max_staged) break; (*nstaged)++; }
-        kinds[(*to - taken) >> 4] |= (rw & 3u) << (((*to - taken) & 15u) * 2u);
-        (*to)++;
+        uint32_t n = 1u;                                                  // slots the op takes
+        if (kind == SVC_OP_OUTCOME_BYTES) {
+            uint32_t len;
+            memcpy(&len, s->payload + (size_t)slot * SVC_PAYLOAD + SVC_BYTES_HDR + 4, 4);
+            n += svc_span_conts(len);
+        }
+        if (n > 1u) {
+            if (*to - taken + n > SVC_MAX_OPS) break;
+            bool all = true;
+            for (uint32_t j = 1; j < n && all; ++j)
+                all = (s->ready[(slot + j) & (SVC_SLOTS - 1u)].load(std::memory_order_acquire) >> 2) == (uint32_t)((*to + j) / SVC_SLOTS) + 1u;
+            if (!all) break;
+        }
+        if (kind == SVC_OP_RECORD || kind == SVC_OP_OUTCOME_BYTES) { if (*nstaged + n > max_staged) break; *nstaged += n; }
+        for (uint32_t j = 0; j < n; ++j, ++*to) {
+            kinds[(*to - taken) >> 4] |= kind << (((*to - taken) & 15u) * 2u);
+            if (j) conts[(*to - taken) >> 5] |= 1u << ((*to - taken) & 31u);
+        }
     }
     if (*to != s->scanned.load(std::memory_order_relaxed)) s->scanned.store(*to, std::memory_order_release);
 }

@@ -56,7 +56,8 @@ k_svc(const agr_dev d0, const svc_dev v, const agr_k2_scratch k2, const unsigned
     extern __shared__ __align__(128) uint8_t smem[];
     __shared__ __align__(16) uint32_t s_dw[2][64];           // the accepted descriptors, as words
     __shared__ uint32_t s_go[2], s_nout[2], s_nbyt[2];
-    // s_rec_op: the ops whose whole slot is pulled into the stage — records, then the outcomes with bytes
+    // s_rec_op: the ops whose whole slot is pulled into the stage — records, then the outcomes with bytes and their spans'
+    // continuation slots, in ring order (so a span's slots lie next to each other)
     __shared__ uint16_t s_rec_op[2][SVC_MAX_RECS], s_out_op[2][SVC_MAX_OPS];
     __shared__ uint16_t s_out_stage[2][SVC_MAX_OPS];         // outcome -> its stage slot (outcomes with bytes), 0xffff = none
     __shared__ uint32_t s_wc[12], s_wf[12];
@@ -115,17 +116,19 @@ k_svc(const agr_dev d0, const svc_dev v, const agr_k2_scratch k2, const unsigned
                     for (uint32_t base = 0; base < D.count; base += 32u) {
                         const uint32_t op = base + lane;
                         const uint32_t kind = (op < D.count) ? ((D.kinds[op >> 4] >> ((op & 15u) * 2u)) & 3u) : 0u;
-                        const bool is_out = kind == SVC_OP_OUTCOME || kind == SVC_OP_OUTCOME_BYTES;
+                        const bool cont = (op < D.count) && ((D.cont[op >> 5] >> (op & 31u)) & 1u);   // staged, not an outcome
+                        const bool is_out = kind == SVC_OP_OUTCOME || (kind == SVC_OP_OUTCOME_BYTES && !cont);
                         const uint32_t mr = __ballot_sync(FULL, kind == SVC_OP_RECORD), mo = __ballot_sync(FULL, is_out);
                         const uint32_t mb = __ballot_sync(FULL, kind == SVC_OP_OUTCOME_BYTES);
                         if (kind == SVC_OP_RECORD) s_rec_op[st][br + __popc(mr & lt)] = (uint16_t)op;
                         if (is_out) {
                             const uint32_t oi = bo + __popc(mo & lt);
                             uint16_t sp = 0xffffu;
-                            if (kind == SVC_OP_OUTCOME_BYTES) { sp = (uint16_t)(D.n_records + bb + __popc(mb & lt)); s_rec_op[st][sp] = (uint16_t)op; }
+                            if (kind == SVC_OP_OUTCOME_BYTES) sp = (uint16_t)(D.n_records + bb + __popc(mb & lt));
                             s_out_op[st][oi] = (uint16_t)op;
                             s_out_stage[st][oi] = sp;
                         }
+                        if (kind == SVC_OP_OUTCOME_BYTES) s_rec_op[st][D.n_records + bb + __popc(mb & lt)] = (uint16_t)op;
                         br += __popc(mr); bo += __popc(mo); bb += __popc(mb);
                     }
                     nout = bo; nbyt = bb;
@@ -249,6 +252,16 @@ k_svc(const agr_dev d0, const svc_dev v, const agr_k2_scratch k2, const unsigned
             if (wt == 0 && dupfix) *v.dupfix = 0u;
         }
 
+        // ------------------------------------------------------------------ spans' continuation slots: their bytes are in the stage,
+        // and nobody collects them — answered as collected, so their slots may be taken for the next lap
+        for (uint32_t i = wt; i < s_nbyt[st]; i += SVC_WORKERS) {
+            const uint32_t op = s_rec_op[st][nrec + i];
+            if ((D.cont[op >> 5] >> (op & 31u)) & 1u) {
+                const unsigned long long slot_abs = from + op;
+                st_res(v.res + (slot_abs & (SVC_SLOTS - 1u)), 0u, 0u, 0u, (svc_tag(slot_abs) | SVC_COLLECTED) << 16);
+            }
+        }
+
         // ------------------------------------------------------------------ outcomes: link, apply, ordered append
         if (nout) {                                                               // nout is uniform over the workers
             const uint32_t nbyt = s_nbyt[st];
@@ -264,7 +277,8 @@ k_svc(const agr_dev d0, const svc_dev v, const agr_k2_scratch k2, const unsigned
                 uint32_t len = 0u, hl = 0u, sp = 0xffffu;
                 if (wt < nout && (sp = s_out_stage[st][wt]) != 0xffffu) {
                     const uint8_t* p = s_rec + (size_t)sp * 512u;
-                    len = min(*reinterpret_cast<const uint32_t*>(p + SVC_BYTES_HDR + 4), SVC_BYTES_MAX);
+                    // (a span's length: at most what its continuation slots staged after it hold)
+                    len = svc_span_len(*reinterpret_cast<const uint32_t*>(p + SVC_BYTES_HDR + 4), svc_conts_after(D.cont, s_out_op[st][wt], D.count));
                     hl = min(*reinterpret_cast<const uint32_t*>(p + SVC_BYTES_HDR), len);
                 }
                 const unsigned long long x = ((unsigned long long)((len + 15u) & ~15u) << 32) | len;
@@ -320,7 +334,8 @@ k_svc(const agr_dev d0, const svc_dev v, const agr_k2_scratch k2, const unsigned
                 }
                 d.log_len[0] = nc; d.log_len[1] = nf;
             }
-            // the winners' segments, from the stage into their places (warp per segment)
+            // the winners' segments, from the stage into their places (warp per segment; a span's continues in the stage slots
+            // after its head)
             if (bytes_in) {
                 for (uint32_t i = wwarp; i < nout; i += SVC_WORKERS / 32u) {
                     if (!(__ldcg(&k2.eff[i]) & K2_EFF_WIN)) continue;

@@ -17,6 +17,12 @@
 // Every other entry point stops the kernel first (it runs on the handle's stream), so the rest of the engine never sees it.
 #pragma once
 #include <stdint.h>
+#include "../../include/agentainer_gpu.h"   // AGR_OUT_TICKET_MAX_BYTES
+#if defined(__CUDACC__)
+#define SVC_HD __host__ __device__
+#else
+#define SVC_HD
+#endif
 
 #define SVC_SLOTS 16384u          // ring slots (power of two)
 #define SVC_MAX_OPS 256u          // operations per batch (<= 128 of them records: what one shared-memory stage of the kernel holds)
@@ -31,6 +37,35 @@
 #define SVC_NO_BYTES (~0ULL)      // svc_desc.resp_base when the batch's bytes found no room in the response byte slab
 
 enum { SVC_OP_SKIP = 0, SVC_OP_RECORD = 1, SVC_OP_OUTCOME = 2, SVC_OP_OUTCOME_BYTES = 3 };
+
+// A SPAN (agr_submit_complete_large): an SVC_OP_OUTCOME_BYTES op whose len word exceeds SVC_BYTES_MAX is the HEAD of
+// svc_span_conts(len) CONTINUATION slots that follow it in ring order, each holding the next SVC_PAYLOAD bytes of the segment.
+//   callers     claim the whole span with one fetch_add, publish the continuations (also as SVC_OP_OUTCOME_BYTES) and then the
+//               head; if any slot of it is not free, all of them go out as SVC_OP_SKIP;
+//   dispatcher  takes a span whole or not at all (svc_scan), marks its continuations in svc_desc.cont;
+//   kernel      stages a span's slots next to each other, so the segment is contiguous in shared memory.
+// A continuation is not an operation: nobody collects it, so whoever answers its batch (k_svc, svc_fail_ops) writes its answer
+// with SVC_COLLECTED already set.  Until then its slot is not free, so it is never rewritten before its bytes were pulled.
+#define SVC_SPAN_MAX (1u + (AGR_OUT_TICKET_MAX_BYTES - SVC_BYTES_MAX + SVC_PAYLOAD - 1u) / SVC_PAYLOAD)   // 33 slots
+static_assert(SVC_SPAN_MAX <= 128u / 2u, "a span of the longest segment must fit a batch that already holds other ops");
+// continuation slots of a head whose len word says len (a word beyond the longest segment counts as the longest)
+SVC_HD static inline uint32_t svc_span_conts(uint32_t len) {
+    if (len <= SVC_BYTES_MAX) return 0u;
+    if (len > AGR_OUT_TICKET_MAX_BYTES) len = AGR_OUT_TICKET_MAX_BYTES;
+    return (len - SVC_BYTES_MAX + SVC_PAYLOAD - 1u) / SVC_PAYLOAD;
+}
+// the segment length of an op with `conts` continuations staged: its len word clamped to what those slots hold.  The dispatcher
+// reserves the batch's bytes and the kernel places them with this one function, so the two totals cannot differ.
+SVC_HD static inline uint32_t svc_span_len(uint32_t len, uint32_t conts) {
+    const uint32_t cap = SVC_BYTES_MAX + conts * SVC_PAYLOAD;
+    return len < cap ? len : cap;
+}
+// continuations that follow op in a batch of count ops (cont: svc_desc.cont, one bit per op)
+SVC_HD static inline uint32_t svc_conts_after(const uint32_t* cont, uint32_t op, uint32_t count) {
+    uint32_t k = 0;
+    while (op + 1u + k < count && ((cont[(op + 1u + k) >> 5] >> ((op + 1u + k) & 31u)) & 1u)) ++k;
+    return k;
+}
 
 // batch descriptor (256 B = 64 words), written by the dispatcher (host), polled by the kernel: sixteen lanes read 16 B each
 // in ONE poll; the kernel accepts it when the batch number matches and the check word agrees with the other 62 words (a poll
@@ -47,7 +82,8 @@ struct __attribute__((aligned(64))) svc_desc {
     uint64_t idx_base;
     uint64_t resp_base;                   // SVC_OP_OUTCOME_BYTES ops: physical offset of the batch's region of the response byte
                                           // slab (their 16 B-rounded segments in ring order), or SVC_NO_BYTES
-    uint64_t reserved[14];
+    uint32_t cont[SVC_MAX_OPS / 32];      // words 32..39: 1 bit per op, set for a span's continuation slots
+    uint64_t reserved[10];
     uint64_t check;                       // words 60..61: XOR of svc_mix_word over words 0..59 and 62..63
     uint64_t seq;                         // words 62..63: batch number; the kernel waits for desc[seq % SVC_DESCS].seq == seq
 };

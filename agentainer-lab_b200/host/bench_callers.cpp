@@ -9,8 +9,9 @@
 // With <bytes> = store | fused every StoreResponse keeps a response of 64 B of flattened headers plus <body> bytes of body
 // (requests.go:134-175): store = today's pattern, the completion (blocking call or ticket) and then agr_store_response;
 // fused = the bytes travel with the completion, agr_submit_complete_ex (tickets) or agr_complete_ex(n = 1) (blocking), and a
-// body above AGR_OUT_INLINE_BYTES falls back to the locked agr_complete_ex(n = 1).
-//   bench_callers <threads> <seconds> [device] [mint|hash] [agents] [inflight per thread, 0 = blocking calls] [none|store|fused] [body]
+// body above AGR_OUT_INLINE_BYTES falls back to the locked agr_complete_ex(n = 1); large = the same with
+// agr_submit_complete_large (blocking threads: it and agr_wait), which carries up to AGR_OUT_TICKET_MAX_BYTES in one ticket.
+//   bench_callers <threads> <seconds> [device] [mint|hash] [agents] [inflight per thread, 0 = blocking calls] [none|store|fused|large] [body]
 #include <atomic>
 #include <chrono>
 #include <cstdio>
@@ -36,7 +37,7 @@ int main(int argc, char** argv) {
     const bool mint = !(argc > 4 && strcmp(argv[4], "hash") == 0);
     const int n_agents = argc > 5 ? atoi(argv[5]) : 256;
     const int inflight = argc > 6 ? atoi(argv[6]) : 0;
-    const int bytes_mode = argc > 7 ? (strcmp(argv[7], "store") == 0 ? 1 : strcmp(argv[7], "fused") == 0 ? 2 : 0) : 0;
+    const int bytes_mode = argc > 7 ? (strcmp(argv[7], "store") == 0 ? 1 : strcmp(argv[7], "fused") == 0 ? 2 : strcmp(argv[7], "large") == 0 ? 3 : 0) : 0;
     const uint32_t body_len = argc > 8 ? (uint32_t)atoi(argv[8]) : 256u;
     static constexpr char kHdr[] = "Content-Type: application/json\nX-Trace-Id: 0123456789abcdef0123\n";
     static_assert(sizeof kHdr - 1 == 64, "64 B of headers");
@@ -45,12 +46,15 @@ int main(int argc, char** argv) {
     std::string seg = hdr; seg.append(body.begin(), body.end());
     const uint64_t seg_off[2] = {0, seg.size()};
     const uint32_t seg_hlen = (uint32_t)hdr.size();
-    const bool inline_fits = seg.size() <= AGR_OUT_INLINE_BYTES;
+    const bool ticket_fits = seg.size() <= (bytes_mode == 3 ? AGR_OUT_TICKET_MAX_BYTES : AGR_OUT_INLINE_BYTES);
     agr_config cfg; memset(&cfg, 0, sizeof cfg);
     cfg.device = device;
     cfg.slab_rows = 1ull << 26;                         // 64 Mi rows = 32 GiB of slab (~43 GB with the per-row arrays)
     cfg.max_agents = 1024; cfg.max_batch = 1u << 16; cfg.log_entries = cfg.slab_rows;
     cfg.resp_bytes = bytes_mode ? 8ull << 30 : 1 << 20;               // append-only: room for a few seconds of stored responses
+    if (bytes_mode == 3) {                              // bodies up to 16 KB arrive at GB/s: half the rows, four times the bytes
+        cfg.slab_rows = 1ull << 25; cfg.log_entries = cfg.slab_rows; cfg.resp_bytes = 32ull << 30;
+    }
     cfg.flags = AGR_CFG_PERSISTENCE | AGR_CFG_COMBINE | (mint ? AGR_CFG_MINT_IDS : 0u);
     agr_handle* h = nullptr;
     if (agr_create(&cfg, &h) < 0) { fprintf(stderr, "agr_create: %s\n", agr_last_error()); return 2; }
@@ -76,7 +80,8 @@ int main(int argc, char** argv) {
         if (inflight > 0) {
             // Tickets are answered in hand-over order (batch by batch), so the thread keeps its requests in a FIFO and polls only
             // the OLDEST one: a poll that says "not yet" means nothing younger is ready either.
-            struct flight { int stage; agr_ticket t; std::chrono::steady_clock::time_point t0; uint32_t rec; uint8_t rid[16]; };
+            // stage 0: ingest ticket, 1: completion ticket, 2 (large): a completion waiting to be handed over again
+            struct flight { int stage; agr_ticket t; std::chrono::steady_clock::time_point t0; uint32_t rec; uint8_t rid[16]; agr_outcome o; };
             std::vector<flight> q((size_t)inflight);
             size_t head = 0, count = 0;                                   // FIFO over q: [head, head + count)
             auto push = [&](const flight& f) { q[(head + count) % q.size()] = f; count++; };
@@ -95,6 +100,14 @@ int main(int argc, char** argv) {
                 uint32_t reaped = 0;
                 while (count && reaped < 64) {
                     flight f = q[head];
+                    if (f.stage == 2) {
+                        head = (head + 1) % q.size(); count--;
+                        const int rc2 = agr_submit_complete_large(h, &f.o, (const uint8_t*)hdr.data(), seg_hlen, body.data(), body_len, &f.t);
+                        if (rc2 < 0) { bad++; stop.store(true); break; }
+                        if (rc2 == AGR_EAGAIN) { push(f); break; }           // still no room: collect more first
+                        f.stage = 1; push(f); reaped++;
+                        continue;
+                    }
                     agr_result res;
                     const int rc = agr_poll(h, f.t, &res);
                     if (rc == AGR_EAGAIN) break;
@@ -105,7 +118,7 @@ int main(int argc, char** argv) {
                         agr_outcome o; memset(&o, 0, sizeof o);
                         memcpy(o.request_id, res.request_id, 16); memcpy(o.agent_id, recs[f.rec].agent_id, AGR_AGENT_ID_BYTES);
                         o.kind = AGR_OUT_RESPONSE; o.http_status = 200; o.seq = n;
-                        if (bytes_mode == 2 && !inline_fits) {                // too big for a ticket: the locked batch call, n = 1
+                        if (bytes_mode >= 2 && !ticket_fits) {                // too big for a ticket: the locked batch call, n = 1
                             int32_t r1 = -1;
                             if (agr_complete_ex(h, &o, 1, (const uint8_t*)seg.data(), seg_off, &seg_hlen, &r1) < 0 || r1 != 0) { bad++; stop.store(true); break; }
                             const auto t1 = std::chrono::steady_clock::now();
@@ -113,6 +126,16 @@ int main(int argc, char** argv) {
                             continue;
                         }
                         int rc2;
+                        if (bytes_mode == 3) {
+                            // a span needs up to 33 free slots in a row, and the thread's own uncollected tickets may be among
+                            // them: on AGR_EAGAIN collect first, as the header asks, and hand it over again when it comes round
+                            memcpy(&f.rid, o.request_id, 16); f.o = o;
+                            rc2 = agr_submit_complete_large(h, &o, (const uint8_t*)hdr.data(), seg_hlen, body.data(), body_len, &f.t);
+                            if (rc2 < 0) { bad++; stop.store(true); break; }
+                            f.stage = rc2 == AGR_EAGAIN ? 2 : 1;
+                            push(f);
+                            continue;
+                        }
                         // AGR_EAGAIN: the slot drawn still holds somebody's uncollected answer; the next draw is another slot
                         while ((rc2 = (bytes_mode == 2 ? agr_submit_complete_ex(h, &o, (const uint8_t*)hdr.data(), seg_hlen, body.data(), body_len, &f.t)
                                                        : agr_submit_complete(h, &o, &f.t))) == AGR_EAGAIN && !stop.load(std::memory_order_relaxed)) {}
@@ -130,7 +153,7 @@ int main(int argc, char** argv) {
                     }
                 }
             }
-            while (count) { agr_result res; agr_wait(h, q[head].t, &res); head = (head + 1) % q.size(); count--; }   // drain
+            while (count) { agr_result res; if (q[head].stage != 2) agr_wait(h, q[head].t, &res); head = (head + 1) % q.size(); count--; }   // drain
             total += n;
             return;
         }
@@ -145,7 +168,11 @@ int main(int argc, char** argv) {
             memcpy(o.request_id, id[0], 16); memcpy(o.agent_id, r.agent_id, AGR_AGENT_ID_BYTES);
             o.kind = AGR_OUT_RESPONSE; o.http_status = 200; o.seq = n + 1;
             int32_t res = -1;
-            if (bytes_mode == 2) {
+            if (bytes_mode == 3 && ticket_fits) {
+                agr_ticket tk; agr_result rr; int rc2;
+                while ((rc2 = agr_submit_complete_large(h, &o, (const uint8_t*)hdr.data(), seg_hlen, body.data(), body_len, &tk)) == AGR_EAGAIN) {}
+                if (rc2 < 0 || agr_wait(h, tk, &rr) < 0 || rr.result != 0) { bad++; break; }
+            } else if (bytes_mode >= 2) {
                 if (agr_complete_ex(h, &o, 1, (const uint8_t*)seg.data(), seg_off, &seg_hlen, &res) < 0 || res != 0) { bad++; break; }
             } else {
                 if (agr_complete(h, &o, 1, &res) < 0 || res != 0) { bad++; break; }
@@ -181,7 +208,7 @@ int main(int argc, char** argv) {
            "\"id_mode\": \"%s\", \"agents\": %d, \"inflight_per_thread\": %d, \"response_bytes\": \"%s\", \"hdr_bytes\": %u, \"body_bytes\": %u, \"errors\": %llu, \"stored\": %llu, \"completions\": %llu, \"host_cpus\": %u}\n",
            threads, secs, rt, rt / secs, 2.0 * rt / secs, pct(0.50), pct(0.99), all.size(),
            (unsigned long long)(s1.svc_batches - s0.svc_batches), (double)(s1.svc_ops - s0.svc_ops) / std::max<double>(1.0, (double)(s1.svc_batches - s0.svc_batches)),
-           mint ? "mint" : "hash", n_agents, inflight, bytes_mode == 0 ? "none" : bytes_mode == 1 ? "store" : "fused",
+           mint ? "mint" : "hash", n_agents, inflight, bytes_mode == 0 ? "none" : bytes_mode == 1 ? "store" : bytes_mode == 2 ? "fused" : "large",
            bytes_mode ? seg_hlen : 0u, bytes_mode ? body_len : 0u, (unsigned long long)bad.load(), (unsigned long long)s2.stored, (unsigned long long)s2.completions,
            std::thread::hardware_concurrency());
     agr_destroy(h);

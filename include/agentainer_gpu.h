@@ -262,10 +262,18 @@ int agr_submit_ingest(agr_handle* h, const agr_record* rec, agr_ticket* ticket);
 int agr_submit_complete(agr_handle* h, const agr_outcome* outcome, agr_ticket* ticket);
 /* agr_submit_complete with the outcome's bytes in the ticket (agr_complete_ex(n = 1) semantics): headers then body for a
  * response, the error text in body for an error (hdr_len 0).  hdr_len + body_len <= AGR_OUT_INLINE_BYTES, else AGR_EINVAL:
- * the caller then uses agr_complete_ex(n = 1).  The ticket's result is AGR_ENOSPC when the transition was applied but the
+ * the caller then uses agr_submit_complete_large, or agr_complete_ex(n = 1).  The ticket's result is AGR_ENOSPC when the transition was applied but the
  * bytes found no room in the response byte slab. */
 int agr_submit_complete_ex(agr_handle* h, const agr_outcome* outcome, const uint8_t* headers, uint32_t hdr_len,
                            const uint8_t* body, uint32_t body_len, agr_ticket* ticket);
+/* agr_submit_complete_ex for hdr_len + body_len <= AGR_OUT_TICKET_MAX_BYTES: a segment longer than AGR_OUT_INLINE_BYTES takes
+ * consecutive ring slots (one more per further 512 B), up to AGR_OUT_INLINE_BYTES it is one slot like agr_submit_complete_ex.
+ * Same results: AGR_EINVAL for NULL arguments, bytes on a kind other than AGR_OUT_RESPONSE / AGR_OUT_ERROR, a segment above
+ * the limit (agr_complete_ex(n = 1) takes those) or an engine without AGR_CFG_COMBINE; AGR_EAGAIN when a slot drawn still holds
+ * an uncollected answer; a ticket result of AGR_ENOSPC when the transition was applied but the bytes found no room. */
+int agr_submit_complete_large(agr_handle* h, const agr_outcome* outcome, const uint8_t* headers, uint32_t hdr_len,
+                              const uint8_t* body, uint32_t body_len, agr_ticket* ticket);
+#define AGR_OUT_TICKET_MAX_BYTES 16384u   /* largest segment agr_submit_complete_large carries (33 ring slots) */
 int agr_poll(agr_handle* h, agr_ticket ticket, agr_result* out);
 int agr_wait(agr_handle* h, agr_ticket ticket, agr_result* out);
 uint32_t agr_ring_capacity(void);
