@@ -72,7 +72,7 @@ ABI_SYMBOLS = [
     "agr_agent_hash", "agr_agent_shard", "agr_comm_unique_id", "agr_comm_init", "agr_ingest_sharded", "agr_complete_sharded", "agr_snapshot", "agr_restore", "agr_verify", "agr_store_response_body", "agr_get_response_body",
     "agr_store_response", "agr_store_error_text", "agr_get_record_json", "agr_pending_json", "agr_rows_json", "agr_expire", "agr_reclaim", "agr_set_agent_states", "agr_json_decode",
     "agr_submit_ingest", "agr_submit_complete", "agr_poll", "agr_wait", "agr_ring_capacity", "agr_ingest_sharded_rows", "agr_fill_rows", "agr_reclaim_async",
-    "agr_complete_ex", "agr_submit_complete_ex", "agr_submit_complete_large",
+    "agr_complete_ex", "agr_submit_complete_ex", "agr_submit_complete_large", "agr_debug_skip_arrivals",
 ]
 
 _lib = None
@@ -133,6 +133,7 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
         "agr_stream": (vp, [vp]),
         "agr_slab_ptr": (vp, [vp, u64]),
         "agr_debug_read": (i32, [vp, i32, u64, u32, vp]),
+        "agr_debug_skip_arrivals": (i32, [vp, u64]),
         "agr_op_time": (i32, [vp, i32, C.POINTER(C.c_double)]),
         "agr_kernel_time": (i32, [vp, C.POINTER(C.c_double), C.POINTER(u64)]),
         "agr_synth_agent_id": (i32, [C.POINTER(AgrSynth), u32, C.c_char_p]),
@@ -381,6 +382,10 @@ class Engine:
         out = np.zeros(n, dtype=verdict_dtype if sel == 4 else np.uint64 if sel in (3, 5, 6) else np.uint32)
         _check(self.lib, self.lib.agr_debug_read(self.h, sel, first_rid, n, _ptr(out)))
         return out
+
+    def skip_arrivals(self, n: int) -> None:
+        """Test only: move an empty ring's arrival counter forward by n (agr_debug_skip_arrivals)."""
+        _check(self.lib, self.lib.agr_debug_skip_arrivals(self.h, n))
 
     def slab_ptr(self, rid: int) -> int:
         return self.lib.agr_slab_ptr(self.h, rid) or 0

@@ -115,11 +115,16 @@ AGR_HD unsigned long long agr_fnv1a64(const char* s, uint32_t maxlen) {
 
 // ---- engine-minted request ids (AGR_CFG_MINT_IDS).  The reference mints uuid.New() INSIDE StoreRequest
 // (internal/requests/requests.go:87); in this mode the engine does the same, and the id is an exact invertible
-// function of where the record lives: lo = a keyed 60-bit permutation of (row | shard << 40 | generation << 48) laid
-// around the UUIDv4 version nibble, hi = a keyed hash of the same value with the RFC 4122 variant bits.  A lookup
-// decodes the row from lo and accepts only if mint(row) equals ALL 128 presented bits — an exact membership test with
-// no table, no atomics and no random DRAM traffic on the ingest path.
+// function of where the record lives: lo = a keyed 60-bit permutation of x = (row mod 2^40 | shard << 40 |
+// (generation ^ row >> 40) << 48) laid around the UUIDv4 version nibble, hi = a keyed hash of x with the RFC 4122 variant
+// bits.  The row is the arrival number: a ring keeps counting past 2^40, and its 2^40-row periods are told apart by the
+// 12-bit generation field, so ids are unique for AGR_ROW_LIMIT = 2^52 arrivals (rows below 2^40 keep the ids they always
+// had).  A lookup decodes the row's low 40 bits from lo, places them in the live window (agr_unmint_in_window) and accepts
+// only if mint(row) equals ALL 128 presented bits — an exact membership test with no table, no atomics and no random DRAM
+// traffic on the ingest path.
 #define AGR_MINT_M60 ((1ULL << 60) - 1)
+#define AGR_MINT_ROW_M40 ((1ULL << 40) - 1)
+#define AGR_ROW_LIMIT (1ULL << 52)      // rows (arrival numbers) an engine hands out: agr_reserve_rows stops there
 #define AGR_MINT_C1 0x9e3779b97f4a7c15ULL
 #define AGR_MINT_C2 0xbf58476d1ce4e5b9ULL
 AGR_HD unsigned long long agr_inv_odd(unsigned long long c) {           // inverse mod 2^64 (Newton), masked by callers
@@ -143,19 +148,35 @@ AGR_HD unsigned long long agr_perm60_inv(unsigned long long y) {
 }
 AGR_HD void agr_mint_id(unsigned long long rid, uint32_t shard, uint32_t gen, unsigned long long secret,
                         unsigned long long& lo, unsigned long long& hi) {
-    const unsigned long long x = (rid & 0xffffffffffULL) | ((unsigned long long)(shard & 0xffu) << 40) | ((unsigned long long)(gen & 0xfffu) << 48);
+    const unsigned long long x = (rid & AGR_MINT_ROW_M40) | ((unsigned long long)(shard & 0xffu) << 40) |
+                                 (((unsigned long long)gen ^ (rid >> 40)) & 0xfffULL) << 48;
     const unsigned long long y = agr_perm60(x ^ (secret & AGR_MINT_M60));
     lo = (y & ((1ULL << 52) - 1)) | (0x4ULL << 52) | ((y >> 52) << 56);
     hi = agr_fmix64((x + 0x632be59bd9b4e019ULL) * 0x9e3779b97f4a7c15ULL ^ (secret >> 7));
     hi = (hi & ~0xc0ULL) | 0x80ULL;
 }
-// decodes (rid, shard, gen) from lo; returns false if lo cannot be a minted id.  Callers must still compare
-// agr_mint_id(rid, shard, gen) with the presented (lo, hi).
-AGR_HD bool agr_unmint_id(unsigned long long lo, unsigned long long secret, unsigned long long& rid, uint32_t& shard, uint32_t& gen) {
+// decodes x's fields from lo: the row's low 40 bits, the shard and the generation field (gen ^ row >> 40); returns false if
+// lo cannot be a minted id.  Callers must still place the row (agr_unmint_in_window) and compare all 128 bits.
+AGR_HD bool agr_unmint_id(unsigned long long lo, unsigned long long secret, unsigned long long& rid40, uint32_t& shard, uint32_t& genf) {
     if (((lo >> 52) & 0xfULL) != 0x4ULL) return false;
     const unsigned long long y = (lo & ((1ULL << 52) - 1)) | ((lo >> 56) << 52);
     const unsigned long long x = agr_perm60_inv(y) ^ (secret & AGR_MINT_M60);
-    rid = x & 0xffffffffffULL; shard = (uint32_t)((x >> 40) & 0xffu); gen = (uint32_t)((x >> 48) & 0xfffu);
+    rid40 = x & AGR_MINT_ROW_M40; shard = (uint32_t)((x >> 40) & 0xffu); genf = (uint32_t)((x >> 48) & 0xfffu);
+    return true;
+}
+// The row of the live window [tail, head_l) an id was minted for, or false.  The window is narrower than 2^40 rows (it never
+// exceeds slab_rows), so at most one row in it has the decoded low 40 bits: row = tail + ((rid40 - tail) mod 2^40).  That row
+// must lie below head_l, carry this shard and the generation field its period gives, and mint to all 128 presented bits.
+AGR_HD bool agr_unmint_in_window(unsigned long long lo, unsigned long long hi, unsigned long long secret, uint32_t shard, uint32_t gen,
+                                 unsigned long long tail, unsigned long long head_l, unsigned long long& row) {
+    unsigned long long r40; uint32_t s, g;
+    if (!agr_unmint_id(lo, secret, r40, s, g)) return false;
+    const unsigned long long a = tail + ((r40 - tail) & AGR_MINT_ROW_M40);
+    if (a >= head_l || s != shard || g != (uint32_t)((gen ^ (a >> 40)) & 0xfffULL)) return false;   // not a live row
+    unsigned long long mlo, mhi;
+    agr_mint_id(a, shard, gen, secret, mlo, mhi);
+    if (mlo != lo || mhi != hi) return false;
+    row = a;
     return true;
 }
 

@@ -68,16 +68,13 @@ __device__ __forceinline__ const uint8_t* rec_ptr(const agr_dev& d, uint32_t rid
 }
 
 // (agent slot is checked by the callers) request id -> row holding the record stored under it, or AGR_RID_NONE.
-// Hash mode: probe the dedupe index.  Mint mode: decode the row from the id and accept only an exact 128-bit match.
+// Hash mode: probe the dedupe index.  Mint mode: decode the row from the id relative to the live window and accept only an
+// exact 128-bit match (agr_unmint_in_window).
 __device__ __forceinline__ uint32_t lookup_rid(const agr_dev& d, unsigned long long lo, unsigned long long hi) {
     if ((lo | hi) == 0ULL) return AGR_RID_NONE;
     if (d.cfg_flags & AGR_CFG_MINT_IDS) {
-        unsigned long long rid; uint32_t shard, gen;
-        if (!agr_unmint_id(lo, d.id_secret, rid, shard, gen)) return AGR_RID_NONE;
-        if (rid < d.tail || rid >= d.head_l || shard != d.shard_id || gen != d.id_gen) return AGR_RID_NONE;   // not a live row
-        unsigned long long mlo, mhi;
-        agr_mint_id(rid, shard, gen, d.id_secret, mlo, mhi);
-        return (mlo == lo && mhi == hi) ? row_physical(d, rid) : AGR_RID_NONE;
+        unsigned long long rid;
+        return agr_unmint_in_window(lo, hi, d.id_secret, d.shard_id, d.id_gen, d.tail, d.head_l, rid) ? row_physical(d, rid) : AGR_RID_NONE;
     }
     const unsigned long long idx = table_find(d, lo, hi);
     if (idx == ~0ULL) return AGR_RID_NONE;

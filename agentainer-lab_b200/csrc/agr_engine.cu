@@ -226,10 +226,12 @@ static inline uint64_t phys_row(const agr_handle* h, uint64_t l) { return is_rin
 static inline uint64_t rows_span(const agr_handle* h) {       // physical rows that have ever been handed out
     return is_ring(h) ? std::min<uint64_t>(h->rows_used, h->cfg.slab_rows) : h->rows_used;
 }
+static inline void sync_svc_rows(agr_handle* h);
 static inline void sync_window(agr_handle* h) {               // the live window the kernels check decoded ids against
     h->d.tail = h->tail; h->d.head_l = h->rows_used;
     h->d.ring_rows = is_ring(h) ? (uint32_t)h->cfg.slab_rows : 0u;
     h->d.tail_phys = is_ring(h) ? (uint32_t)(h->tail % h->cfg.slab_rows) : 0u;
+    sync_svc_rows(h);
 }
 
 struct nccl_api {
@@ -297,6 +299,7 @@ struct svc_host {
     alignas(64) std::atomic<uint64_t> head{0};          // next ring slot to hand out (absolute number)
     alignas(64) std::atomic<uint32_t> waiters{0};       // callers blocked in svc_wait right now
     alignas(64) std::atomic<uint64_t> scanned{0};       // dispatcher: first slot whose ready word it has not consumed yet (>= taken)
+    std::atomic<uint64_t> rows_out{0};                  // = the handle's rows_used (sync_window): callers rebuild a row's high bits from it (svc_try)
     // ---- the dispatcher's own
     alignas(64) uint64_t taken = 0;                     // first slot not yet put into a batch
     uint64_t seq = 0;                                   // last batch number published
@@ -313,6 +316,11 @@ struct svc_host {
     alignas(64) std::mutex smu; std::condition_variable scv;   // the dispatcher sleeps here when the ring has been empty for a while
 };
 
+// (called under the handle mutex by every change of rows_used: reserve_rows_locked stores the new value before the dispatcher
+// publishes the batch whose answers name the rows)
+static inline void sync_svc_rows(agr_handle* h) {
+    if (h->svc) h->svc->rows_out.store(h->rows_used, std::memory_order_release);
+}
 
 static void svc_fail_ops(svc_host* s, uint64_t from, uint64_t to, int rc, bool records_only, const uint32_t* conts);
 // stops the resident kernel; the caller holds h->mu, so no new batch can be published meanwhile
@@ -594,8 +602,9 @@ static int svc_ingest(agr_handle* h, const agr_record* recs, uint32_t n, agr_ver
         if ((r.w0 & 0xffu) == 0u) rc = (int)r.w1;
         else {
             if (out) { memcpy(&out[i], &r.w0, 4); memcpy((uint8_t*)&out[i] + 4, &r.w1, 4); }
-            if (ids) svc_request_id(h, pos[i], r.rid, ids[i]);
-            if (i == 0 && first_rid) *first_rid = r.rid;
+            const uint64_t row = svc_row(s, r);
+            if (ids) svc_request_id(h, pos[i], row, ids[i]);
+            if (i == 0 && first_rid) *first_rid = row;
         }
         svc_release(s, pos[i]);
     }
@@ -938,6 +947,7 @@ static int reserve_rows_locked(agr_handle* h, uint32_t n, uint64_t* first) {
     const uint64_t at = h->rows_used % R;
     const uint64_t pad = (at + n > R) ? R - at : 0;
     if (h->rows_used + pad + n - h->tail > R) return fail(AGR_ENOSPC, "slab full: agr_expire + agr_reclaim release rows at the tail");
+    if (h->rows_used + pad + n > AGR_ROW_LIMIT) return fail(AGR_ENOSPC, "row ids exhausted: a shard hands out 2^52 rows (minted ids stay unique that long)");
     h->rows_used += pad;
     *first = h->rows_used;
     h->rows_used += n;
@@ -1142,7 +1152,7 @@ static int collect(agr_handle* h, agr_ticket ticket, const svc_answer& r, agr_re
         out->is_outcome = rec ? 0u : 1u;
         if (rec) {
             if ((r.w0 & 0xffu) == 0u) out->result = (int32_t)r.w1;
-            else { memcpy(&out->verdict, &r.w0, 4); memcpy((uint8_t*)&out->verdict + 4, &r.w1, 4); out->rid = r.rid; svc_request_id(h, t, r.rid, out->request_id); }
+            else { memcpy(&out->verdict, &r.w0, 4); memcpy((uint8_t*)&out->verdict + 4, &r.w1, 4); out->rid = svc_row(s, r); svc_request_id(h, t, out->rid, out->request_id); }
         } else out->result = (int32_t)r.w0;
     }
     svc_release(s, t);
@@ -2481,6 +2491,29 @@ int agr_debug_read(agr_handle* h, int which, uint64_t first_rid, uint32_t n, voi
         const unsigned long long v = rt_verdict(words[i]);
         memcpy((uint8_t*)out + (size_t)i * sizeof(agr_verdict), &v, sizeof v);
     }
+    return 0;
+}
+
+// Test-only: a ring engine whose window is empty moves its arrival counter forward by n, as if n records had arrived and been
+// expired and released.  Every logical cursor moves together; the chunks' time bounds become "unknown" as after a restore.
+int agr_debug_skip_arrivals(agr_handle* h, uint64_t n) {
+    if (!h) return fail(AGR_EINVAL, "NULL argument");
+    HLock lk(h);
+    CK(cudaSetDevice(h->device));
+    if (!is_ring(h)) return fail(AGR_EINVAL, "engine was not created with AGR_CFG_RING");
+    if (n > AGR_ROW_LIMIT - h->rows_used) return fail(AGR_EINVAL, "skip would pass the row id bound (2^52)");
+    if (h->tail != h->rows_used || !h->resv.empty() || h->reclaim_pending) return fail(AGR_EINVAL, "window not empty: expire and reclaim every row first");
+    unsigned long long lens[2];
+    CK(cudaMemcpyAsync(lens, h->d.log_len, sizeof lens, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    if (lens[0] || lens[1]) return fail(AGR_EINVAL, "window not empty: the completed / failed logs hold entries");
+    if (n == 0) return 0;
+    h->rows_used += n; h->tail += n; h->released_total += n;
+    h->scan_lo = h->tail; h->sweep_clean = h->rows_used; h->reclaim_bound = h->tail;
+    h->d.idx_base = h->tail;
+    sync_window(h);                                          // agr_dev's window, and rows_out for the single-request callers
+    CK(cudaMemsetAsync(h->d.cmin, 0, (size_t)(h->cfg.slab_rows / AGR_CHUNK_ROWS + 2) * 8, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
     return 0;
 }
 

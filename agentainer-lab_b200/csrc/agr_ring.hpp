@@ -5,6 +5,7 @@
 // H provides:
 //   svc_res* res; uint8_t* payload; std::atomic<uint32_t>* ready;          pinned, device-mapped in the engine
 //   std::atomic<uint64_t> head, scanned; std::atomic<uint32_t> waiters; uint32_t spin_cpus;
+//   std::atomic<uint64_t> rows_out                                          only where svc_row is used (callers that collect records)
 //   std::atomic<bool> sleeping; std::mutex smu; std::condition_variable scv;   the dispatcher's sleep / wake-up
 // The dispatcher (engine) or its stand-in (simulation) consumes ready words in slot order, keeps `scanned` = first slot whose
 // ready word it has not consumed, and sees to it that every consumed operation other than SVC_OP_SKIP gets its 16-byte answer.
@@ -155,7 +156,15 @@ static bool svc_submit_outcome_span(H* s, const void* outcome, uint32_t hdr_len,
     *abs = a0;
     return ok;
 }
-struct svc_answer { uint32_t w0, w1; uint64_t rid; };
+// A record's answer carries the low 48 bits of its row (arrival number): svc_answer.rid.  svc_row rebuilds the full row from H's
+// rows_out (rows handed out so far, stored with release by the dispatcher before it publishes the batch that names the row).
+// Read after the answer's tag was acquired (svc_try / svc_wait), rows_out is above the row and less than 2^48 rows above it, so
+// the row is the one below rows_out with those low bits.  Only callers that collect records need rows_out in H.
+static inline uint64_t svc_full_row(uint64_t low48, uint64_t rows_out) {
+    const uint64_t top = rows_out - 1u;
+    return top - ((top - low48) & ((1ULL << 48) - 1u));
+}
+struct svc_answer { uint32_t w0, w1; uint64_t rid; };   // rid: low 48 bits of a record's row (svc_row gives all of it)
 template <class H>
 static inline bool svc_try(H* s, uint64_t a, svc_answer* out) {
     const svc_res* r = s->res + (a & (SVC_SLOTS - 1u));
@@ -163,6 +172,11 @@ static inline bool svc_try(H* s, uint64_t a, svc_answer* out) {
     if ((w3 >> 16) != svc_tag(a)) return false;
     out->w0 = svc_word(r, 0); out->w1 = svc_word(r, 1); out->rid = (uint64_t)svc_word(r, 2) | ((uint64_t)(w3 & 0xffffu) << 32);
     return true;
+}
+// the full row of a collected record's answer (call after svc_try / svc_wait returned it, before svc_release)
+template <class H>
+static inline uint64_t svc_row(H* s, const svc_answer& r) {
+    return svc_full_row(r.rid, s->rows_out.load(std::memory_order_acquire));
 }
 // Blocking wait.  The first spin_cpus waiters spin (the answer is ~20 us away); waiters beyond that many would only burn the
 // process's CPU allowance against each other (a container with a CPU quota throttles ALL its threads once it is spent), so they

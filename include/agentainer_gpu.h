@@ -495,6 +495,12 @@ int agr_complete_sharded(agr_handle* h, const agr_outcome* outs, uint32_t n, int
 enum { AGR_DBG_STATE = 0, AGR_DBG_ROUTE = 1, AGR_DBG_AUX = 2, AGR_DBG_CKSUM = 3, AGR_DBG_VERDICT = 4, AGR_DBG_MTIME = 5,
        AGR_DBG_CMIN = 6 };
 int agr_debug_read(agr_handle* h, int which, uint64_t first_rid, uint32_t n, void* out);
+/* TEST ONLY: puts an AGR_CFG_RING engine far along its arrival counter without ingesting.  The window must be empty (every row
+ * released: rows_tail == rows_used, no reserved row unfilled, empty completed / failed logs — what agr_expire + agr_reclaim leave
+ * when everything is due); the row ids then move forward by n as if n records had arrived, expired and been released.  Time
+ * bounds of the TTL sweep become unknown, as after agr_restore.  AGR_EINVAL on append-only engines, while anything is live, and
+ * when rows_used + n would pass 2^52 (row ids stop there: agr_reserve_rows returns AGR_ENOSPC). */
+int agr_debug_skip_arrivals(agr_handle* h, uint64_t n);
 
 /* -------------------------------------------------- synthetic stream (bench) */
 /* Counter-based generator of BASELINE.json's synthetic streams; integer-only, identical on host and device. */

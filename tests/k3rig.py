@@ -16,8 +16,15 @@ def agent_names(n):
 class Rig:
     """One engine, the restatement, and the records the test ingested (for the byte-for-byte compare)."""
 
-    def __init__(self, *, slab_rows, max_agents, flags=K.AGR_CFG_PERSISTENCE | K.AGR_CFG_MINT_IDS, keep_records=True, **kw):
+    def __init__(self, *, slab_rows, max_agents, flags=K.AGR_CFG_PERSISTENCE | K.AGR_CFG_MINT_IDS, keep_records=True, base=0,
+                 mint_ids=None, **kw):
         self.eng = A.Engine(device=0, slab_rows=slab_rows, max_agents=max_agents, flags=flags, **kw)
+        # base: the engine's arrival counter when the rig starts (agr_debug_skip_arrivals); the restatement and the kept records
+        # count rows from there.  mint_ids(first, n): where the ids of minted rows come from (default: the engine's agr_mint_ids)
+        self.base = base
+        if base:
+            self.eng.skip_arrivals(base)
+        self.mint_ids = mint_ids or self.eng.mint_ids
         self.ref = K3Ref()
         self.mint = bool(flags & K.AGR_CFG_MINT_IDS)
         self.names = []
@@ -62,11 +69,12 @@ class Rig:
         return recs
 
     def ingest(self, slots):
-        """One agr_ingest call; returns its first row."""
+        """One agr_ingest call; returns its first row (counted from base)."""
         slots = np.asarray(slots, dtype=np.int64)
         recs = self.records(slots)
         _, first = self.eng.ingest(recs, want_verdicts=False)
-        ids = self.eng.mint_ids(first, len(recs)) if self.mint else recs["request_id"]
+        ids = self.mint_ids(first, len(recs)) if self.mint else recs["request_id"]
+        first -= self.base
         self.ref.add_rows(first, slots, ids)
         self.keep_rows(first, recs)
         return first
@@ -120,7 +128,7 @@ class Rig:
         disp, recs = self.eng.replay_scan(with_records=with_records)
         rows, slots = self.ref.tick()
         assert len(disp) == len(rows), f"dispatched {len(disp)} rows, the reference {len(rows)}"
-        assert np.array_equal(disp["rid"].astype(np.int64), rows), "dispatch rows / order differ"
+        assert np.array_equal(disp["rid"].astype(np.int64) - self.base, rows), "dispatch rows / order differ"
         assert np.array_equal(disp["agent_slot"].astype(np.int64), slots)
         assert np.array_equal(disp["request_id"], self.ref.ids[rows])
         if with_records:

@@ -35,6 +35,19 @@ def test_ring_protocol_on_cpu(ring_sim, args):
         assert d["eagain"] > 0 and d["skipped_slots"] >= d["eagain"], d      # the oversubscribed runs really went through the no-op path
 
 
+@pytest.mark.parametrize("base", [2**48 - 40000, 2**48 - 1, 2**49 + 2**48 - 3000, 2**52 - 2**48 // 2 - 17])
+def test_answers_name_full_rows_past_2_48(ring_sim, base):
+    """A record's answer carries 48 bits of its row; svc_try rebuilds the rest from the rows handed out so far.  The stand-in hands
+    out row base + slot number, so the rows of these runs cross a multiple of 2^48; every caller checks the full row it got."""
+    for args in (("1", "3", "512", "20000", "0", str(base)), ("1", "8", "4096", "6000", "20", str(base))):
+        res = subprocess.run([ring_sim, *args], capture_output=True, text=True, timeout=300)
+        d = json.loads(res.stdout.strip().splitlines()[-1])
+        assert res.returncode == 0 and d["ok"] and d["wrong_rows"] == 0, (d, res.stderr[-1000:])
+        assert d["row_base"] == base and d["last_row"] >= base + d["operations"] - 1
+        if base % 2**48 > 2**48 - 40000:
+            assert d["last_row"] // 2**48 > base // 2**48          # the run really crossed the edge
+
+
 def test_ring_protocol_under_thread_sanitizer(tmp_path):
     """The same simulation built with -fsanitize=thread: the shipped caller-side code (acquire / release accesses on the answer
     cells, release / acquire on the ready words, streaming stores behind an sfence) has no data race ThreadSanitizer can see."""
