@@ -73,6 +73,7 @@ ABI_SYMBOLS = [
     "agr_store_response", "agr_store_error_text", "agr_get_record_json", "agr_pending_json", "agr_rows_json", "agr_expire", "agr_reclaim", "agr_set_agent_states", "agr_json_decode",
     "agr_submit_ingest", "agr_submit_complete", "agr_poll", "agr_wait", "agr_ring_capacity", "agr_ingest_sharded_rows", "agr_fill_rows", "agr_reclaim_async",
     "agr_complete_ex", "agr_submit_complete_ex", "agr_submit_complete_large", "agr_debug_skip_arrivals",
+    "agr_debug_world", "agr_debug_k4", "agr_debug_exchange_begin", "agr_debug_exchange_end",
 ]
 
 _lib = None
@@ -134,6 +135,10 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
         "agr_slab_ptr": (vp, [vp, u64]),
         "agr_debug_read": (i32, [vp, i32, u64, u32, vp]),
         "agr_debug_skip_arrivals": (i32, [vp, u64]),
+        "agr_debug_world": (i32, [vp, i32, i32]),
+        "agr_debug_k4": (i32, [vp, vp, u32, u32, u32, i32, vp, vp, u32, vp, vp, vp, vp, vp, vp, vp, vp]),
+        "agr_debug_exchange_begin": (i32, [vp, u64, u32, vp, C.POINTER(AgrExchangeInfo)]),
+        "agr_debug_exchange_end": (i32, [vp, vp, vp]),
         "agr_op_time": (i32, [vp, i32, C.POINTER(C.c_double)]),
         "agr_kernel_time": (i32, [vp, C.POINTER(C.c_double), C.POINTER(u64)]),
         "agr_synth_agent_id": (i32, [C.POINTER(AgrSynth), u32, C.c_char_p]),
@@ -378,14 +383,50 @@ class Engine:
 
     def debug_read(self, which: str, first_rid: int, n: int) -> np.ndarray:
         """Per-row words of logical rows [first_rid, +n); "cmin": the TTL sweep's time bounds of physical chunks [first_rid, +n)."""
-        sel = {"state": 0, "route": 1, "aux": 2, "cksum": 3, "verdict": 4, "mtime": 5, "cmin": 6}[which]
-        out = np.zeros(n, dtype=verdict_dtype if sel == 4 else np.uint64 if sel in (3, 5, 6) else np.uint32)
+        sel = {"state": 0, "route": 1, "aux": 2, "cksum": 3, "verdict": 4, "mtime": 5, "cmin": 6, "index_used": 7}[which]
+        out = np.zeros(n, dtype=verdict_dtype if sel == 4 else np.uint64 if sel in (3, 5, 6, 7) else np.uint32)
         _check(self.lib, self.lib.agr_debug_read(self.h, sel, first_rid, n, _ptr(out)))
         return out
 
     def skip_arrivals(self, n: int) -> None:
         """Test only: move an empty ring's arrival counter forward by n (agr_debug_skip_arrivals)."""
         _check(self.lib, self.lib.agr_debug_skip_arrivals(self.h, n))
+
+    def debug_world(self, rank: int, world: int) -> None:
+        """Test only: shard `rank` of `world` without a communicator (agr_debug_world)."""
+        _check(self.lib, self.lib.agr_debug_world(self.h, rank, world))
+
+    def debug_k4(self, items: np.ndarray, agent_off: int, inplace: bool, local_res: np.ndarray, remote_res: np.ndarray) -> dict:
+        """Test only: K4 over `items` (a structured or (n, item_bytes) uint8 array) as shard rank of world (agr_debug_k4)."""
+        items = np.ascontiguousarray(items)
+        n, ib = len(items), (items.dtype.itemsize if items.dtype.names else items.shape[1])
+        raw = items.view(np.uint8).reshape(n, ib)
+        rb = local_res.dtype.itemsize
+        lres, rres = np.ascontiguousarray(local_res), np.ascontiguousarray(remote_res)
+        assert remote_res.dtype == local_res.dtype and len(lres) >= n and len(rres) >= n
+        m = max(n, 1)
+        r = dict(owner=np.zeros(m, np.uint8), perm=np.zeros(m, np.uint32), gtotal=np.zeros(32, np.uint32), goff=np.zeros(33, np.uint32),
+                 send=np.zeros((m, ib), np.uint8), local=np.zeros((m, ib), np.uint8), items=np.zeros((m, ib), np.uint8),
+                 res=np.zeros(m, local_res.dtype))
+        src = raw if n else np.zeros((1, ib), np.uint8)
+        _check(self.lib, self.lib.agr_debug_k4(self.h, _ptr(src), n, ib, agent_off, int(inplace), _ptr(lres if n else r["res"]),
+                                               _ptr(rres if n else r["res"]), rb, _ptr(r["owner"]), _ptr(r["perm"]), _ptr(r["gtotal"]),
+                                               _ptr(r["goff"]), _ptr(r["send"]), _ptr(r["local"]), _ptr(r["items"]), _ptr(r["res"])))
+        return {k: (v[:n] if k not in ("gtotal", "goff") else v) for k, v in r.items()}
+
+    def debug_exchange_begin(self, first_rid: int, n: int):
+        """Test only: agr_debug_exchange_begin; returns (the records owned by peers, owner-major, exchange info)."""
+        send = np.zeros(max(n, 1), dtype=record_dtype)
+        info = AgrExchangeInfo()
+        _check(self.lib, self.lib.agr_debug_exchange_begin(self.h, first_rid, n, _ptr(send), C.byref(info)))
+        return send[: info.n_sent].copy(), info
+
+    def debug_exchange_end(self, back: np.ndarray, n: int) -> np.ndarray:
+        """Test only: agr_debug_exchange_end with the owners' verdicts of the shipped records (in send order)."""
+        back = np.ascontiguousarray(back, dtype=verdict_dtype)
+        out = np.zeros(max(n, 1), dtype=verdict_dtype)
+        _check(self.lib, self.lib.agr_debug_exchange_end(self.h, _ptr(back) if len(back) else None, _ptr(out)))
+        return out[:n]
 
     def slab_ptr(self, rid: int) -> int:
         return self.lib.agr_slab_ptr(self.h, rid) or 0

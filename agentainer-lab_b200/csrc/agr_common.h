@@ -69,8 +69,8 @@ AGR_HD uint32_t rt_flags(uint32_t r) { return r >> RT_FLAG_SHIFT; }
 
 #define AGR_RID_NONE 0xffffffffu
 #define AGR_CFGI_SPLIT_INDEX 0x10000u   // internal cfg_flags bit: K1 runs as stream kernel + k1_index kernel
-#define AGR_CFGI_HOLES 0x20000u         // internal cfg_flags bit (set per launch by the exchange path): rows whose record carries
-#define AGR_FI_HOLE 0x80000000u         // AGR_FI_HOLE in its flags were emptied by K4 (shipped to their owner shard) and are skipped
+#define AGR_CFGI_HOLES 0x20000u         // internal cfg_flags bit (set per launch by the exchange path): rows of the batch that K4
+                                        // shipped to their owner shard (agr_dev::xowner) are skipped
 
 // ---- dedupe-index slot.  key == 0 means empty (a UUIDv4 is never all-zero); inv_rid = ~rid so that a zeroed
 // slot is "no rid yet" and atomicMax keeps the LOWEST rid (arrival order wins among duplicate ids).

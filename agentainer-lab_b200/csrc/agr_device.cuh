@@ -135,20 +135,27 @@ __device__ __forceinline__ void agent_resolve(const agr_dev& d, ag_probe p, cons
 // decided here and nothing is left to the post pass:
 //   - a target that arrived BEFORE this batch: its route and state words are final (two 4-byte loads);
 //   - an earlier target of the SAME batch: it is stored, with this row's slot, exactly when its agent id equals this row's (slots
-//     are never reused, so equal slots mean equal ids), persistence is on and it is neither replay-flagged, a hole, nor too long
+//     are never reused, so equal slots mean equal ids), persistence is on and it is neither replay-flagged nor too long
 //     for its row.  Its header bytes 32..83 are loaded instead of its words, which this launch may not have written yet;
 //   - any other row (this one, a later one) is not a dedupe hit.
+// (An earlier row of the same agent is owned by the same shard, so it is never a hole of an exchange batch.)
 // The loads are issued here and consumed by k1_finish, one tile later.  Without `decide`, or with caller-supplied ids, every
 // tracked replay is left to the post pass.
+// bi: the row's index in its batch.  In an exchange batch (AGR_CFGI_HOLES) a row whose record K4 shipped to its owner shard
+// (xowner[bi] != shard_id) is a hole: it is neither stored nor indexed here, and it gets no verdict.  The caller's flags word
+// plays no part in that.
+__device__ __forceinline__ bool k1_is_hole(const agr_dev& d, const uint32_t bi) {
+    return (d.cfg_flags & AGR_CFGI_HOLES) && __ldg(d.xowner + bi) != d.shard_id;
+}
 __device__ __forceinline__ void k1_begin(const agr_dev& d, const ag_probe& ap, const uint4& h0, const uint4& h1, const uint4& h2, const uint4& h3,
                                          const uint4& h4, const uint32_t body_len, const uint32_t payload_cap, const bool decide,
-                                         const unsigned long long first_log, const unsigned long long my_log, k1_ctx& c) {
+                                         const unsigned long long first_log, const unsigned long long my_log, const uint32_t bi, k1_ctx& c) {
     c.id_lo = pack64(h0.x, h0.y); c.id_hi = pack64(h0.z, h0.w);
     c.replay = (h4.z & AGR_F_REPLAY) != 0;                                                // server.go:506
-    c.hole = (d.cfg_flags & AGR_CFGI_HOLES) && (h4.z & AGR_FI_HOLE);                       // row emptied by the exchange (K4)
+    c.hole = k1_is_hole(d, bi);                                                           // row emptied by the exchange (K4)
     agent_resolve(d, ap, h2, h3, c.slot, c.astatus);                                      // server.go:498
     const bool found = c.slot != RT_SLOT_NONE && c.astatus != AG_STATUS_REMOVED;
-    c.want_store = found && (d.cfg_flags & AGR_CFG_PERSISTENCE) && !c.replay;             // server.go:508
+    c.want_store = found && (d.cfg_flags & AGR_CFG_PERSISTENCE) && !c.replay && !c.hole;  // server.go:508
     c.bad = c.want_store && ((unsigned long long)(h4.w & 0xffffu) + (h4.w >> 16) + body_len > payload_cap);
     // split mode: the insert is done by k1_index after the stream kernel; the row is provisionally "stored"
     // mint mode: the id is a function of the row, nothing to insert; the caller's request_id is ignored
@@ -237,7 +244,6 @@ __device__ __forceinline__ k1_result k1_finish(const agr_dev& d, uint32_t rid, c
                 const uint4 x1 = make_uint4(c.t_agent1.x ^ c.r_agent1.x, c.t_agent1.y ^ c.r_agent1.y, c.t_agent1.z ^ c.r_agent1.z, c.t_agent1.w ^ c.r_agent1.w);
                 const bool same_agent = (x0.x | x0.y | x0.z | x0.w | x1.x | x1.y | x1.z | x1.w) == 0u;
                 const bool stored = (d.cfg_flags & AGR_CFG_PERSISTENCE) && !(c.t_flags & AGR_F_REPLAY) &&
-                                    !((d.cfg_flags & AGR_CFGI_HOLES) && (c.t_flags & AGR_FI_HOLE)) &&
                                     (unsigned long long)(c.t_lens & 0xffffu) + (c.t_lens >> 16) + c.t_body <= AGR_REC - AGR_OFF_PAYLOAD;
                 if (same_agent && stored) { vflags |= AGR_VF_KNOWN; lc[C_DEDUPE_HITS]++; }
             } else if (c.known == 2u) {

@@ -177,7 +177,7 @@ k1_ingest_tma(const __grid_constant__ CUtensorMap tmap, const agr_dev d, const u
         }
         // this tile: agent loads have landed by now; classify and put the index CAS in flight.  pcx is dead here
         // (just consumed), so the CAS writes straight into the loop-carried registers.
-        if (valid) k1_begin(d, ap, h0, h1, h2, h3, h4, h5.x, AGR_REC - AGR_OFF_PAYLOAD, MINT, first_log, first_log + i, pcx);
+        if (valid) k1_begin(d, ap, h0, h1, h2, h3, h4, h5.x, AGR_REC - AGR_OFF_PAYLOAD, MINT, first_log, first_log + i, i, pcx);
         ph1 = h1; ph5y = h5.y; prid = rid; pvalid = valid; ptile = tile;
         if (s == STAGES - 1) phase ^= 1u;
     }

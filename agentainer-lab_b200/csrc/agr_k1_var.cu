@@ -161,7 +161,7 @@ k1_ingest_var(const agr_dev d, const uint8_t* __restrict__ blob, const uint32_t*
         auto decide = [&](uint32_t r, const uint4& h0, const uint4& h1, const uint4& h2, const uint4& h3, const uint4& h4, const uint4& h5) {
             const uint32_t rid = first_rid + a + r;
             k1_ctx cx;
-            k1_begin(d, k1_agent_issue(d, h2, h3), h0, h1, h2, h3, h4, h5.x, (so[r + 1] - so[r]) - AGR_OFF_PAYLOAD, false, 0ULL, 0ULL, cx);
+            k1_begin(d, k1_agent_issue(d, h2, h3), h0, h1, h2, h3, h4, h5.x, (so[r + 1] - so[r]) - AGR_OFF_PAYLOAD, false, 0ULL, 0ULL, a + r, cx);
             const k1_result res = k1_finish(d, rid, h1, h5, cx, lc);
             k1v_note_time(d, rid, res.state, h4);
             d.state[rid] = res.state;
@@ -291,7 +291,7 @@ k1_ingest_var_lsu(const agr_dev d, const uint8_t* __restrict__ blob, const uint3
                             h4 = ldg_nc_v4(gp + 64), h5 = ldg_nc_v4(gp + 80);
                 const uint32_t rid = first_rid + a + r;
                 k1_ctx cx;
-                k1_begin(d, k1_agent_issue(d, h2, h3), h0, h1, h2, h3, h4, h5.x, (so[r + 1] - so[r]) - AGR_OFF_PAYLOAD, false, 0ULL, 0ULL, cx);
+                k1_begin(d, k1_agent_issue(d, h2, h3), h0, h1, h2, h3, h4, h5.x, (so[r + 1] - so[r]) - AGR_OFF_PAYLOAD, false, 0ULL, 0ULL, a + r, cx);
                 const k1_result res = k1_finish(d, rid, h1, h5, cx, lc);
                 k1v_note_time(d, rid, res.state, h4);
                 d.state[rid] = res.state;

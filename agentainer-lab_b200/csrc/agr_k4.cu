@@ -73,8 +73,6 @@ __global__ void __launch_bounds__(256) k4_pass(const agr_k4_params p) {
                 const uint8_t* s = p.items + (size_t)si * p.item_bytes;
                 for (uint32_t c = lane; c < chunks; c += 32)
                     *reinterpret_cast<uint4*>(dst + c * 16) = __ldcg(reinterpret_cast<const uint4*>(s + c * 16));
-                // the row it came from is now empty: K1 skips rows whose record carries AGR_FI_HOLE (k1_begin)
-                if (p.inplace && lane == 0) *reinterpret_cast<uint32_t*>(p.items_rw + (size_t)si * p.item_bytes + AGR_OFF_FLAGS) |= AGR_FI_HOLE;
             }
         }
     }

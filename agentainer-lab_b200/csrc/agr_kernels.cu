@@ -40,7 +40,7 @@ __global__ void __launch_bounds__(WARPS * 32) k1_ingest_v0(const agr_dev d, cons
         // ---- long-latency chain first: agent probe -> classification -> first index CAS in flight
         const ag_probe ap = k1_agent_issue(d, h2, h3);
         k1_ctx cx;
-        if (valid) k1_begin(d, ap, h0, h1, h2, h3, h4, h5.x, AGR_REC - AGR_OFF_PAYLOAD, false, 0ULL, 0ULL, cx);
+        if (valid) k1_begin(d, ap, h0, h1, h2, h3, h4, h5.x, AGR_REC - AGR_OFF_PAYLOAD, false, 0ULL, 0ULL, i, cx);
         // ---- pass 2 (pure streaming, independent of the decision chain): payload checksum
         uint32_t c0 = 0, c1 = 0;
         {

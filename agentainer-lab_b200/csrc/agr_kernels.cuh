@@ -58,6 +58,7 @@ struct agr_dev {
     uint32_t ring_rows;        // 0 = append-only slab
     uint32_t tail_phys;        // tail % ring_rows
     uint32_t cfg_flags;
+    const uint8_t* xowner;     // exchange batch (AGR_CFGI_HOLES): K4's owner shard of each of its rows; rows owned by a peer are holes
 };
 
 // single-key lookup descriptor (agr_get_record & co.: the host resolves agent_id -> slot)
@@ -172,7 +173,7 @@ struct agr_k4_params {
     uint8_t* local_dst;        // where this shard's own items go (final slab rows / local op array)
     uint8_t* send_dst;         // owner-major send buffer (peer segments are shipped as they lie)
     uint32_t inplace;          // 1: items are slab rows already in their final place: own items are not moved, peers' items are
-    uint8_t* items_rw;         //    copied to the (peers-only) send buffer and their rows marked empty (AGR_FI_HOLE)
+                               //    copied to the (peers-only) send buffer; their rows are left as they are (K1 skips them by owner)
 };
 void agr_launch_k4_count(const agr_k4_params& p, cudaStream_t st);
 void agr_launch_k4_scatter(const agr_k4_params& p, cudaStream_t st);

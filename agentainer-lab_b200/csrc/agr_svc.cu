@@ -220,7 +220,7 @@ k_svc(const agr_dev d0, const svc_dev v, const agr_k2_scratch k2, const unsigned
             const uint4 h0 = lds_v4(hp), h1 = lds_v4(hp + 16), h2 = lds_v4(hp + 32), h3 = lds_v4(hp + 48), h4 = lds_v4(hp + 64), h5 = lds_v4(hp + 80);
             const uint32_t rid = D.first_p + wt;
             k1_ctx cx;
-            k1_begin(d, k1_agent_issue(d, h2, h3), h0, h1, h2, h3, h4, h5.x, AGR_REC - AGR_OFF_PAYLOAD, false, 0ULL, 0ULL, cx);
+            k1_begin(d, k1_agent_issue(d, h2, h3), h0, h1, h2, h3, h4, h5.x, AGR_REC - AGR_OFF_PAYLOAD, false, 0ULL, 0ULL, wt, cx);
             const k1_result r = k1_finish(d, rid, h1, h5, cx, lc);
             d.state[rid] = r.state;
             d.route[rid] = r.route;

@@ -464,7 +464,7 @@ void* agr_slab_ptr(agr_handle* h, uint64_t rid); /* device address of a slab row
  * the host when it parses /agent/{id} (server.go:494-495) and needs no collective.  Records that reach a non-owner shard
  * (BASELINE config 4: replay-flagged requests re-injected through another shard's proxy) are routed here:
  * the batch is DMA'd straight into its slab rows; K4 bins it by owner there, copies only the records owned by a PEER into the
- * send buffer (their rows are marked empty) and ONE grouped ncclSend/ncclRecv all-to-all over NVLink ships every peer segment
+ * send buffer (their rows stay as they are and K1 skips them) and ONE grouped ncclSend/ncclRecv all-to-all over NVLink ships every peer segment
  * into rows reserved at its owner; K1 runs over the own rows while the exchange is in flight and over the received rows after
  * it, and the verdicts travel back the same way and are restored to the caller's order.
  * NCCL is loaded at run time (libnccl.so.2); without it agr_comm_init fails with AGR_ECOMM.  Collective: every rank of
@@ -491,9 +491,10 @@ int agr_complete_sharded(agr_handle* h, const agr_outcome* outs, uint32_t n, int
  * 2 aux (u32), 3 checksum (u64), 4 verdict (agr_verdict: what agr_ingest_rows returned for the row), 5 mtime (u64: the
  * last-SET time K2 wrote, or — rings — K1; 0 = the TTL sweep takes the record's created_at).  6 cmin (u64) is per physical
  * 4096-row chunk instead: first_rid is a chunk index and first_rid + n <= slab_rows / 4096 + 1; the value is a lower bound of
- * the last-SET times of the chunk's stored rows (0 = unknown, ~0 = no stored row).  out must hold n elements of that width. */
+ * the last-SET times of the chunk's stored rows (0 = unknown, ~0 = no stored row).  7 index used (u64, first_rid 0, n 1): how many
+ * slots of the dedupe index hold an id (hash-id mode).  out must hold n elements of that width. */
 enum { AGR_DBG_STATE = 0, AGR_DBG_ROUTE = 1, AGR_DBG_AUX = 2, AGR_DBG_CKSUM = 3, AGR_DBG_VERDICT = 4, AGR_DBG_MTIME = 5,
-       AGR_DBG_CMIN = 6 };
+       AGR_DBG_CMIN = 6, AGR_DBG_INDEX_USED = 7 };
 int agr_debug_read(agr_handle* h, int which, uint64_t first_rid, uint32_t n, void* out);
 /* TEST ONLY: puts an AGR_CFG_RING engine far along its arrival counter without ingesting.  The window must be empty (every row
  * released: rows_tail == rows_used, no reserved row unfilled, empty completed / failed logs — what agr_expire + agr_reclaim leave
@@ -501,6 +502,25 @@ int agr_debug_read(agr_handle* h, int which, uint64_t first_rid, uint32_t n, voi
  * bounds of the TTL sweep become unknown, as after agr_restore.  AGR_EINVAL on append-only engines, while anything is live, and
  * when rows_used + n would pass 2^52 (row ids stop there: agr_reserve_rows returns AGR_ENOSPC). */
 int agr_debug_skip_arrivals(agr_handle* h, uint64_t n);
+/* TEST ONLY: the stages of the multi-GPU exchange on one device, without a communicator.
+ * agr_debug_world: everything agr_comm_init does except creating the communicator: the handle becomes shard `rank` of `world`
+ * (minted ids carry the rank) and gets the exchange's scratch.  AGR_EINVAL on a handle that has a communicator.
+ * agr_debug_k4: K4 (count + scan + scatter + unpermute, set up as the exchange sets them up) over n items of item_bytes (48..512, a
+ * multiple of 16) whose 32 B agent id lies at agent_off.  inplace != 0: the form the records take (own items stay, the send
+ * buffer holds the peers' items only); 0: the outcomes' form (own items to a local buffer, every owner in the send buffer).
+ * Returns the owner and owner-major position of every item, gtotal[world] and goff[world + 1], the send and local buffers (n items
+ * each, zero where K4 wrote nothing), the items after the pass, and the unpermuted results (res_bytes 4 or 8) of local_res (by
+ * item in place, by local position otherwise) and remote_res (by owner-major position), n of each.
+ * agr_debug_exchange_begin / _end: agr_ingest_sharded_rows split at its two all-to-alls.  Begin bins rows [first_rid, +n) in
+ * place, runs K1 over the own rows (the peers' rows are holes) and copies the records owned by peers, owner-major (the order of
+ * info->sent_to), to send_out; nothing is received.  End takes the owners' verdicts of those records in the same order and
+ * returns all n verdicts in the caller's order. */
+int agr_debug_world(agr_handle* h, int rank, int world);
+int agr_debug_k4(agr_handle* h, const void* items, uint32_t n, uint32_t item_bytes, uint32_t agent_off, int inplace,
+                 const void* local_res, const void* remote_res, uint32_t res_bytes, uint8_t* owner, uint32_t* perm, uint32_t* gtotal,
+                 uint32_t* goff, void* send_out, void* local_out, void* items_out, void* res_out);
+int agr_debug_exchange_begin(agr_handle* h, uint64_t first_rid, uint32_t n, agr_record* send_out, agr_exchange_info* info);
+int agr_debug_exchange_end(agr_handle* h, const agr_verdict* back, agr_verdict* out);
 
 /* -------------------------------------------------- synthetic stream (bench) */
 /* Counter-based generator of BASELINE.json's synthetic streams; integer-only, identical on host and device. */

@@ -25,7 +25,7 @@ def test_every_declared_symbol_is_exported(lib):
     for s in syms:
         assert hasattr(lib, s), f"{s} declared in the header but not exported"
     assert sorted(A.ABI_SYMBOLS) == syms
-    assert len(syms) == 67 and "agr_debug_skip_arrivals" in syms
+    assert len(syms) == 71 and "agr_debug_skip_arrivals" in syms and "agr_debug_k4" in syms
 
 
 def test_header_constants_match_python():
@@ -80,6 +80,8 @@ def test_null_arguments_are_rejected(lib):
     assert lib.agr_replay_scan(None, None, None, 0, C.byref(n)) == K.AGR_EINVAL
     assert lib.agr_create(None, None) == K.AGR_EINVAL
     assert lib.agr_debug_skip_arrivals(None, C.c_uint64(1)) == K.AGR_EINVAL
+    assert lib.agr_debug_world(None, 0, 2) == K.AGR_EINVAL
+    assert lib.agr_debug_exchange_end(None, None, None) == K.AGR_EINVAL
 
 
 def test_ctypes_structs_match_the_c_header(tmp_path):
