@@ -36,7 +36,6 @@ static_assert(sizeof(agr_record) == 512, "agr_record must be 512 B");
 static_assert(sizeof(agr_outcome) == 64, "agr_outcome must be 64 B");
 static_assert(sizeof(agr_dispatch) == 32, "agr_dispatch must be 32 B");
 static_assert(sizeof(agr_verdict) == 8, "agr_verdict must be 8 B");
-static_assert(sizeof(agr_verdict) == 8, "agr_verdict must be 8 B");
 static_assert(sizeof(agr_slot) == 32, "agr_slot must be 32 B");
 static_assert(sizeof(agr_agent_key) == 48, "agr_agent_key must be 48 B");
 static_assert(sizeof(agr_dop) == 32, "agr_dop must be 32 B");
@@ -58,6 +57,13 @@ struct exchange_plan {
     agr_k4_params p{};
     uint32_t G = 1, me = 0, scnt[32], rcnt[32], soff[33], roff[33], n_local = 0, n_recv = 0;
     uint32_t recv_res_base = 0;      // index of the first received item's result in the result array
+};
+
+// grow-only scratch: a buffer and the element count it was allocated with (regrow sets both)
+template <typename T>
+struct scratch {
+    T* p = nullptr;
+    size_t cap = 0;
 };
 
 struct agr_handle {
@@ -99,22 +105,20 @@ struct agr_handle {
     agr_outcome* h_outs = nullptr;             // pinned [max_batch]
     agr_outcome* d_outs = nullptr;             // [max_batch]
     int32_t* h_results = nullptr;              // pinned [max_batch]
-    agr_k2_scratch k2{}; uint32_t k2_cap = 0;   // K2 scratch sized for k2_cap outcomes
+    agr_k2_scratch k2{};
     uint32_t* d_hrid = nullptr;                // rows found by the single-key resolve (k_resolve)
     uint32_t* h_k2flag = nullptr;              // pinned: k2_append's overflow flag of the last batch
     agr_dop* d_ops = nullptr;
     std::vector<std::pair<uint64_t, uint64_t>> resv;   // rows handed out by agr_reserve_rows and not ingested yet: [first, end)
     // K3
-    uint32_t* d_matrix = nullptr; size_t matrix_entries = 0;
-    uint32_t* d_cta_matrix = nullptr; size_t cta_matrix_entries = 0;
-    uint32_t* d_selmask = nullptr; size_t selmask_words = 0;   // one selection bit per scanned item (k3_mark -> k3_place)
+    scratch<uint32_t> d_matrix, d_cta_matrix;
+    scratch<uint32_t> d_selmask;               // one selection bit per scanned item (k3_mark -> k3_place)
     uint32_t* d_gtotal = nullptr; uint32_t* d_goff = nullptr;
-    uint32_t* d_out_rid = nullptr; uint32_t* d_out_slot = nullptr; uint32_t out_cap = 0;
+    scratch<uint32_t> d_out_rid, d_out_slot;
     uint32_t* d_min_inq = nullptr;
-    uint8_t* d_gather = nullptr; size_t gather_bytes = 0;
-    uint8_t* h_gather = nullptr; size_t h_gather_bytes = 0;
+    scratch<uint8_t> d_gather, h_gather;       // (h_gather pinned)
     uint32_t* h_small = nullptr;               // pinned scratch (>= 64 words)
-    unsigned long long* d_cdf = nullptr; uint32_t cdf_n = 0;
+    scratch<unsigned long long> d_cdf;
     // launch accounting
     uint64_t k1_launches = 0, k2_launches = 0, k3_launches = 0, k4_launches = 0;
     uint64_t replay_scans = 0, replay_dispatched = 0;
@@ -129,10 +133,10 @@ struct agr_handle {
     // agr_complete_ex staging, allocated on first use: per-op offsets / slab places / header lengths, and the batch's bytes
     unsigned long long *h_boff = nullptr, *d_boff = nullptr, *h_bdst = nullptr, *d_bdst = nullptr;
     uint32_t *h_bhlen = nullptr, *d_bhlen = nullptr;
-    uint8_t *h_bsrc = nullptr, *d_bsrc = nullptr; size_t h_bsrc_cap = 0, d_bsrc_cap = 0;
+    scratch<uint8_t> h_bsrc, d_bsrc;           // (h_bsrc pinned)
     // K5 (JSON wire form) scratch
-    uint32_t* d_jlen = nullptr; unsigned long long* d_joff = nullptr; unsigned long long* d_jchunk = nullptr; uint32_t j_cap = 0;
-    uint8_t* d_json = nullptr; uint64_t json_cap = 0;
+    scratch<uint32_t> d_jlen; scratch<unsigned long long> d_joff, d_jchunk;
+    scratch<uint8_t> d_json;
     uint64_t k5_launches = 0;
     uint64_t expired_total = 0;                // records dropped by agr_expire so far
     // single-request front end (AGR_CFG_COMBINE): pinned op ring + dispatcher thread + resident service kernel (agr_svc.h)
@@ -142,8 +146,7 @@ struct agr_handle {
     uint64_t vtail = 0;                        // ring: logical offset of the first byte that has not been released
     uint32_t* d_voffsets = nullptr; uint32_t* d_tile_first = nullptr;   // per-batch offsets [max_batch+1], tile index
     uint32_t* h_voffsets = nullptr;
-    uint32_t* d_lens = nullptr; unsigned long long* d_goffs = nullptr;  // gather scratch [out_cap]
-    uint32_t lens_cap = 0;
+    scratch<uint32_t> d_lens; scratch<unsigned long long> d_goffs;      // gather scratch
     // multi-GPU exchange (K4)
     ncclComm_t comm = nullptr; int rank = 0, world = 1;
     uint8_t* d_stage = nullptr;                // incoming batch before binning [max_batch * 512]
@@ -172,23 +175,6 @@ static int dev_alloc(agr_handle* h, T** p, size_t count, bool zero) {
     *p = (T*)q;
     return 0;
 }
-// grow-only scratch: replaces *p by a larger buffer and releases the old one (every user of the old buffer has been
-// synchronised by then: the callers hold the handle mutex and the previous operation ended with a stream sync)
-template <typename T>
-static int dev_regrow(agr_handle* h, T** p, size_t count, bool zero) {
-    T* old = *p;
-    int rc = dev_alloc(h, p, count, zero);
-    if (rc < 0) return rc;
-    if (old) {
-        cudaStreamSynchronize(h->stream);
-        auto it = std::find(h->dev_allocs.begin(), h->dev_allocs.end(), (void*)old);
-        if (it != h->dev_allocs.end()) h->dev_allocs.erase(it);
-        cudaFree(old);
-    }
-    return 0;
-}
-template <typename T>
-static int host_regrow(agr_handle* h, T** p, size_t count);
 template <typename T>
 static int host_alloc(agr_handle* h, T** p, size_t count) {
     void* q = nullptr;
@@ -198,20 +184,24 @@ static int host_alloc(agr_handle* h, T** p, size_t count) {
     *p = (T*)q;
     return 0;
 }
+#define TRY(x) do { int r_ = (x); if (r_ < 0) return r_; } while (0)
+// replaces s by a buffer of count elements (device memory, or pinned host memory) and releases the old one (every user of
+// the old buffer has been synchronised by then: the callers hold the handle mutex and the previous operation ended with a
+// stream sync)
 template <typename T>
-static int host_regrow(agr_handle* h, T** p, size_t count) {
-    T* old = *p;
-    int rc = host_alloc(h, p, count);
-    if (rc < 0) return rc;
+static int regrow(agr_handle* h, scratch<T>& s, size_t count, bool pinned = false) {
+    T* old = s.p;
+    TRY(pinned ? host_alloc(h, &s.p, count) : dev_alloc(h, &s.p, count, false));
+    s.cap = count;
     if (old) {
         cudaStreamSynchronize(h->stream);
-        auto it = std::find(h->host_allocs.begin(), h->host_allocs.end(), (void*)old);
-        if (it != h->host_allocs.end()) h->host_allocs.erase(it);
-        cudaFreeHost(old);
+        std::vector<void*>& allocs = pinned ? h->host_allocs : h->dev_allocs;
+        auto it = std::find(allocs.begin(), allocs.end(), (void*)old);
+        if (it != allocs.end()) allocs.erase(it);
+        if (pinned) cudaFreeHost(old); else cudaFree(old);
     }
     return 0;
 }
-#define TRY(x) do { int r_ = (x); if (r_ < 0) return r_; } while (0)
 
 // K2 scratch for up to n outcomes per batch
 static int k2_scratch_alloc(agr_handle* h, size_t n) {
@@ -225,7 +215,6 @@ static int k2_scratch_alloc(agr_handle* h, size_t n) {
     h->k2.ticket = (uint32_t*)words;
     h->k2.overflow = h->k2.ticket + 1;
     h->k2.tiles = words + 1;
-    h->k2_cap = (uint32_t)n;
     return 0;
 }
 
@@ -276,6 +265,42 @@ static bool is_pinned(const void* p) {
     if (cudaPointerGetAttributes(&attr, p) == cudaSuccess) return attr.type == cudaMemoryTypeHost;
     cudaGetLastError();
     return false;
+}
+// host -> device on the compute stream: pinned caller memory is copied in place, pageable memory through the pinned stage
+static int h2d_staged(agr_handle* h, void* dst, const void* src, size_t bytes, void* stage) {
+    if (!is_pinned(src)) { memcpy(stage, src, bytes); src = stage; }
+    CK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, h->stream));
+    return 0;
+}
+// caller records -> slab rows on the copy stream: pinned (or registered) memory is DMA'd in place, pageable memory goes
+// through the two pinned bounce buffers; bk is the bounce buffer to use next, carried from one call to the next
+static int upload_rows(agr_handle* h, uint8_t* dst, const uint8_t* src, size_t bytes, bool src_pinned, int& bk) {
+    if (src_pinned) {
+        CK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, h->copy_stream));
+        return 0;
+    }
+    for (size_t o = 0; o < bytes;) {
+        const size_t piece = std::min(h->bounce_bytes, bytes - o);
+        CK(cudaEventSynchronize(h->bounce_ev[bk]));
+        par_memcpy(h->bounce[bk], src + o, piece);
+        CK(cudaMemcpyAsync(dst + o, h->bounce[bk], piece, cudaMemcpyHostToDevice, h->copy_stream));
+        CK(cudaEventRecord(h->bounce_ev[bk], h->copy_stream));
+        o += piece; bk ^= 1;
+    }
+    return 0;
+}
+// the lengths of the completed and failed logs
+static int read_log_lens(agr_handle* h, unsigned long long lens[2]) {
+    CK(cudaMemcpyAsync(lens, h->d.log_len, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    return 0;
+}
+// the last counter slot, used as an 8-byte scratch count by the maintenance kernels: zeroed before the launch, read after
+static unsigned long long* count_slot(agr_handle* h) { return (unsigned long long*)(h->d.ctr + C_NCTR - 1); }
+static int read_count(agr_handle* h, unsigned long long* v) {
+    CK(cudaMemcpyAsync(v, count_slot(h), 8, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    return 0;
 }
 
 static uint64_t next_pow2(uint64_t v) { uint64_t p = 1; while (p < v) p <<= 1; return p; }
@@ -915,8 +940,7 @@ int agr_drop_agent(agr_handle* h, const char* agent_id) {
     h->agent_status[slot] = AG_STATUS_REMOVED;
     TRY(push_agent_status(h, (uint32_t)slot, AG_STATUS_REMOVED));                          // DEL agent:{id} (agent.go:344)
     unsigned long long lens[2];
-    CK(cudaMemcpyAsync(lens, h->d.log_len, sizeof lens, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
+    TRY(read_log_lens(h, lens));
     agr_launch_drop_agent(h->d, (uint32_t)slot, rows_span(h), std::max(lens[0], lens[1]), h->stream);
     h->k3_launches += 2;
     CK(cudaGetLastError());
@@ -941,6 +965,15 @@ static void resv_remove(agr_handle* h, uint64_t first, uint64_t end) {
     }
     h->resv.swap(keep);
 }
+// The cursor rule of the three rings (slab rows, variable-length record bytes, response bytes), in logical units: a piece of
+// `need` units never wraps — if it does not fit before the end of the lap, the rest of the lap is skipped (*pad units) — and
+// it fits when everything from the tail to the end of the piece stays within one lap of `cap`.
+static bool ring_fits(uint64_t used, uint64_t tail, uint64_t cap, uint64_t need, uint64_t* pad) {
+    const uint64_t at = used % cap;
+    *pad = (at + need > cap) ? cap - at : 0;
+    return used + *pad + need - tail <= cap;
+}
+
 // ------------------------------------------------------------------------------------------ K1
 static int reserve_rows_locked(agr_handle* h, uint32_t n, uint64_t* first) {
     if (!is_ring(h)) {
@@ -950,12 +983,9 @@ static int reserve_rows_locked(agr_handle* h, uint32_t n, uint64_t* first) {
         sync_window(h);
         return 0;
     }
-    // ring: a batch never wraps — if it does not fit before the end of the slab, the rows up to the end are skipped
-    // (they stay "no record": released rows are zeroed), at most max_batch rows per lap
-    const uint64_t R = h->cfg.slab_rows;
-    const uint64_t at = h->rows_used % R;
-    const uint64_t pad = (at + n > R) ? R - at : 0;
-    if (h->rows_used + pad + n - h->tail > R) return fail(AGR_ENOSPC, "slab full: agr_expire + agr_reclaim release rows at the tail");
+    // ring: rows skipped at the end of a lap stay "no record" (released rows are zeroed), at most max_batch rows per lap
+    uint64_t pad = 0;
+    if (!ring_fits(h->rows_used, h->tail, h->cfg.slab_rows, n, &pad)) return fail(AGR_ENOSPC, "slab full: agr_expire + agr_reclaim release rows at the tail");
     if (h->rows_used + pad + n > AGR_ROW_LIMIT) return fail(AGR_ENOSPC, "row ids exhausted: a shard hands out 2^52 rows (minted ids stay unique that long)");
     h->rows_used += pad;
     *first = h->rows_used;
@@ -970,6 +1000,31 @@ static inline void flip_batch_words(agr_handle* h) {
     h->d.dupfix = h->dupfix_base + 4u * h->batch_phase;
     h->d.dupfix_next = h->dupfix_base + 4u * (h->batch_phase ^ 1u);
 }
+
+// AGR_CFG_TIMING: the next event pair of the ring agr_kernel_time reads (one pair per timed K1 launch)
+static int claim_k1_events(agr_handle* h, cudaEvent_t* e0, cudaEvent_t* e1) {
+    if (h->tev.empty()) {
+        h->tev.resize(2 * AGR_TIMING_RING);
+        for (auto& e : h->tev) CK(cudaEventCreate(&e));
+    }
+    const uint64_t k = h->tev_next++ % AGR_TIMING_RING;
+    *e0 = h->tev[2 * k]; *e1 = h->tev[2 * k + 1];
+    return 0;
+}
+// AGR_CFG_TIMING: events around the last launch group g (0 = K2, 1 = K3 select, 2 = K5 encode) that agr_op_time reads
+static int op_time_begin(agr_handle* h, int g) {
+    if (!(h->cfg.flags & AGR_CFG_TIMING)) return 0;
+    for (auto& e : h->op_ev) if (!e) CK(cudaEventCreate(&e));
+    CK(cudaEventRecord(h->op_ev[2 * g], h->stream));
+    return 0;
+}
+static int op_time_end(agr_handle* h, int g) {
+    if (!(h->cfg.flags & AGR_CFG_TIMING)) return 0;
+    CK(cudaEventRecord(h->op_ev[2 * g + 1], h->stream));
+    h->op_timed[g] = true;
+    return 0;
+}
+
 static int launch_k1_locked(agr_handle* h, uint64_t first, uint32_t n, agr_verdict* d_out, uint8_t* d_ids = nullptr) {
     sync_window(h);
     flip_batch_words(h);
@@ -977,14 +1032,7 @@ static int launch_k1_locked(agr_handle* h, uint64_t first, uint32_t n, agr_verdi
     // AGR_CFG_TIMING: events around the K1 kernel of every launch, or of every k-th one (k1_variant bits 16..23): an event record
     // is a stream operation of its own between two kernels, and two of them per step cost a back-to-back loop a few microseconds
     const uint32_t tstride = std::max<uint32_t>(1u, (h->cfg.k1_variant >> 16) & 0xffu);
-    if ((h->cfg.flags & AGR_CFG_TIMING) && (h->timing_calls++ % tstride) == 0) {
-        if (h->tev.empty()) {
-            h->tev.resize(2 * AGR_TIMING_RING);
-            for (auto& e : h->tev) CK(cudaEventCreate(&e));
-        }
-        const uint64_t k = h->tev_next++ % AGR_TIMING_RING;
-        e0 = h->tev[2 * k]; e1 = h->tev[2 * k + 1];
-    }
+    if ((h->cfg.flags & AGR_CFG_TIMING) && (h->timing_calls++ % tstride) == 0) TRY(claim_k1_events(h, &e0, &e1));
     h->k1_launches += agr_launch_k1(h->d, (uint32_t)phys_row(h, first), first, n, h->cfg.k1_variant,
                                     (h->cfg.k1_variant & 0xfu) != AGR_K1_LSU ? h->tmap : nullptr, h->sm_count, h->stream, e0, e1, d_out, d_ids);
     CK(cudaGetLastError());
@@ -1104,21 +1152,7 @@ static int ingest_ex_locked(agr_handle* h, const agr_record* recs, uint32_t n, a
     int bk = 0;
     for (uint32_t c = 0; c < nchunks; ++c) {
         const uint32_t off = c * AGR_INGEST_CHUNK, cn = std::min(AGR_INGEST_CHUNK, n - off);
-        uint8_t* dst = h->d.slab + (phys_row(h, first) + off) * AGR_REC;
-        const uint8_t* src = (const uint8_t*)(recs + off);
-        size_t bytes = (size_t)cn * AGR_REC;
-        if (src_pinned) {
-            CK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, h->copy_stream));
-        } else {
-            for (size_t o = 0; o < bytes;) {
-                size_t piece = std::min(h->bounce_bytes, bytes - o);
-                CK(cudaEventSynchronize(h->bounce_ev[bk]));
-                par_memcpy(h->bounce[bk], src + o, piece);
-                CK(cudaMemcpyAsync(dst + o, h->bounce[bk], piece, cudaMemcpyHostToDevice, h->copy_stream));
-                CK(cudaEventRecord(h->bounce_ev[bk], h->copy_stream));
-                o += piece; bk ^= 1;
-            }
-        }
+        TRY(upload_rows(h, h->d.slab + (phys_row(h, first) + off) * AGR_REC, (const uint8_t*)(recs + off), (size_t)cn * AGR_REC, src_pinned, bk));
         CK(cudaEventRecord(h->chunk_ev[c], h->copy_stream));
         CK(cudaStreamWaitEvent(h->stream, h->chunk_ev[c], 0));
         TRY(launch_k1_locked(h, first + off, cn, out ? h->d_verdicts + off : nullptr, ids ? h->d_ids + (size_t)off * 16 : nullptr));
@@ -1216,22 +1250,13 @@ static int complete_locked(agr_handle* h, const agr_outcome* outs, uint32_t n, i
     if (n > h->cfg.max_batch) return fail(AGR_EINVAL, "n exceeds max_batch");
     if (n == 0) return 0;
     // outcomes go to the device as they are; k2_prepare resolves the agent ids in the device agent table
-    if (is_pinned(outs)) {
-        CK(cudaMemcpyAsync(h->d_outs, outs, (size_t)n * sizeof(agr_outcome), cudaMemcpyHostToDevice, h->stream));
-    } else {
-        memcpy(h->h_outs, outs, (size_t)n * sizeof(agr_outcome));
-        CK(cudaMemcpyAsync(h->d_outs, h->h_outs, (size_t)n * sizeof(agr_outcome), cudaMemcpyHostToDevice, h->stream));
-    }
+    TRY(h2d_staged(h, h->d_outs, outs, (size_t)n * sizeof(agr_outcome), h->h_outs));
     sync_window(h);
-    const bool timing = (h->cfg.flags & AGR_CFG_TIMING) != 0;
-    if (timing) {
-        for (auto& e : h->op_ev) if (!e) CK(cudaEventCreate(&e));
-        CK(cudaEventRecord(h->op_ev[0], h->stream));
-    }
+    TRY(op_time_begin(h, 0));
     agr_launch_k2(h->d, h->d_outs, h->k2, n, h->stream, bytes);
     h->k2_launches += bytes ? 4 : 3;
     CK(cudaGetLastError());
-    if (timing) { CK(cudaEventRecord(h->op_ev[1], h->stream)); h->op_timed[0] = true; }
+    TRY(op_time_end(h, 0));
     CK(cudaMemcpyAsync(h->h_k2flag, h->k2.overflow, 4, cudaMemcpyDeviceToHost, h->stream));
     if (results) {
         CK(cudaMemcpyAsync(h->h_results, h->k2.results, (size_t)n * 4, cudaMemcpyDeviceToHost, h->stream));
@@ -1261,9 +1286,8 @@ static int resp_reserve_locked(agr_handle* h, uint64_t need, uint64_t len, unsig
         return 0;
     }
     if (need > h->resp_cap / 2) return fail(AGR_ENOSPC, "response larger than half the response slab");
-    const uint64_t at = h->resp_used % h->resp_cap;
-    const uint64_t pad = (at + need > h->resp_cap) ? h->resp_cap - at : 0;
-    if (h->resp_used + pad + need - h->resp_tail > h->resp_cap)
+    uint64_t pad = 0;
+    if (!ring_fits(h->resp_used, h->resp_tail, h->resp_cap, need, &pad))
         return fail(AGR_ENOSPC, "response slab full: agr_reclaim releases the bytes of released rows");
     h->resp_used += pad;
     *off = h->resp_used % h->resp_cap;                           // the rows keep PHYSICAL offsets
@@ -1313,27 +1337,21 @@ static int complete_ex_locked(agr_handle* h, const agr_outcome* outs, uint32_t n
     uint64_t run = 0;
     for (uint32_t i = 0; i < n; ++i) { h->h_bdst[i] = run; run += (offsets[i + 1] - offsets[i] + 15u) & ~15ull; }
     CK(cudaMemcpyAsync(h->d_bdst, h->h_bdst, (size_t)n * 8, cudaMemcpyHostToDevice, h->stream));
-    const void* offs = offsets;
-    if (!is_pinned(offsets)) { memcpy(h->h_boff, offsets, ((size_t)n + 1) * 8); offs = h->h_boff; }
-    CK(cudaMemcpyAsync(h->d_boff, offs, ((size_t)n + 1) * 8, cudaMemcpyHostToDevice, h->stream));
-    if (hdr_lens) {
-        const uint32_t* hl = hdr_lens;
-        if (!is_pinned(hdr_lens)) { memcpy(h->h_bhlen, hdr_lens, (size_t)n * 4); hl = h->h_bhlen; }
-        CK(cudaMemcpyAsync(h->d_bhlen, hl, (size_t)n * 4, cudaMemcpyHostToDevice, h->stream));
-    }
+    TRY(h2d_staged(h, h->d_boff, offsets, ((size_t)n + 1) * 8, h->h_boff));
+    if (hdr_lens) TRY(h2d_staged(h, h->d_bhlen, hdr_lens, (size_t)n * 4, h->h_bhlen));
     if (nbytes) {
         // (+ 16: warp_copy16 reads whole aligned 16-byte blocks around a segment)
-        if (nbytes + 16 > h->d_bsrc_cap) { TRY(dev_regrow(h, &h->d_bsrc, (size_t)(nbytes + nbytes / 4 + 16), false)); h->d_bsrc_cap = nbytes + nbytes / 4 + 16; }
+        if (nbytes + 16 > h->d_bsrc.cap) TRY(regrow(h, h->d_bsrc, (size_t)(nbytes + nbytes / 4 + 16)));
         const uint8_t* src = bytes + offsets[0];
         if (!is_pinned(src)) {
-            if (nbytes > h->h_bsrc_cap) { TRY(host_regrow(h, &h->h_bsrc, (size_t)(nbytes + nbytes / 4))); h->h_bsrc_cap = nbytes + nbytes / 4; }
-            par_memcpy(h->h_bsrc, src, nbytes);
-            src = h->h_bsrc;
+            if (nbytes > h->h_bsrc.cap) TRY(regrow(h, h->h_bsrc, (size_t)(nbytes + nbytes / 4), true));
+            par_memcpy(h->h_bsrc.p, src, nbytes);
+            src = h->h_bsrc.p;
         }
-        CK(cudaMemcpyAsync(h->d_bsrc, src, nbytes, cudaMemcpyHostToDevice, h->stream));
+        CK(cudaMemcpyAsync(h->d_bsrc.p, src, nbytes, cudaMemcpyHostToDevice, h->stream));
     }
     agr_k2_bytes b{};
-    b.src = h->d_bsrc; b.src_off = h->d_boff; b.dst = h->d_bdst; b.hlen = hdr_lens ? h->d_bhlen : nullptr; b.base = base;
+    b.src = h->d_bsrc.p; b.src_off = h->d_boff; b.dst = h->d_bdst; b.hlen = hdr_lens ? h->d_bhlen : nullptr; b.base = base;
     b.slab = h->d_resp; b.resp_off = h->d_resp_off; b.resp_len = h->d_resp_len; b.resp_hlen = h->d_resp_hlen;
     b.err_off = h->d_err_off; b.err_len = h->d_err_len;
     return complete_locked(h, outs, n, results, &b, false);
@@ -1395,17 +1413,34 @@ int agr_submit_complete_large(agr_handle* h, const agr_outcome* outcome, const u
 }
 
 // ------------------------------------------------------------------------------------------ K3
+// (each buffer of a group is checked against its own capacity: after a failed regrow of one of them the others keep theirs)
 static int ensure_out(agr_handle* h, uint32_t cap) {
-    if (cap <= h->out_cap) return 0;
     uint32_t ncap = std::max<uint32_t>(cap, 1024);
-    TRY(dev_regrow(h, &h->d_out_rid, ncap, false));
-    TRY(dev_regrow(h, &h->d_out_slot, ncap, false));
-    h->out_cap = ncap;
+    if (cap > h->d_out_rid.cap) TRY(regrow(h, h->d_out_rid, ncap));
+    if (cap > h->d_out_slot.cap) TRY(regrow(h, h->d_out_slot, ncap));
     return 0;
 }
 static int ensure_gather(agr_handle* h, size_t bytes) {
-    if (bytes > h->gather_bytes) { TRY(dev_regrow(h, &h->d_gather, bytes, false)); h->gather_bytes = bytes; }
-    if (bytes > h->h_gather_bytes) { TRY(host_regrow(h, &h->h_gather, bytes)); h->h_gather_bytes = bytes; }
+    if (bytes > h->d_gather.cap) TRY(regrow(h, h->d_gather, bytes));
+    if (bytes > h->h_gather.cap) TRY(regrow(h, h->h_gather, bytes, true));
+    return 0;
+}
+// copies out what the K3 gather makes of rows d_rids[0..n): dispatch entries, records and / or request ids (each skipped when
+// NULL), through one device buffer laid out in that order and one device -> host copy
+static int gather_rows_locked(agr_handle* h, const uint32_t* d_rids, uint32_t n, agr_dispatch* disp, agr_record* recs, uint8_t (*ids)[16]) {
+    const size_t disp_bytes = disp ? (size_t)n * 32 : 0, rec_bytes = recs ? (size_t)n * AGR_REC : 0, id_bytes = ids ? (size_t)n * 16 : 0;
+    const size_t bytes = disp_bytes + rec_bytes + id_bytes;
+    TRY(ensure_gather(h, bytes));
+    uint8_t* g = h->d_gather.p;
+    agr_launch_k3_gather(h->d, d_rids, nullptr, n, recs ? g + disp_bytes : nullptr, disp ? g : nullptr, ids ? g + disp_bytes + rec_bytes : nullptr,
+                         h->stream);
+    h->k3_launches += 1;
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(h->h_gather.p, g, bytes, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    if (disp) memcpy(disp, h->h_gather.p, disp_bytes);
+    if (recs) memcpy(recs, h->h_gather.p + disp_bytes, rec_bytes);
+    if (ids) memcpy(ids, h->h_gather.p + disp_bytes + rec_bytes, id_bytes);
     return 0;
 }
 
@@ -1427,27 +1462,23 @@ static int select_locked(agr_handle* h, int mode, uint32_t slot, const uint32_t*
     p.per_warp = (uint32_t)per;
     p.nwarps = (uint32_t)((items + per - 1) / per);
     size_t need = (size_t)p.nwarps * p.groups;
-    if (need > h->matrix_entries) { TRY(dev_regrow(h, &h->d_matrix, need, false)); h->matrix_entries = need; }
+    if (need > h->d_matrix.cap) TRY(regrow(h, h->d_matrix, need));
     const size_t need_cta = (size_t)((p.nwarps + 7) / 8) * p.groups;
-    if (need_cta > h->cta_matrix_entries) { TRY(dev_regrow(h, &h->d_cta_matrix, need_cta, false)); h->cta_matrix_entries = need_cta; }
-    p.cta_matrix = h->d_cta_matrix;
+    if (need_cta > h->d_cta_matrix.cap) TRY(regrow(h, h->d_cta_matrix, need_cta));
+    p.cta_matrix = h->d_cta_matrix.p;
     const size_t mask_words = (size_t)p.nwarps * (p.per_warp >> 5);
-    if (mask_words > h->selmask_words) { TRY(dev_regrow(h, &h->d_selmask, mask_words, false)); h->selmask_words = mask_words; }
-    p.selmask = h->d_selmask;
+    if (mask_words > h->d_selmask.cap) TRY(regrow(h, h->d_selmask, mask_words));
+    p.selmask = h->d_selmask.p;
     TRY(ensure_out(h, cap));
-    p.matrix = h->d_matrix; p.gtotal = h->d_gtotal; p.goff = h->d_goff;
-    p.out_rid = h->d_out_rid; p.out_slot = h->d_out_slot; p.cap = cap;
+    p.matrix = h->d_matrix.p; p.gtotal = h->d_gtotal; p.goff = h->d_goff;
+    p.out_rid = h->d_out_rid.p; p.out_slot = h->d_out_slot.p; p.cap = cap;
     p.min_inq = (mode == K3_TICK) ? h->d_min_inq : nullptr;
     if (mode == K3_TICK) CK(cudaMemsetAsync(h->d_min_inq, 0xff, 4, h->stream));
-    const bool timing = (h->cfg.flags & AGR_CFG_TIMING) != 0;
-    if (timing) {
-        for (auto& e : h->op_ev) if (!e) CK(cudaEventCreate(&e));
-        CK(cudaEventRecord(h->op_ev[2], h->stream));
-    }
+    TRY(op_time_begin(h, 1));
     agr_launch_k3_select(h->d, p, h->sm_count, h->stream);
     h->k3_launches += 4;
     CK(cudaGetLastError());
-    if (timing) { CK(cudaEventRecord(h->op_ev[3], h->stream)); h->op_timed[1] = true; }
+    TRY(op_time_end(h, 1));
     CK(cudaMemcpyAsync(h->h_small, h->d_goff + p.groups, 4, cudaMemcpyDeviceToHost, h->stream));
     if (mode == K3_TICK) CK(cudaMemcpyAsync(h->h_small + 1, h->d_min_inq, 4, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
@@ -1472,18 +1503,7 @@ int agr_replay_scan(agr_handle* h, agr_dispatch* out, agr_record* recs, uint32_t
     if (total > cap) return fail(AGR_ECAP, "dispatch array too small");
     h->replay_dispatched += total;
     if (total == 0 || !out) return 0;
-    size_t bytes = (size_t)total * 32 + (recs ? (size_t)total * AGR_REC : 0);
-    TRY(ensure_gather(h, bytes));
-    uint8_t* d_disp = h->d_gather;
-    uint8_t* d_recs = recs ? h->d_gather + (size_t)total * 32 : nullptr;
-    agr_launch_k3_gather(h->d, h->d_out_rid, nullptr, total, d_recs, d_disp, nullptr, h->stream);
-    h->k3_launches += 1;
-    CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(h->h_gather, h->d_gather, bytes, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    memcpy(out, h->h_gather, (size_t)total * 32);
-    if (recs) memcpy(recs, h->h_gather + (size_t)total * 32, (size_t)total * AGR_REC);
-    return 0;
+    return gather_rows_locked(h, h->d_out_rid.p, total, out, recs, nullptr);
 }
 
 int agr_pending(agr_handle* h, const char* agent_id, agr_record* out, uint32_t cap, uint32_t* n) {
@@ -1498,15 +1518,7 @@ int agr_pending(agr_handle* h, const char* agent_id, agr_record* out, uint32_t c
     *n = total;
     if (total > cap) return fail(AGR_ECAP, "output array too small");
     if (total == 0 || !out) return 0;
-    size_t bytes = (size_t)total * AGR_REC;
-    TRY(ensure_gather(h, bytes));
-    agr_launch_k3_gather(h->d, h->d_out_rid, nullptr, total, h->d_gather, nullptr, nullptr, h->stream);
-    h->k3_launches += 1;
-    CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(h->h_gather, h->d_gather, bytes, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    memcpy(out, h->h_gather, bytes);
-    return 0;
+    return gather_rows_locked(h, h->d_out_rid.p, total, nullptr, out, nullptr);
 }
 
 int agr_list(agr_handle* h, const char* agent_id, int which, uint8_t (*ids)[16], uint32_t cap, uint32_t* n) {
@@ -1523,8 +1535,7 @@ int agr_list(agr_handle* h, const char* agent_id, int which, uint8_t (*ids)[16],
         TRY(select_locked(h, K3_AGENT_PENDING_IDS, (uint32_t)slot, nullptr, h->expired_total ? h->tail : h->scan_lo, ingested_bound(h), cap, &total));
     } else {
         unsigned long long lens[2];
-        CK(cudaMemcpyAsync(lens, h->d.log_len, sizeof lens, cudaMemcpyDeviceToHost, h->stream));
-        CK(cudaStreamSynchronize(h->stream));
+        TRY(read_log_lens(h, lens));
         const uint32_t* log = (which == AGR_LIST_COMPLETED) ? h->d.completed_log : h->d.failed_log;
         uint64_t len = (which == AGR_LIST_COMPLETED) ? lens[0] : lens[1];
         TRY(select_locked(h, K3_LOG_AGENT, (uint32_t)slot, log, 0, len, cap, &total));
@@ -1532,22 +1543,13 @@ int agr_list(agr_handle* h, const char* agent_id, int which, uint8_t (*ids)[16],
     *n = total;
     if (total > cap) return fail(AGR_ECAP, "output array too small");
     if (total == 0 || !ids) return 0;
-    size_t bytes = (size_t)total * 16;
-    TRY(ensure_gather(h, bytes));
-    agr_launch_k3_gather(h->d, h->d_out_rid, nullptr, total, nullptr, nullptr, h->d_gather, h->stream);
-    h->k3_launches += 1;
-    CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(h->h_gather, h->d_gather, bytes, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    memcpy(ids, h->h_gather, bytes);
-    return 0;
+    return gather_rows_locked(h, h->d_out_rid.p, total, nullptr, nullptr, ids);
 }
 
-// storage.Get("agent:{a}:requests:{r}") (server.go:661-662): read-only resolve in the dedupe index, then a 1-row gather
-int agr_get_record(agr_handle* h, const char* agent_id, const uint8_t request_id[16], agr_record* out) {
-    if (!h || !agent_id || !request_id || !out) return fail(AGR_EINVAL, "NULL argument");
-    HLock lk(h);
-    CK(cudaSetDevice(h->device));
+// The read-only resolve of one request id in the dedupe index: its physical row is left in d_hrid[0] (and in *rid, unless
+// rid is NULL).  count_launch:
+// the resolve launch counts in k3_launches (agr_get_record_var's does not).
+static int resolve_one_locked(agr_handle* h, const char* agent_id, const uint8_t request_id[16], uint32_t* rid, bool count_launch) {
     int slot = agent_find(h, agent_id);
     if (slot < 0) return fail(AGR_ENOTFOUND, "request not found");
     agr_dop& op = h->h_ops[0];
@@ -1556,19 +1558,22 @@ int agr_get_record(agr_handle* h, const char* agent_id, const uint8_t request_id
     CK(cudaMemcpyAsync(h->d_ops, h->h_ops, sizeof(agr_dop), cudaMemcpyHostToDevice, h->stream));
     sync_window(h);
     agr_launch_resolve(h->d, h->d_ops, h->d_hrid, 1, h->stream);
-    h->k3_launches += 1;
+    if (count_launch) h->k3_launches += 1;
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(h->h_small, h->d_hrid, 4, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
     if (h->h_small[0] == AGR_RID_NONE) return fail(AGR_ENOTFOUND, "request not found");
-    TRY(ensure_gather(h, AGR_REC));
-    agr_launch_k3_gather(h->d, h->d_hrid, nullptr, 1, h->d_gather, nullptr, nullptr, h->stream);
-    h->k3_launches += 1;
-    CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(h->h_gather, h->d_gather, AGR_REC, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    memcpy(out, h->h_gather, AGR_REC);
+    if (rid) *rid = h->h_small[0];
     return 0;
+}
+
+// storage.Get("agent:{a}:requests:{r}") (server.go:661-662): read-only resolve in the dedupe index, then a 1-row gather
+int agr_get_record(agr_handle* h, const char* agent_id, const uint8_t request_id[16], agr_record* out) {
+    if (!h || !agent_id || !request_id || !out) return fail(AGR_EINVAL, "NULL argument");
+    HLock lk(h);
+    CK(cudaSetDevice(h->device));
+    TRY(resolve_one_locked(h, agent_id, request_id, nullptr, true));
+    return gather_rows_locked(h, h->d_hrid, 1, nullptr, out, nullptr);
 }
 
 // ------------------------------------------------------------------------------------------ variable-length records
@@ -1593,9 +1598,7 @@ int agr_ingest_var(agr_handle* h, const uint8_t* blob, const uint32_t* offsets, 
         if (h->vused + bytes > h->vcap) return fail(AGR_ENOSPC, "byte slab full");
     } else {                                                      // byte ring: a blob never wraps either
         if (bytes > h->vcap / 2) return fail(AGR_EINVAL, "batch larger than half the byte slab");
-        const uint64_t at = h->vused % h->vcap;
-        vpad = (at + bytes > h->vcap) ? h->vcap - at : 0;
-        if (h->vused + vpad + bytes - h->vtail > h->vcap) return fail(AGR_ENOSPC, "byte slab full: agr_expire + agr_reclaim release bytes at the tail");
+        if (!ring_fits(h->vused, h->vtail, h->vcap, bytes, &vpad)) return fail(AGR_ENOSPC, "byte slab full: agr_expire + agr_reclaim release bytes at the tail");
     }
     TRY(reserve_rows_locked(h, n, &first));
     if (first_rid) *first_rid = first;
@@ -1604,15 +1607,12 @@ int agr_ingest_var(agr_handle* h, const uint8_t* blob, const uint32_t* offsets, 
     h->vused += bytes;
     cudaStream_t st = h->stream;
     CK(cudaMemcpyAsync(h->d.slab + base, blob, bytes, cudaMemcpyHostToDevice, st));
-    if (is_pinned(offsets)) CK(cudaMemcpyAsync(h->d_voffsets, offsets, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, st));
-    else { memcpy(h->h_voffsets, offsets, ((size_t)n + 1) * 4); CK(cudaMemcpyAsync(h->d_voffsets, h->h_voffsets, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, st)); }
+    TRY(h2d_staged(h, h->d_voffsets, offsets, ((size_t)n + 1) * 4, h->h_voffsets));
     sync_window(h);
     flip_batch_words(h);
     cudaEvent_t e0 = nullptr, e1 = nullptr;
     if (h->cfg.flags & AGR_CFG_TIMING) {
-        if (h->tev.empty()) { h->tev.resize(2 * AGR_TIMING_RING); for (auto& e : h->tev) CK(cudaEventCreate(&e)); }
-        const uint64_t k = h->tev_next++ % AGR_TIMING_RING;
-        e0 = h->tev[2 * k]; e1 = h->tev[2 * k + 1];
+        TRY(claim_k1_events(h, &e0, &e1));
         CK(cudaEventRecord(e0, st));
     }
     CK(agr_launch_k1_var(h->d, h->d.slab + base, h->d_voffsets, n, bytes, h->d_tile_first, (uint32_t)phys_row(h, first), base, h->sm_count, st, h->cfg.k1_variant));
@@ -1630,15 +1630,12 @@ int agr_ingest_var(agr_handle* h, const uint8_t* blob, const uint32_t* offsets, 
 
 // packs the variable-length records of rows d_out_rid[0..total) into the caller's blob
 static int gather_var_locked(agr_handle* h, uint32_t total, uint8_t* blob, uint64_t blob_cap, uint64_t* offsets, uint64_t* blob_bytes) {
-    if (total > h->lens_cap) {
-        uint32_t ncap = std::max<uint32_t>(total, 1024);
-        TRY(dev_regrow(h, &h->d_lens, ncap, false));
-        TRY(dev_regrow(h, &h->d_goffs, (size_t)ncap + 1, false));
-        h->lens_cap = ncap;
-    }
-    agr_launch_var_lens(h->d, h->d_out_rid, total, h->d_lens, h->stream);
+    const uint32_t ncap = std::max<uint32_t>(total, 1024);
+    if (total > h->d_lens.cap) TRY(regrow(h, h->d_lens, ncap));
+    if ((size_t)total + 1 > h->d_goffs.cap) TRY(regrow(h, h->d_goffs, (size_t)ncap + 1));
+    agr_launch_var_lens(h->d, h->d_out_rid.p, total, h->d_lens.p, h->stream);
     std::vector<uint32_t> lens(total);
-    CK(cudaMemcpyAsync(lens.data(), h->d_lens, (size_t)total * 4, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaMemcpyAsync(lens.data(), h->d_lens.p, (size_t)total * 4, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
     std::vector<unsigned long long> offs((size_t)total + 1);
     offs[0] = 0;
@@ -1648,13 +1645,13 @@ static int gather_var_locked(agr_handle* h, uint32_t total, uint8_t* blob, uint6
     if (!blob) return 0;
     if (offs[total] > blob_cap) return fail(AGR_ECAP, "blob too small");
     TRY(ensure_gather(h, (size_t)offs[total] + 16));
-    CK(cudaMemcpyAsync(h->d_goffs, offs.data(), ((size_t)total + 1) * 8, cudaMemcpyHostToDevice, h->stream));
-    agr_launch_var_copy(h->d, h->d_out_rid, total, h->d_goffs, h->d_gather, h->stream);
+    CK(cudaMemcpyAsync(h->d_goffs.p, offs.data(), ((size_t)total + 1) * 8, cudaMemcpyHostToDevice, h->stream));
+    agr_launch_var_copy(h->d, h->d_out_rid.p, total, h->d_goffs.p, h->d_gather.p, h->stream);
     h->k3_launches += 2;
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(h->h_gather, h->d_gather, (size_t)offs[total], cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaMemcpyAsync(h->h_gather.p, h->d_gather.p, (size_t)offs[total], cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
-    memcpy(blob, h->h_gather, (size_t)offs[total]);
+    memcpy(blob, h->h_gather.p, (size_t)offs[total]);
     return 0;
 }
 
@@ -1672,15 +1669,7 @@ int agr_replay_scan_var(agr_handle* h, agr_dispatch* out, uint8_t* blob, uint64_
     if (total > cap) return fail(AGR_ECAP, "dispatch array too small");
     h->replay_dispatched += total;
     if (total == 0) return 0;
-    if (out) {
-        TRY(ensure_gather(h, (size_t)total * 32));
-        agr_launch_k3_gather(h->d, h->d_out_rid, nullptr, total, nullptr, h->d_gather, nullptr, h->stream);
-        h->k3_launches += 1;
-        CK(cudaGetLastError());
-        CK(cudaMemcpyAsync(h->h_gather, h->d_gather, (size_t)total * 32, cudaMemcpyDeviceToHost, h->stream));
-        CK(cudaStreamSynchronize(h->stream));
-        memcpy(out, h->h_gather, (size_t)total * 32);
-    }
+    if (out) TRY(gather_rows_locked(h, h->d_out_rid.p, total, out, nullptr, nullptr));
     return gather_var_locked(h, total, blob, blob_cap, offsets, blob_bytes);
 }
 
@@ -1689,19 +1678,9 @@ int agr_get_record_var(agr_handle* h, const char* agent_id, const uint8_t reques
     if (!(h->cfg.flags & AGR_CFG_VARLEN)) return fail(AGR_EINVAL, "engine was not created with AGR_CFG_VARLEN");
     HLock lk(h);
     CK(cudaSetDevice(h->device));
-    int slot = agent_find(h, agent_id);
-    if (slot < 0) return fail(AGR_ENOTFOUND, "request not found");
-    agr_dop& op = h->h_ops[0];
-    memcpy(&op.id_lo, request_id, 8); memcpy(&op.id_hi, request_id + 8, 8);
-    op.slot = (uint32_t)slot; op.http = 0; op.kind = 0; op.pad = 0; op.seq = 0;
-    CK(cudaMemcpyAsync(h->d_ops, h->h_ops, sizeof(agr_dop), cudaMemcpyHostToDevice, h->stream));
-    sync_window(h);
-    agr_launch_resolve(h->d, h->d_ops, h->d_hrid, 1, h->stream);
-    CK(cudaMemcpyAsync(h->h_small, h->d_hrid, 4, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    if (h->h_small[0] == AGR_RID_NONE) return fail(AGR_ENOTFOUND, "request not found");
+    TRY(resolve_one_locked(h, agent_id, request_id, nullptr, false));
     TRY(ensure_out(h, 1));
-    CK(cudaMemcpyAsync(h->d_out_rid, h->d_hrid, 4, cudaMemcpyDeviceToDevice, h->stream));
+    CK(cudaMemcpyAsync(h->d_out_rid.p, h->d_hrid, 4, cudaMemcpyDeviceToDevice, h->stream));
     uint64_t bytes = 0;
     std::vector<uint8_t> tmp(AGR_VAR_MAX_RECORD);
     uint64_t offs[2];
@@ -1713,28 +1692,11 @@ int agr_get_record_var(agr_handle* h, const char* agent_id, const uint8_t reques
 }
 
 // ------------------------------------------------------------------------------------------ stored responses
-static int resolve_one_locked(agr_handle* h, const char* agent_id, const uint8_t request_id[16], uint32_t* rid) {
-    int slot = agent_find(h, agent_id);
-    if (slot < 0) return fail(AGR_ENOTFOUND, "request not found");
-    agr_dop& op = h->h_ops[0];
-    memcpy(&op.id_lo, request_id, 8); memcpy(&op.id_hi, request_id + 8, 8);
-    op.slot = (uint32_t)slot; op.http = 0; op.kind = 0; op.pad = 0; op.seq = 0;
-    CK(cudaMemcpyAsync(h->d_ops, h->h_ops, sizeof(agr_dop), cudaMemcpyHostToDevice, h->stream));
-    sync_window(h);
-    agr_launch_resolve(h->d, h->d_ops, h->d_hrid, 1, h->stream);
-    h->k3_launches += 1;
-    CK(cudaMemcpyAsync(h->h_small, h->d_hrid, 4, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    if (h->h_small[0] == AGR_RID_NONE) return fail(AGR_ENOTFOUND, "request not found");
-    *rid = h->h_small[0];
-    return 0;
-}
-
 // which: 0 = response (hdr_len leading bytes are its flattened headers), 1 = error text
 static int store_bytes_locked(agr_handle* h, const char* agent_id, const uint8_t request_id[16], int which, const uint8_t* a, uint32_t alen,
                               const uint8_t* b, uint32_t blen) {
     uint32_t rid = 0;
-    TRY(resolve_one_locked(h, agent_id, request_id, &rid));
+    TRY(resolve_one_locked(h, agent_id, request_id, &rid, true));
     const uint32_t len = alen + blen;
     const uint64_t need = ((uint64_t)len + 15u) & ~15ull;
     unsigned long long off;
@@ -1774,7 +1736,7 @@ int agr_get_response_body(agr_handle* h, const char* agent_id, const uint8_t req
     HLock lk(h);
     CK(cudaSetDevice(h->device));
     uint32_t rid = 0;
-    TRY(resolve_one_locked(h, agent_id, request_id, &rid));
+    TRY(resolve_one_locked(h, agent_id, request_id, &rid, true));
     unsigned long long off = 0; uint32_t l = 0;
     CK(cudaMemcpyAsync(&off, h->d_resp_off + rid, 8, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaMemcpyAsync(&l, h->d_resp_len + rid, 4, cudaMemcpyDeviceToHost, h->stream));
@@ -1790,38 +1752,27 @@ int agr_get_response_body(agr_handle* h, const char* agent_id, const uint8_t req
 static int json_encode_locked(agr_handle* h, const uint32_t* d_rids, uint64_t first_rid, uint32_t n, bool array, uint64_t* total, bool roundtrip = false) {
     *total = 0;
     if (n == 0) return 0;
-    if (n > h->j_cap) {
-        const uint32_t cap = std::max<uint32_t>(n, 1024);
-        TRY(dev_regrow(h, &h->d_jlen, cap, false));
-        TRY(dev_regrow(h, &h->d_joff, (size_t)cap + 1, false));
-        TRY(dev_regrow(h, &h->d_jchunk, (size_t)agr_k5_chunks(cap) + 1, false));
-        h->j_cap = cap;
-    }
+    const uint32_t cap = std::max<uint32_t>(n, 1024);
+    if (n > h->d_jlen.cap) TRY(regrow(h, h->d_jlen, cap));
+    if ((size_t)n + 1 > h->d_joff.cap) TRY(regrow(h, h->d_joff, (size_t)cap + 1));
+    if ((size_t)agr_k5_chunks(n) + 1 > h->d_jchunk.cap) TRY(regrow(h, h->d_jchunk, (size_t)agr_k5_chunks(cap) + 1));
     agr_k5_params p{};
     p.rids = d_rids; p.first_l = first_rid; p.n = n; p.array = array ? 1u : 0u; p.roundtrip = roundtrip ? 1u : 0u;
     sync_window(h);
-    p.len = h->d_jlen; p.off = h->d_joff; p.chunk_sum = h->d_jchunk; p.out = nullptr;
+    p.len = h->d_jlen.p; p.off = h->d_joff.p; p.chunk_sum = h->d_jchunk.p; p.out = nullptr;
     p.bytes = h->d_resp; p.resp_off = h->d_resp_off; p.resp_len = h->d_resp_len; p.resp_hlen = h->d_resp_hlen;
     p.err_off = h->d_err_off; p.err_len = h->d_err_len; p.ptime = h->d.ptime;
-    const bool timing = (h->cfg.flags & AGR_CFG_TIMING) != 0;
-    if (timing) {
-        for (auto& e : h->op_ev) if (!e) CK(cudaEventCreate(&e));
-        CK(cudaEventRecord(h->op_ev[4], h->stream));
-    }
+    TRY(op_time_begin(h, 2));
     agr_launch_k5_measure(h->d, p, h->stream);
     CK(cudaGetLastError());
     unsigned long long tot = 0;
-    CK(cudaMemcpyAsync(&tot, h->d_jchunk + agr_k5_chunks(n), 8, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaMemcpyAsync(&tot, h->d_jchunk.p + agr_k5_chunks(n), 8, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
-    if (tot + 16 > h->json_cap) {
-        const uint64_t cap = std::max<uint64_t>(tot + tot / 4 + 16, 1 << 16);
-        TRY(dev_regrow(h, &h->d_json, (size_t)cap, false));
-        h->json_cap = cap;
-    }
-    p.out = h->d_json;
+    if (tot + 16 > h->d_json.cap) TRY(regrow(h, h->d_json, (size_t)std::max<uint64_t>(tot + tot / 4 + 16, 1 << 16)));
+    p.out = h->d_json.p;
     agr_launch_k5_emit(h->d, p, h->stream);
     CK(cudaGetLastError());
-    if (timing) { CK(cudaEventRecord(h->op_ev[5], h->stream)); h->op_timed[2] = true; }
+    TRY(op_time_end(h, 2));
     h->k5_launches += 3;
     *total = tot;
     return 0;
@@ -1830,7 +1781,7 @@ static int json_copy_out(agr_handle* h, uint64_t total, uint8_t* out, uint64_t c
     *len = total;
     if (!out) { CK(cudaStreamSynchronize(h->stream)); return 0; }
     if (total > cap) return fail(AGR_ECAP, "output buffer too small");
-    if (total) CK(cudaMemcpyAsync(out, h->d_json, (size_t)total, cudaMemcpyDeviceToHost, h->stream));
+    if (total) CK(cudaMemcpyAsync(out, h->d_json.p, (size_t)total, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
     return 0;
 }
@@ -1848,7 +1799,7 @@ int agr_rows_json(agr_handle* h, uint64_t first_rid, uint32_t n, int as_array, u
         if (offsets) offsets[0] = 0;
         return 0;
     }
-    if (offsets && n) CK(cudaMemcpyAsync(offsets, h->d_joff, ((size_t)n + 1) * 8, cudaMemcpyDeviceToHost, h->stream));
+    if (offsets && n) CK(cudaMemcpyAsync(offsets, h->d_joff.p, ((size_t)n + 1) * 8, cudaMemcpyDeviceToHost, h->stream));
     else if (offsets) offsets[0] = 0;
     return json_copy_out(h, total, out, cap, len);
 }
@@ -1861,7 +1812,7 @@ int agr_pending_json(agr_handle* h, const char* agent_id, uint8_t* out, uint64_t
     uint32_t total_rows = 0;
     int slot = agent_find(h, agent_id);
     if (slot >= 0) {
-        const uint32_t cap0 = std::max<uint32_t>(h->out_cap, 1024);
+        const uint32_t cap0 = std::max<uint32_t>((uint32_t)h->d_out_rid.cap, 1024);
         TRY(select_locked(h, K3_AGENT_PENDING, (uint32_t)slot, nullptr, h->scan_lo, ingested_bound(h), cap0, &total_rows));
         if (total_rows > cap0)                                   // counts only: run again with room for all of it
             TRY(select_locked(h, K3_AGENT_PENDING, (uint32_t)slot, nullptr, h->scan_lo, ingested_bound(h), total_rows, &total_rows));
@@ -1873,7 +1824,7 @@ int agr_pending_json(agr_handle* h, const char* agent_id, uint8_t* out, uint64_t
         return 0;
     }
     uint64_t total = 0;
-    TRY(json_encode_locked(h, h->d_out_rid, 0, total_rows, true, &total, true));   // GetPendingRequests unmarshals every record
+    TRY(json_encode_locked(h, h->d_out_rid.p, 0, total_rows, true, &total, true));   // GetPendingRequests unmarshals every record
     return json_copy_out(h, total, out, cap, len);
 }
 
@@ -1881,8 +1832,7 @@ int agr_get_record_json(agr_handle* h, const char* agent_id, const uint8_t reque
     if (!h || !agent_id || !request_id || !len) return fail(AGR_EINVAL, "NULL argument");
     HLock lk(h);
     CK(cudaSetDevice(h->device));
-    uint32_t rid = 0;
-    TRY(resolve_one_locked(h, agent_id, request_id, &rid));
+    TRY(resolve_one_locked(h, agent_id, request_id, nullptr, true));
     uint64_t total = 0, l = 0;
     TRY(json_encode_locked(h, h->d_hrid, 0, 1, false, &total));   // k2.hrid[0] = the physical row resolve_one_locked found
     int rc = json_copy_out(h, total, out, cap, &l);
@@ -1896,7 +1846,7 @@ struct snap_header {
     uint32_t flags, n_agents, shard, gen;
     uint64_t rows_used, vused, log_len[2], id_secret, scan_lo, resp_used, expired_total, tail, released_total, slab_rows, vtail, vcap, resp_tail, resp_cap;
 };
-static int dump_dev(agr_handle* h, FILE* f, const void* dsrc, size_t bytes) {
+static int dump_dev(agr_handle* h, FILE* f, void* dsrc, size_t bytes) {
     const size_t chunk = h->bounce_bytes;
     for (size_t o = 0; o < bytes; o += chunk) {
         const size_t m = std::min(chunk, bytes - o);
@@ -1914,6 +1864,38 @@ static int load_dev(agr_handle* h, FILE* f, void* ddst, size_t bytes) {
         CK(cudaMemcpyAsync((uint8_t*)ddst + o, h->bounce[0], m, cudaMemcpyHostToDevice, h->stream));
         CK(cudaStreamSynchronize(h->stream));
     }
+    return 0;
+}
+// the physical rows a snapshot holds
+static size_t snap_rows(const snap_header& hd) {
+    return (hd.flags & AGR_CFG_RING) ? (size_t)std::min<uint64_t>(hd.rows_used, hd.slab_rows) : (size_t)hd.rows_used;
+}
+// The sections that follow the header and the agent table, in file order, each handed to io (dump_dev or load_dev) as
+// (device array, bytes).  Every size comes from the header alone: the one description of the layout that agr_snapshot
+// and agr_restore share (tests/test_snapshot_layout_gpu.py reads a file against it).
+static int snap_sections(agr_handle* h, const snap_header& hd, FILE* f, int (*io)(agr_handle*, FILE*, void*, size_t)) {
+    const bool ring = (hd.flags & AGR_CFG_RING) != 0, varlen = (hd.flags & AGR_CFG_VARLEN) != 0;
+    const size_t R = snap_rows(hd);
+    const struct { void* p; size_t bytes; } sections[] = {
+        {h->d.slab, varlen ? (size_t)(ring ? std::min<uint64_t>(hd.vused, hd.vcap) : hd.vused) : R * AGR_REC},
+        {h->d.state, R * 4},
+        {h->d.route, R * 4},
+        {h->d.aux, R * 4},
+        {h->d.cksum, R * 8},
+        {h->d.voff, varlen ? R * 8 : 0},
+        {h->d.vlen, varlen ? R * 4 : 0},
+        {h->d.completed_log, (size_t)hd.log_len[0] * 4},
+        {h->d.failed_log, (size_t)hd.log_len[1] * 4},
+        {h->d_resp, (size_t)(ring ? std::min<uint64_t>(hd.resp_used, hd.resp_cap) : hd.resp_used)},
+        {h->d_resp_off, R * 8},
+        {h->d_resp_len, R * 4},
+        {h->d_resp_hlen, R * 4},
+        {h->d_err_off, R * 8},
+        {h->d_err_len, R * 4},
+        {h->d.ptime, R * 8},
+        {h->d.mtime, R * 8},
+    };
+    for (const auto& s : sections) TRY(io(h, f, s.p, s.bytes));
     return 0;
 }
 
@@ -1941,27 +1923,7 @@ int agr_snapshot(agr_handle* h, const char* path) {
         strncpy(name, h->agent_names[a].c_str(), AGR_AGENT_ID_BYTES - 1);
         fwrite(name, 1, AGR_AGENT_ID_BYTES, f); fwrite(&h->agent_status[a], 1, 1, f);
     }
-    const size_t R = (size_t)rows_span(h);
-    const size_t slab_bytes = (h->cfg.flags & AGR_CFG_VARLEN) ? (size_t)(is_ring(h) ? std::min<uint64_t>(hd.vused, h->vcap) : hd.vused) : R * AGR_REC;
-    if ((rc = dump_dev(h, f, h->d.slab, slab_bytes)) < 0) return done(rc);
-    if ((rc = dump_dev(h, f, h->d.state, R * 4)) < 0) return done(rc);
-    if ((rc = dump_dev(h, f, h->d.route, R * 4)) < 0) return done(rc);
-    if ((rc = dump_dev(h, f, h->d.aux, R * 4)) < 0) return done(rc);
-    if ((rc = dump_dev(h, f, h->d.cksum, R * 8)) < 0) return done(rc);
-    if (h->cfg.flags & AGR_CFG_VARLEN) {
-        if ((rc = dump_dev(h, f, h->d.voff, R * 8)) < 0) return done(rc);
-        if ((rc = dump_dev(h, f, h->d.vlen, R * 4)) < 0) return done(rc);
-    }
-    if ((rc = dump_dev(h, f, h->d.completed_log, (size_t)lens[0] * 4)) < 0) return done(rc);
-    if ((rc = dump_dev(h, f, h->d.failed_log, (size_t)lens[1] * 4)) < 0) return done(rc);
-    if ((rc = dump_dev(h, f, h->d_resp, (size_t)(is_ring(h) ? std::min<uint64_t>(hd.resp_used, h->resp_cap) : hd.resp_used))) < 0) return done(rc);
-    if ((rc = dump_dev(h, f, h->d_resp_off, R * 8)) < 0) return done(rc);
-    if ((rc = dump_dev(h, f, h->d_resp_len, R * 4)) < 0) return done(rc);
-    if ((rc = dump_dev(h, f, h->d_resp_hlen, R * 4)) < 0) return done(rc);
-    if ((rc = dump_dev(h, f, h->d_err_off, R * 8)) < 0) return done(rc);
-    if ((rc = dump_dev(h, f, h->d_err_len, R * 4)) < 0) return done(rc);
-    if ((rc = dump_dev(h, f, h->d.ptime, R * 8)) < 0) return done(rc);
-    if ((rc = dump_dev(h, f, h->d.mtime, R * 8)) < 0) return done(rc);
+    if ((rc = snap_sections(h, hd, f, dump_dev)) < 0) return done(rc);
     return done(0);
 }
 
@@ -1998,27 +1960,8 @@ int agr_restore(const agr_config* cfg, const char* path, agr_handle** out) {
         if (removed) { HLock lk(h); h->agent_status[a] = AG_STATUS_REMOVED; if ((rc = push_agent_status(h, a, AG_STATUS_REMOVED)) < 0) return bail(rc); }
     }
     HLock lk(h);
-    const size_t R = snap_ring ? (size_t)std::min<uint64_t>(hd.rows_used, hd.slab_rows) : (size_t)hd.rows_used;
-    const size_t slab_bytes = (hd.flags & AGR_CFG_VARLEN) ? (size_t)(snap_ring ? std::min<uint64_t>(hd.vused, hd.vcap) : hd.vused) : R * AGR_REC;
-    if ((rc = load_dev(h, f, h->d.slab, slab_bytes)) < 0) return bail(rc);
-    if ((rc = load_dev(h, f, h->d.state, R * 4)) < 0) return bail(rc);
-    if ((rc = load_dev(h, f, h->d.route, R * 4)) < 0) return bail(rc);
-    if ((rc = load_dev(h, f, h->d.aux, R * 4)) < 0) return bail(rc);
-    if ((rc = load_dev(h, f, h->d.cksum, R * 8)) < 0) return bail(rc);
-    if (hd.flags & AGR_CFG_VARLEN) {
-        if ((rc = load_dev(h, f, h->d.voff, R * 8)) < 0) return bail(rc);
-        if ((rc = load_dev(h, f, h->d.vlen, R * 4)) < 0) return bail(rc);
-    }
-    if ((rc = load_dev(h, f, h->d.completed_log, (size_t)hd.log_len[0] * 4)) < 0) return bail(rc);
-    if ((rc = load_dev(h, f, h->d.failed_log, (size_t)hd.log_len[1] * 4)) < 0) return bail(rc);
-    if ((rc = load_dev(h, f, h->d_resp, (size_t)(snap_ring ? std::min<uint64_t>(hd.resp_used, hd.resp_cap) : hd.resp_used))) < 0) return bail(rc);
-    if ((rc = load_dev(h, f, h->d_resp_off, R * 8)) < 0) return bail(rc);
-    if ((rc = load_dev(h, f, h->d_resp_len, R * 4)) < 0) return bail(rc);
-    if ((rc = load_dev(h, f, h->d_resp_hlen, R * 4)) < 0) return bail(rc);
-    if ((rc = load_dev(h, f, h->d_err_off, R * 8)) < 0) return bail(rc);
-    if ((rc = load_dev(h, f, h->d_err_len, R * 4)) < 0) return bail(rc);
-    if ((rc = load_dev(h, f, h->d.ptime, R * 8)) < 0) return bail(rc);
-    if ((rc = load_dev(h, f, h->d.mtime, R * 8)) < 0) return bail(rc);
+    const size_t R = snap_rows(hd);
+    if ((rc = snap_sections(h, hd, f, load_dev)) < 0) return bail(rc);
     h->resp_used = hd.resp_used; h->resp_tail = hd.resp_tail; h->expired_total = hd.expired_total;
     unsigned long long lens[2] = {hd.log_len[0], hd.log_len[1]};
     if (cudaMemcpy(h->d.log_len, lens, sizeof lens, cudaMemcpyHostToDevice) != cudaSuccess) return bail(fail(AGR_ECUDA, "restore: log_len"));
@@ -2040,7 +1983,7 @@ int agr_expire(agr_handle* h, uint64_t now, uint64_t ttl, uint64_t* expired) {
     if (!h) return fail(AGR_EINVAL, "NULL argument");
     HLock lk(h);
     CK(cudaSetDevice(h->device));
-    unsigned long long* d_cnt = expired ? (unsigned long long*)(h->d.ctr + C_NCTR - 1) : nullptr;     // last counter slot as scratch
+    unsigned long long* d_cnt = expired ? count_slot(h) : nullptr;
     if (d_cnt) CK(cudaMemsetAsync(d_cnt, 0, 8, h->stream));
     sync_window(h);
     if ((!is_ring(h) || (h->cfg.flags & AGR_CFG_VARLEN)) && h->rows_used > h->sweep_clean) {
@@ -2063,8 +2006,7 @@ int agr_expire(agr_handle* h, uint64_t now, uint64_t ttl, uint64_t* expired) {
         return 0;
     }
     unsigned long long v = 0;
-    CK(cudaMemcpyAsync(&v, d_cnt, 8, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
+    TRY(read_count(h, &v));
     h->expired_total += v;
     *expired = v;
     return 0;
@@ -2123,13 +2065,11 @@ static int reclaim_apply(agr_handle* h, uint64_t* released) {
         h->k1_launches += 2;
     }
     if (h->resp_used != h->resp_tail) {   // the response / error byte ring: its tail follows the oldest blob a live row still refers to
-        unsigned long long* d_span = (unsigned long long*)(h->d.ctr + C_NCTR - 1);              // last counter slot as scratch
-        CK(cudaMemsetAsync(d_span, 0, 8, h->stream));
-        agr_launch_bytes_span(h->d, h->resp_used % h->resp_cap, h->resp_cap, h->d_resp_off, h->d_resp_len, h->d_err_off, h->d_err_len, d_span, h->stream);
+        CK(cudaMemsetAsync(count_slot(h), 0, 8, h->stream));
+        agr_launch_bytes_span(h->d, h->resp_used % h->resp_cap, h->resp_cap, h->d_resp_off, h->d_resp_len, h->d_err_off, h->d_err_len, count_slot(h), h->stream);
         CK(cudaGetLastError());
         unsigned long long span = 0;
-        CK(cudaMemcpyAsync(&span, d_span, 8, cudaMemcpyDeviceToHost, h->stream));
-        CK(cudaStreamSynchronize(h->stream));
+        TRY(read_count(h, &span));
         h->resp_tail = h->resp_used - span;
         h->k3_launches += 1;
     }
@@ -2184,15 +2124,13 @@ int agr_verify(agr_handle* h, uint64_t* rows_checked, uint64_t* bad) {
     if (!h || !bad) return fail(AGR_EINVAL, "NULL argument");
     HLock lk(h);
     CK(cudaSetDevice(h->device));
-    unsigned long long* d_bad = (unsigned long long*)(h->d.ctr + C_NCTR - 1);     // last counter slot as scratch
-    CK(cudaMemsetAsync(d_bad, 0, 8, h->stream));
+    CK(cudaMemsetAsync(count_slot(h), 0, 8, h->stream));
     sync_window(h);
-    agr_launch_verify(h->d, rows_span(h), d_bad, h->stream);
+    agr_launch_verify(h->d, rows_span(h), count_slot(h), h->stream);
     h->k3_launches += 1;
     CK(cudaGetLastError());
     unsigned long long v = 0;
-    CK(cudaMemcpyAsync(&v, d_bad, 8, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
+    TRY(read_count(h, &v));
     *bad = v;
     if (rows_checked) *rows_checked = rows_span(h);
     return 0;
@@ -2205,8 +2143,7 @@ int agr_stats_get(agr_handle* h, agr_stats* out) {
     CK(cudaSetDevice(h->device));
     unsigned long long c[C_NCTR], lens[2];
     CK(cudaMemcpyAsync(c, h->d.ctr, sizeof c, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaMemcpyAsync(lens, h->d.log_len, sizeof lens, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
+    TRY(read_log_lens(h, lens));
     memset(out, 0, sizeof *out);
     out->rows_used = h->rows_used; out->rows_cap = h->cfg.slab_rows;
     out->ingested = c[C_INGESTED]; out->stored = c[C_STORED]; out->replay_flagged = c[C_REPLAY];
@@ -2440,25 +2377,12 @@ int agr_ingest_sharded(agr_handle* h, const agr_record* recs, uint32_t n, agr_ve
     uint64_t first = h->rows_used;
     if (n) {
         TRY(reserve_rows_locked(h, n, &first));
-        // the batch goes STRAIGHT into its slab rows, in chunks on the copy stream (a pageable source through the bounce buffers)
-        const bool src_pinned = is_pinned(recs);
+        // the batch goes STRAIGHT into its slab rows, on the copy stream
         while (h->chunk_ev.size() < 2) { cudaEvent_t e; CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming)); h->chunk_ev.push_back(e); }
         CK(cudaEventRecord(h->chunk_ev[0], h->stream));
         CK(cudaStreamWaitEvent(h->copy_stream, h->chunk_ev[0], 0));
-        uint8_t* dst = h->d.slab + phys_row(h, first) * AGR_REC;
-        const size_t bytes = (size_t)n * AGR_REC;
-        if (src_pinned) CK(cudaMemcpyAsync(dst, recs, bytes, cudaMemcpyHostToDevice, h->copy_stream));
-        else {
-            int bk = 0;
-            for (size_t o = 0; o < bytes;) {
-                const size_t piece = std::min(h->bounce_bytes, bytes - o);
-                CK(cudaEventSynchronize(h->bounce_ev[bk]));
-                par_memcpy(h->bounce[bk], (const uint8_t*)recs + o, piece);
-                CK(cudaMemcpyAsync(dst + o, h->bounce[bk], piece, cudaMemcpyHostToDevice, h->copy_stream));
-                CK(cudaEventRecord(h->bounce_ev[bk], h->copy_stream));
-                o += piece; bk ^= 1;
-            }
-        }
+        int bk = 0;
+        TRY(upload_rows(h, batch_rows(h, first), (const uint8_t*)recs, (size_t)n * AGR_REC, is_pinned(recs), bk));
         CK(cudaEventRecord(h->chunk_ev[1], h->copy_stream));
         CK(cudaStreamWaitEvent(h->stream, h->chunk_ev[1], 0));
     }
@@ -2663,8 +2587,7 @@ int agr_debug_skip_arrivals(agr_handle* h, uint64_t n) {
     if (n > AGR_ROW_LIMIT - h->rows_used) return fail(AGR_EINVAL, "skip would pass the row id bound (2^52)");
     if (h->tail != h->rows_used || !h->resv.empty() || h->reclaim_pending) return fail(AGR_EINVAL, "window not empty: expire and reclaim every row first");
     unsigned long long lens[2];
-    CK(cudaMemcpyAsync(lens, h->d.log_len, sizeof lens, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
+    TRY(read_log_lens(h, lens));
     if (lens[0] || lens[1]) return fail(AGR_EINVAL, "window not empty: the completed / failed logs hold entries");
     if (n == 0) return 0;
     h->rows_used += n; h->tail += n; h->released_total += n;
@@ -2792,10 +2715,10 @@ int agr_synth_fill_rows(agr_handle* h, const agr_synth* s, uint64_t first_index,
     if (s->zipf_milli) {
         std::vector<unsigned long long> cdf;
         zipf_cdf(s->n_agents, s->zipf_milli, cdf);
-        if (h->cdf_n < s->n_agents) { TRY(dev_regrow(h, &h->d_cdf, s->n_agents, false)); h->cdf_n = s->n_agents; }
-        CK(cudaMemcpyAsync(h->d_cdf, cdf.data(), (size_t)s->n_agents * 8, cudaMemcpyHostToDevice, h->stream));
+        if (h->d_cdf.cap < s->n_agents) TRY(regrow(h, h->d_cdf, s->n_agents));
+        CK(cudaMemcpyAsync(h->d_cdf.p, cdf.data(), (size_t)s->n_agents * 8, cudaMemcpyHostToDevice, h->stream));
         CK(cudaStreamSynchronize(h->stream));
-        dcdf = h->d_cdf;
+        dcdf = h->d_cdf.p;
     }
     agr_launch_synth(h->d.slab + phys_row(h, first_rid) * AGR_REC, synth_params(s, dcdf), first_index, n, h->stream);
     CK(cudaGetLastError());                                      // (stream-ordered before whatever reads the rows: no wait here)
