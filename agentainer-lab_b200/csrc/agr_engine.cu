@@ -160,8 +160,17 @@ struct agr_handle {
     exchange_plan xdbg{}; uint64_t xdbg_first = 0; uint32_t xdbg_n = 0; bool xdbg_open = false;   // agr_debug_exchange_begin -> _end
     // AGR_CFG_TIMING: CUDA-event pairs around the dominant K1 kernel, on the launching stream
     std::vector<cudaEvent_t> tev; uint64_t tev_next = 0, tev_read = 0, timing_calls = 0;
-    cudaEvent_t op_ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // [0,1] last K2 group, [2,3] last K3 select group, [4,5] last K5 encode
-    bool op_timed[3] = {false, false, false};
+    cudaEvent_t op_ev[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // [0,1] last K2 group, [2,3] last K3 select group, [4,5] last K5 encode, [6,7] last snapshot cut
+    bool op_timed[4] = {false, false, false, false};
+    // AGR_CFG_ONLINE_SNAPSHOT: the cut's device shadow of the sections rewritten in place (the two log lengths at offset 0, then
+    // every such section at shadow_off), the writer's own stream, its two pinned buffers, and the pins (agr_snapshot)
+    uint8_t* d_shadow = nullptr; size_t shadow_off[17] = {};
+    cudaStream_t snap_stream = nullptr;
+    cudaEvent_t snap_ev[3] = {nullptr, nullptr, nullptr};   // [0] the cut, [1 + b] the last copy into snap_buf[b]
+    uint8_t* snap_buf[2] = {nullptr, nullptr}; size_t snap_buf_bytes = 0;
+    int snap_cur = 0; size_t snap_pend = 0;                 // buffer of the next chunk; bytes of the chunk waiting in the other one
+    std::mutex snap_mu;                                      // one online snapshot at a time: there is one shadow
+    bool pinned = false; uint64_t pin_tail = 0, pin_vtail = 0, pin_resp_tail = 0;   // (h->mu) the cut's ring tails while it is written
 };
 #define AGR_TIMING_RING 1024
 
@@ -687,6 +696,8 @@ void* agr_host_alloc(size_t bytes) {
 }
 void agr_host_free(void* p) { if (p) cudaFreeHost(p); }
 
+static int snap_online_create(agr_handle* h);
+
 static int create_impl(const agr_config* cfg_in, agr_handle* h) {
     agr_config c{};
     if (cfg_in) c = *cfg_in;
@@ -813,6 +824,7 @@ static int create_impl(const agr_config* cfg_in, agr_handle* h) {
     TRY(dev_alloc(h, &h->d_gtotal, ((size_t)c.max_agents + 8) * 66, false));   // gtotal + 64 segment partials per group
     TRY(dev_alloc(h, &h->d_goff, (size_t)c.max_agents + 2, false));
     TRY(dev_alloc(h, &h->d_min_inq, (size_t)1, false));
+    if (c.flags & AGR_CFG_ONLINE_SNAPSHOT) TRY(snap_online_create(h));
     CK(cudaStreamSynchronize(h->stream));
     if ((c.flags & AGR_CFG_COMBINE) && !varlen) TRY(svc_create(h));
     return 0;
@@ -837,6 +849,8 @@ void agr_destroy(agr_handle* h) {
     for (int k = 0; k < 2; ++k) if (h->bounce_ev[k]) cudaEventDestroy(h->bounce_ev[k]);
     for (auto e : h->tev) cudaEventDestroy(e);
     for (auto e : h->op_ev) if (e) cudaEventDestroy(e);
+    for (auto e : h->snap_ev) if (e) cudaEventDestroy(e);
+    if (h->snap_stream) cudaStreamDestroy(h->snap_stream);
     for (auto e : h->chunk_ev) cudaEventDestroy(e);
     if (h->reclaim_ev) cudaEventDestroy(h->reclaim_ev);
     if (h->copy_stream) cudaStreamDestroy(h->copy_stream);
@@ -973,6 +987,14 @@ static bool ring_fits(uint64_t used, uint64_t tail, uint64_t cap, uint64_t need,
     *pad = (at + need > cap) ? cap - at : 0;
     return used + *pad + need - tail <= cap;
 }
+// While an online snapshot is being written, its file streams the rows and bytes of the cut's window from where they lie, so
+// a reservation may not lap into that window even once agr_reclaim has released it: the ring's tail is min(tail, pin).
+static const char* const PINNED_FULL = "ring full up to the window of the snapshot being written (agr_snapshot with AGR_CFG_ONLINE_SNAPSHOT): "
+                                       "its rows and bytes are reused once the file is written";
+static inline bool ring_fits_pinned(const agr_handle* h, uint64_t used, uint64_t tail, uint64_t pin, uint64_t cap, uint64_t need) {
+    uint64_t pad = 0;
+    return !h->pinned || ring_fits(used, std::min(tail, pin), cap, need, &pad);
+}
 
 // ------------------------------------------------------------------------------------------ K1
 static int reserve_rows_locked(agr_handle* h, uint32_t n, uint64_t* first) {
@@ -986,6 +1008,7 @@ static int reserve_rows_locked(agr_handle* h, uint32_t n, uint64_t* first) {
     // ring: rows skipped at the end of a lap stay "no record" (released rows are zeroed), at most max_batch rows per lap
     uint64_t pad = 0;
     if (!ring_fits(h->rows_used, h->tail, h->cfg.slab_rows, n, &pad)) return fail(AGR_ENOSPC, "slab full: agr_expire + agr_reclaim release rows at the tail");
+    if (!ring_fits_pinned(h, h->rows_used, h->tail, h->pin_tail, h->cfg.slab_rows, n)) return fail(AGR_ENOSPC, std::string("slab ") + PINNED_FULL);
     if (h->rows_used + pad + n > AGR_ROW_LIMIT) return fail(AGR_ENOSPC, "row ids exhausted: a shard hands out 2^52 rows (minted ids stay unique that long)");
     h->rows_used += pad;
     *first = h->rows_used;
@@ -1011,7 +1034,7 @@ static int claim_k1_events(agr_handle* h, cudaEvent_t* e0, cudaEvent_t* e1) {
     *e0 = h->tev[2 * k]; *e1 = h->tev[2 * k + 1];
     return 0;
 }
-// AGR_CFG_TIMING: events around the last launch group g (0 = K2, 1 = K3 select, 2 = K5 encode) that agr_op_time reads
+// AGR_CFG_TIMING: events around the last launch group g (0 = K2, 1 = K3 select, 2 = K5 encode, 3 = snapshot cut) that agr_op_time reads
 static int op_time_begin(agr_handle* h, int g) {
     if (!(h->cfg.flags & AGR_CFG_TIMING)) return 0;
     for (auto& e : h->op_ev) if (!e) CK(cudaEventCreate(&e));
@@ -1289,6 +1312,7 @@ static int resp_reserve_locked(agr_handle* h, uint64_t need, uint64_t len, unsig
     uint64_t pad = 0;
     if (!ring_fits(h->resp_used, h->resp_tail, h->resp_cap, need, &pad))
         return fail(AGR_ENOSPC, "response slab full: agr_reclaim releases the bytes of released rows");
+    if (!ring_fits_pinned(h, h->resp_used, h->resp_tail, h->pin_resp_tail, h->resp_cap, need)) return fail(AGR_ENOSPC, std::string("response slab ") + PINNED_FULL);
     h->resp_used += pad;
     *off = h->resp_used % h->resp_cap;                           // the rows keep PHYSICAL offsets
     h->resp_used += need;
@@ -1599,6 +1623,7 @@ int agr_ingest_var(agr_handle* h, const uint8_t* blob, const uint32_t* offsets, 
     } else {                                                      // byte ring: a blob never wraps either
         if (bytes > h->vcap / 2) return fail(AGR_EINVAL, "batch larger than half the byte slab");
         if (!ring_fits(h->vused, h->vtail, h->vcap, bytes, &vpad)) return fail(AGR_ENOSPC, "byte slab full: agr_expire + agr_reclaim release bytes at the tail");
+        if (!ring_fits_pinned(h, h->vused, h->vtail, h->pin_vtail, h->vcap, bytes)) return fail(AGR_ENOSPC, std::string("byte slab ") + PINNED_FULL);
     }
     TRY(reserve_rows_locked(h, n, &first));
     if (first_rid) *first_rid = first;
@@ -1870,48 +1895,178 @@ static int load_dev(agr_handle* h, FILE* f, void* ddst, size_t bytes) {
 static size_t snap_rows(const snap_header& hd) {
     return (hd.flags & AGR_CFG_RING) ? (size_t)std::min<uint64_t>(hd.rows_used, hd.slab_rows) : (size_t)hd.rows_used;
 }
-// The sections that follow the header and the agent table, in file order, each handed to io (dump_dev or load_dev) as
-// (device array, bytes).  Every size comes from the header alone: the one description of the layout that agr_snapshot
-// and agr_restore share (tests/test_snapshot_layout_gpu.py reads a file against it).
-static int snap_sections(agr_handle* h, const snap_header& hd, FILE* f, int (*io)(agr_handle*, FILE*, void*, size_t)) {
+// One section of the file: its live device array, its size, and what later calls do to it.  kind SNAP_APPEND: only ever
+// appended to inside the window of a snapshot (the slab rows, the record bytes, the response bytes); SNAP_WORDS: per-row words
+// rewritten in place; SNAP_LOG: a log, rewritten in place (k_drop_logs) and compacted by agr_reclaim.  The online snapshot
+// copies the last two kinds into its shadow at the cut and streams the first from where it lies.
+enum { SNAP_APPEND = 0, SNAP_WORDS = 1, SNAP_LOG = 2 };
+struct snap_section { void* p; size_t bytes; int kind; };
+#define SNAP_NSEC 17
+// The sections that follow the header and the agent table, in file order.  Every size comes from the header alone: the one
+// description of the layout that agr_snapshot and agr_restore share (tests/test_snapshot_layout_gpu.py reads a file against it).
+static void snap_table(agr_handle* h, const snap_header& hd, snap_section out[SNAP_NSEC]) {
     const bool ring = (hd.flags & AGR_CFG_RING) != 0, varlen = (hd.flags & AGR_CFG_VARLEN) != 0;
     const size_t R = snap_rows(hd);
-    const struct { void* p; size_t bytes; } sections[] = {
-        {h->d.slab, varlen ? (size_t)(ring ? std::min<uint64_t>(hd.vused, hd.vcap) : hd.vused) : R * AGR_REC},
-        {h->d.state, R * 4},
-        {h->d.route, R * 4},
-        {h->d.aux, R * 4},
-        {h->d.cksum, R * 8},
-        {h->d.voff, varlen ? R * 8 : 0},
-        {h->d.vlen, varlen ? R * 4 : 0},
-        {h->d.completed_log, (size_t)hd.log_len[0] * 4},
-        {h->d.failed_log, (size_t)hd.log_len[1] * 4},
-        {h->d_resp, (size_t)(ring ? std::min<uint64_t>(hd.resp_used, hd.resp_cap) : hd.resp_used)},
-        {h->d_resp_off, R * 8},
-        {h->d_resp_len, R * 4},
-        {h->d_resp_hlen, R * 4},
-        {h->d_err_off, R * 8},
-        {h->d_err_len, R * 4},
-        {h->d.ptime, R * 8},
-        {h->d.mtime, R * 8},
+    const snap_section sections[SNAP_NSEC] = {
+        {h->d.slab, varlen ? (size_t)(ring ? std::min<uint64_t>(hd.vused, hd.vcap) : hd.vused) : R * AGR_REC, SNAP_APPEND},
+        {h->d.state, R * 4, SNAP_WORDS},
+        {h->d.route, R * 4, SNAP_WORDS},
+        {h->d.aux, R * 4, SNAP_WORDS},
+        {h->d.cksum, R * 8, SNAP_WORDS},
+        {h->d.voff, varlen ? R * 8 : 0, SNAP_WORDS},
+        {h->d.vlen, varlen ? R * 4 : 0, SNAP_WORDS},
+        {h->d.completed_log, (size_t)hd.log_len[0] * 4, SNAP_LOG},
+        {h->d.failed_log, (size_t)hd.log_len[1] * 4, SNAP_LOG},
+        {h->d_resp, (size_t)(ring ? std::min<uint64_t>(hd.resp_used, hd.resp_cap) : hd.resp_used), SNAP_APPEND},
+        {h->d_resp_off, R * 8, SNAP_WORDS},
+        {h->d_resp_len, R * 4, SNAP_WORDS},
+        {h->d_resp_hlen, R * 4, SNAP_WORDS},
+        {h->d_err_off, R * 8, SNAP_WORDS},
+        {h->d_err_len, R * 4, SNAP_WORDS},
+        {h->d.ptime, R * 8, SNAP_WORDS},
+        {h->d.mtime, R * 8, SNAP_WORDS},
     };
-    for (const auto& s : sections) TRY(io(h, f, s.p, s.bytes));
+    for (int k = 0; k < SNAP_NSEC; ++k) out[k] = sections[k];
+}
+// Hands every section to io (dump_dev, load_dev or the online writer's dump_online) as (device array, bytes).  The source
+// table says where each section's bytes are: nullptr = the live arrays; the online writer passes the cut's shadow, which
+// holds the sections rewritten in place at h->shadow_off (the append-only ones still come from the live arrays).
+static int snap_sections(agr_handle* h, const snap_header& hd, FILE* f, int (*io)(agr_handle*, FILE*, void*, size_t),
+                         uint8_t* shadow = nullptr) {
+    snap_section sec[SNAP_NSEC];
+    snap_table(h, hd, sec);
+    for (int k = 0; k < SNAP_NSEC; ++k) TRY(io(h, f, shadow && sec[k].kind != SNAP_APPEND ? shadow + h->shadow_off[k] : sec[k].p, sec[k].bytes));
     return 0;
+}
+
+// ---- AGR_CFG_ONLINE_SNAPSHOT
+// The shadow holds every section rewritten in place at full capacity (slab_rows rows, log_entries entries), each at a 256 B
+// boundary behind a 256 B area with the two log lengths the cut read.  Everything is allocated here: nothing is allocated or
+// freed while a snapshot runs (cudaFree would wait for the resident service kernel).
+static int snap_online_create(agr_handle* h) {
+    snap_header cap{};
+    cap.flags = h->cfg.flags & (AGR_CFG_VARLEN | AGR_CFG_RING);
+    cap.rows_used = cap.slab_rows = h->cfg.slab_rows;
+    cap.log_len[0] = cap.log_len[1] = h->d.log_cap;
+    snap_section sec[SNAP_NSEC];
+    snap_table(h, cap, sec);
+    size_t at = 256;
+    for (int k = 0; k < SNAP_NSEC; ++k) {
+        if (sec[k].kind == SNAP_APPEND || sec[k].bytes == 0) continue;
+        h->shadow_off[k] = at;
+        at += (sec[k].bytes + 255) & ~(size_t)255;
+    }
+    TRY(dev_alloc(h, &h->d_shadow, at, false));
+    h->snap_buf_bytes = h->bounce_bytes;
+    for (int b = 0; b < 2; ++b) TRY(host_alloc(h, &h->snap_buf[b], h->snap_buf_bytes));
+    for (auto& e : h->snap_ev) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    // non-blocking: a stream that synchronised with the legacy default stream would also wait behind the resident kernel
+    CK(cudaStreamCreateWithFlags(&h->snap_stream, cudaStreamNonBlocking));
+    return 0;
+}
+// the cut: one kernel copies the per-row words of rows [0, R) and the two log prefixes into the shadow (caller holds HLock)
+static int snap_cut_locked(agr_handle* h, const snap_header& hd) {
+    snap_section sec[SNAP_NSEC];
+    snap_table(h, hd, sec);
+    agr_snap_cut c{};
+    c.shadow = h->d_shadow;
+    int logs[2], nlog = 0;
+    for (int k = 0; k < SNAP_NSEC; ++k) {
+        if (sec[k].kind == SNAP_LOG) logs[nlog++] = k;
+        if (sec[k].kind != SNAP_WORDS || sec[k].bytes == 0) continue;
+        c.src[c.nrow] = (const uint8_t*)sec[k].p; c.dst_off[c.nrow] = h->shadow_off[k]; c.bytes[c.nrow] = sec[k].bytes;
+        c.nrow++;
+    }
+    for (int j = 0; j < 2; ++j) { c.src[c.nrow + j] = (const uint8_t*)sec[logs[j]].p; c.dst_off[c.nrow + j] = h->shadow_off[logs[j]]; }
+    TRY(op_time_begin(h, 3));
+    agr_launch_snap_cut(h->d, c, h->sm_count, h->stream);
+    CK(cudaGetLastError());
+    TRY(op_time_end(h, 3));
+    CK(cudaEventRecord(h->snap_ev[0], h->stream));
+    return 0;
+}
+// writes the chunk waiting in the buffer the next chunk does not use, once its copy has landed
+static int snap_drain(agr_handle* h, FILE* f) {
+    if (!h->snap_pend) return 0;
+    const int b = h->snap_cur ^ 1;
+    const size_t m = h->snap_pend;
+    h->snap_pend = 0;
+    CK(cudaEventSynchronize(h->snap_ev[1 + b]));
+    if (fwrite(h->snap_buf[b], 1, m, f) != m) return fail(AGR_EINVAL, "snapshot: short write");
+    return 0;
+}
+// the online writer's io: chunk k's copy on the writer stream overlaps the fwrite of chunk k - 1 (two pinned buffers)
+static int dump_online(agr_handle* h, FILE* f, void* dsrc, size_t bytes) {
+    for (size_t o = 0; o < bytes;) {
+        const size_t m = std::min(h->snap_buf_bytes, bytes - o);
+        const int b = h->snap_cur;
+        CK(cudaMemcpyAsync(h->snap_buf[b], (const uint8_t*)dsrc + o, m, cudaMemcpyDeviceToHost, h->snap_stream));
+        CK(cudaEventRecord(h->snap_ev[1 + b], h->snap_stream));
+        TRY(snap_drain(h, f));
+        h->snap_cur ^= 1; h->snap_pend = m;
+        o += m;
+    }
+    return 0;
+}
+static void snap_fill_header(agr_handle* h, snap_header& hd) {
+    memcpy(hd.magic, "AGRSNAP3", 8);
+    hd.flags = h->cfg.flags & (AGR_CFG_PERSISTENCE | AGR_CFG_MINT_IDS | AGR_CFG_VARLEN | AGR_CFG_RING);
+    hd.n_agents = (uint32_t)h->agent_names.size(); hd.shard = h->d.shard_id; hd.gen = h->d.id_gen;
+    hd.rows_used = h->rows_used; hd.vused = h->vused; hd.id_secret = h->d.id_secret; hd.scan_lo = h->scan_lo;
+    hd.resp_used = h->resp_used; hd.expired_total = h->expired_total; hd.tail = h->tail; hd.released_total = h->released_total; hd.slab_rows = h->cfg.slab_rows; hd.vtail = h->vtail; hd.vcap = h->vcap; hd.resp_tail = h->resp_tail; hd.resp_cap = h->resp_cap;
+}
+// The handle is held only while the cut is enqueued; the file is written afterwards while every other call goes on.
+static int snapshot_online(agr_handle* h, const char* path) {
+    std::lock_guard<std::mutex> one(h->snap_mu);
+    CK(cudaSetDevice(h->device));
+    FILE* f = fopen(path, "wb");
+    if (!f) return fail(AGR_EINVAL, std::string("snapshot: cannot open ") + path);
+    snap_header hd{};
+    std::vector<char> agents;                                  // the agent table as it was at the cut
+    {
+        HLock lk(h);
+        snap_fill_header(h, hd);
+        agents.assign((size_t)hd.n_agents * (AGR_AGENT_ID_BYTES + 1), 0);
+        for (uint32_t a = 0; a < hd.n_agents; ++a) {
+            char* e = agents.data() + (size_t)a * (AGR_AGENT_ID_BYTES + 1);
+            strncpy(e, h->agent_names[a].c_str(), AGR_AGENT_ID_BYTES - 1);
+            e[AGR_AGENT_ID_BYTES] = (char)h->agent_status[a];
+        }
+        const int rc = snap_cut_locked(h, hd);
+        if (rc < 0) { fclose(f); return rc; }
+        if (is_ring(h)) { h->pinned = true; h->pin_tail = h->tail; h->pin_vtail = h->vtail; h->pin_resp_tail = h->resp_tail; }
+    }
+    auto done = [&](int r) {
+        std::string keep = g_err;
+        if (cudaStreamSynchronize(h->snap_stream) != cudaSuccess && r == 0) { keep = "snapshot: writer stream"; r = AGR_ECUDA; }
+        h->snap_pend = 0; h->snap_cur = 0;
+        { std::lock_guard<std::mutex> g(h->mu); h->pinned = false; }
+        if (fclose(f) != 0 && r == 0) { keep = "snapshot: close failed"; r = AGR_EINVAL; }
+        g_err = keep;
+        return r;
+    };
+    // the writer stream starts behind the cut; the header's log lengths are the ones the cut read
+    if (cudaStreamWaitEvent(h->snap_stream, h->snap_ev[0], 0) != cudaSuccess ||
+        cudaMemcpyAsync(h->snap_buf[0], h->d_shadow, 16, cudaMemcpyDeviceToHost, h->snap_stream) != cudaSuccess ||
+        cudaStreamSynchronize(h->snap_stream) != cudaSuccess) return done(fail(AGR_ECUDA, "snapshot: cut"));
+    memcpy(hd.log_len, h->snap_buf[0], 16);
+    if (fwrite(&hd, sizeof hd, 1, f) != 1 || fwrite(agents.data(), 1, agents.size(), f) != agents.size())
+        return done(fail(AGR_EINVAL, "snapshot: short write"));
+    int rc = snap_sections(h, hd, f, dump_online, h->d_shadow);
+    if (rc == 0) rc = snap_drain(h, f);
+    return done(rc);
 }
 
 int agr_snapshot(agr_handle* h, const char* path) {
     if (!h || !path) return fail(AGR_EINVAL, "NULL argument");
+    if (h->cfg.flags & AGR_CFG_ONLINE_SNAPSHOT) return snapshot_online(h, path);
     HLock lk(h);
     CK(cudaSetDevice(h->device));
     CK(cudaStreamSynchronize(h->stream));
     FILE* f = fopen(path, "wb");
     if (!f) return fail(AGR_EINVAL, std::string("snapshot: cannot open ") + path);
     snap_header hd{};
-    memcpy(hd.magic, "AGRSNAP3", 8);
-    hd.flags = h->cfg.flags & (AGR_CFG_PERSISTENCE | AGR_CFG_MINT_IDS | AGR_CFG_VARLEN | AGR_CFG_RING);
-    hd.n_agents = (uint32_t)h->agent_names.size(); hd.shard = h->d.shard_id; hd.gen = h->d.id_gen;
-    hd.rows_used = h->rows_used; hd.vused = h->vused; hd.id_secret = h->d.id_secret; hd.scan_lo = h->scan_lo;
-    hd.resp_used = h->resp_used; hd.expired_total = h->expired_total; hd.tail = h->tail; hd.released_total = h->released_total; hd.slab_rows = h->cfg.slab_rows; hd.vtail = h->vtail; hd.vcap = h->vcap; hd.resp_tail = h->resp_tail; hd.resp_cap = h->resp_cap;
+    snap_fill_header(h, hd);
     unsigned long long lens[2];
     int rc = 0;
     auto done = [&](int r) { fclose(f); return r; };
@@ -2600,7 +2755,7 @@ int agr_debug_skip_arrivals(agr_handle* h, uint64_t n) {
 }
 
 int agr_op_time(agr_handle* h, int which, double* ms) {
-    if (!h || !ms || which < 0 || which > 2) return fail(AGR_EINVAL, "bad argument");
+    if (!h || !ms || which < 0 || which > 3) return fail(AGR_EINVAL, "bad argument");
     HLock lk(h);
     CK(cudaSetDevice(h->device));
     if (!h->op_timed[which]) return fail(AGR_ENOTFOUND, "no timed launch of that group yet (needs AGR_CFG_TIMING)");

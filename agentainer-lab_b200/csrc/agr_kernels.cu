@@ -1043,6 +1043,40 @@ void agr_launch_drop_agent(const agr_dev& d, uint32_t slot, unsigned long long r
     if (max_log_len) k_drop_logs<<<(unsigned)((max_log_len + 255) / 256), 256, 0, st>>>(d, slot);
 }
 
+// ------------------------------------------------------------------------------------------------ online snapshot cut
+// blockIdx.y = section; the blocks of a section stride over it in 16 B pieces, four independent loads in flight per thread,
+// and block 0 copies the tail (< 16 B).  The log lengths are read here, on the device, so the host never waits to learn them.
+__global__ void __launch_bounds__(256) k_snap_cut(const agr_dev d, const agr_snap_cut c) {
+    const uint32_t s = blockIdx.y;
+    unsigned long long bytes = c.bytes[s];
+    if (s >= c.nrow) {
+        const unsigned long long n = d.log_len[s - c.nrow];
+        bytes = (n < d.log_cap ? n : d.log_cap) * 4ull;
+        if (blockIdx.x == 0 && threadIdx.x == 0) reinterpret_cast<unsigned long long*>(c.shadow)[s - c.nrow] = n;
+    }
+    const uint4* __restrict__ src = reinterpret_cast<const uint4*>(c.src[s]);
+    uint4* __restrict__ dst = reinterpret_cast<uint4*>(c.shadow + c.dst_off[s]);
+    const unsigned long long n16 = bytes >> 4, stride = (unsigned long long)gridDim.x * blockDim.x;
+    unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+    for (; i + 3 * stride < n16; i += 4 * stride) {
+        const uint4 a = src[i], b = src[i + stride], e = src[i + 2 * stride], f = src[i + 3 * stride];
+        dst[i] = a; dst[i + stride] = b; dst[i + 2 * stride] = e; dst[i + 3 * stride] = f;
+    }
+    for (; i < n16; i += stride) dst[i] = src[i];
+    if (blockIdx.x == 0 && threadIdx.x < (bytes & 15u)) {
+        const unsigned long long t = (n16 << 4) + threadIdx.x;
+        c.shadow[c.dst_off[s] + t] = c.src[s][t];
+    }
+}
+void agr_launch_snap_cut(const agr_dev& d, const agr_snap_cut& c, int sm_count, cudaStream_t st) {
+    unsigned long long most = 0;                      // (the logs are at most log_cap entries)
+    for (uint32_t s = 0; s < c.nrow; ++s) most = c.bytes[s] > most ? c.bytes[s] : most;
+    if (d.log_cap * 4ull > most) most = d.log_cap * 4ull;
+    const unsigned long long want = (most / 16 + 1023) / 1024;   // four pieces per thread
+    const uint32_t bx = (uint32_t)(want < 1 ? 1 : want > (unsigned long long)sm_count * 2 ? (unsigned long long)sm_count * 2 : want);
+    k_snap_cut<<<dim3(bx, c.nrow + 2), 256, 0, st>>>(d, c);
+}
+
 // ------------------------------------------------------------------------------------------------ synthetic stream
 __global__ void __launch_bounds__(128) k_synth(uint8_t* dst, const agr_synth_dev s, const unsigned long long first_index, const uint32_t n) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;

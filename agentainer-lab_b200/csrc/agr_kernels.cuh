@@ -216,3 +216,17 @@ void agr_launch_k3_gather(const agr_dev& d, const uint32_t* rids, const uint32_t
 void agr_launch_drop_agent(const agr_dev& d, uint32_t slot, unsigned long long rows, unsigned long long max_log_len,
                            cudaStream_t st);
 void agr_launch_synth(uint8_t* dst, agr_synth_dev s, unsigned long long first_index, uint32_t n, cudaStream_t st);
+
+// Online snapshot (AGR_CFG_ONLINE_SNAPSHOT): the cut copies the sections that later calls rewrite in place (per-row words, the
+// completed / failed logs) into a device shadow.  Every destination is 256 B-aligned; every source is the start of its array.
+// Sections [0, nrow) have the byte counts given here; sections nrow and nrow + 1 are the completed and failed logs, whose
+// lengths the kernel reads from d.log_len and stores as two u64 at the start of the shadow.
+#define AGR_SNAP_CUT_MAX 16
+struct agr_snap_cut {
+    const uint8_t* src[AGR_SNAP_CUT_MAX];
+    unsigned long long dst_off[AGR_SNAP_CUT_MAX];
+    unsigned long long bytes[AGR_SNAP_CUT_MAX];
+    uint8_t* shadow;
+    uint32_t nrow;
+};
+void agr_launch_snap_cut(const agr_dev& d, const agr_snap_cut& c, int sm_count, cudaStream_t st);

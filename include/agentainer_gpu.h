@@ -109,6 +109,10 @@ typedef struct agr_record {
                                        max_batch is clamped to slab_rows / 2).  With caller-supplied ids every agr_reclaim rebuilds the dedupe
                                        index from the live rows.  Without the flag the slab is append-only. */
 #define AGR_CFG_VARLEN        0x10u /* variable-length records (BASELINE config 5): byte-addressed slab, agr_ingest_var / *_var reads */
+#define AGR_CFG_ONLINE_SNAPSHOT 0x80u /* agr_snapshot stops the engine only for a short device-side cut and writes the file while every
+                                       other call goes on (see agr_snapshot).  Costs HBM for the cut's shadow: 64 B per slab row
+                                       (+ 12 B with AGR_CFG_VARLEN) and 8 B per log_entries, about 88 B per row with the defaults;
+                                       agr_create returns AGR_ENOMEM when that does not fit. */
 #define AGR_CFG_DIAG_NO_INDEX  0x100u /* DIAGNOSTIC ONLY (results invalid): K1 skips the dedupe-index insert, to attribute kernel time */
 #define AGR_CFG_DIAG_NO_CKSUM  0x200u /* DIAGNOSTIC ONLY (results invalid): K1 skips the record checksum */
 #define AGR_CFG_SKIP_INFLIGHT 0x2u  /* EXTENSION, off in parity mode: replay scan skips records whose forward is still in flight (fixes Q16) */
@@ -387,7 +391,19 @@ int agr_json_decode(const uint8_t* json, uint32_t len, uint8_t* record, uint32_t
 /* What Redis persistence gave the reference (records and queues survive a server restart, docker-compose.yml:11-12):
  * agr_snapshot writes the live state (slab rows, per-row state words, completed / failed logs, agent table) to a file;
  * agr_restore creates a new engine from it (cfg gives the capacities; id mode and record form must match the snapshot).
- * In hash-id mode the dedupe index is not stored: it is rebuilt on the device from the restored rows. */
+ * In hash-id mode the dedupe index is not stored: it is rebuilt on the device from the restored rows.
+ * Without AGR_CFG_ONLINE_SNAPSHOT every other call waits until the last byte is written.  With it, agr_snapshot holds the
+ * engine only while it enqueues the CUT: one kernel copies the per-row words and the completed / failed logs into a device
+ * shadow, and the host takes the header fields and the agent table.  The file is then written while every other call goes on
+ * (the single-request front end included); it is the engine's state at the cut, in the same format, read by the same
+ * agr_restore.  Slab rows, record bytes and response bytes are streamed from where they lie: until the file is written an
+ * AGR_CFG_RING engine does not reuse rows or bytes of the cut's window, even once agr_reclaim has released them — a reservation
+ * that would reach them fails with AGR_ENOSPC (agr_last_error names the snapshot).  A second agr_snapshot on the same engine
+ * waits for the first.  The file's bytes are unspecified (whatever the slab holds when they are read; a restore treats them as
+ * empty, as it treats what a blocking snapshot writes there) for rows that hold no record at the cut — rows outside
+ * [rows_tail, rows_used), rows skipped at the end of a lap, rows reserved and not ingested — and for byte-ring bytes outside
+ * the record bytes' and the response bytes' live ranges.  agr_snapshot returns once the file is written; a failure at any
+ * point releases the pinned window. */
 int agr_snapshot(agr_handle* h, const char* path);
 int agr_restore(const agr_config* cfg, const char* path, agr_handle** out);
 /* The 24 h TTL of the record keys (SET ... EX 24h at requests.go:106,175,270; every SET restarts it, Q11).  Times are the
@@ -455,7 +471,8 @@ void* agr_stream(agr_handle* h);                 /* cudaStream_t the kernels run
 int agr_kernel_time(agr_handle* h, double* sum_ms, uint64_t* launches);
 /* With AGR_CFG_TIMING: device time (CUDA events on the launching stream) of the most recent kernel group:
  * which = 0 the K2 kernels of the last agr_complete, 1 the K3 select kernels of the last scan / pending / list,
- * 2 the K5 kernels of the last JSON encode (measure + scan + emit, including the host's read of the total between them). */
+ * 2 the K5 kernels of the last JSON encode (measure + scan + emit, including the host's read of the total between them),
+ * 3 the cut of the last agr_snapshot with AGR_CFG_ONLINE_SNAPSHOT. */
 int agr_op_time(agr_handle* h, int which, double* ms);
 void* agr_slab_ptr(agr_handle* h, uint64_t rid); /* device address of a slab row */
 
