@@ -8,9 +8,11 @@
 #include <dlfcn.h>
 #include <sys/random.h>
 #include <nccl.h>      // types only: every NCCL symbol is resolved with dlopen/dlsym at run time
+#include <limits.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
+#include <sys/stat.h>
 #include <string.h>
 
 #include <algorithm>
@@ -64,6 +66,22 @@ template <typename T>
 struct scratch {
     T* p = nullptr;
     size_t cap = 0;
+};
+
+// the header of a full snapshot file (agr_snapshot); a delta file carries the one of its cut
+struct snap_header {
+    char magic[8];                 // "AGRSNAP3"
+    uint32_t flags, n_agents, shard, gen;
+    uint64_t rows_used, vused, log_len[2], id_secret, scan_lo, resp_used, expired_total, tail, released_total, slab_rows, vtail, vcap, resp_tail, resp_cap;
+};
+// AGR_CFG_DELTA_SNAPSHOT: what the next snapshot builds on — the files since the last full one (absolute paths, oldest
+// first), the full file's size and the deltas' total, the last cut's header, its ingested bound and its digest
+struct snap_chain {
+    std::vector<std::string> paths;
+    uint64_t full_bytes = 0, delta_bytes = 0;
+    snap_header base{};
+    uint64_t base_bound = 0;
+    unsigned long long digest[2] = {0, 0};
 };
 
 struct agr_handle {
@@ -171,6 +189,13 @@ struct agr_handle {
     int snap_cur = 0; size_t snap_pend = 0;                 // buffer of the next chunk; bytes of the chunk waiting in the other one
     std::mutex snap_mu;                                      // one online snapshot at a time: there is one shadow
     bool pinned = false; uint64_t pin_tail = 0, pin_vtail = 0, pin_resp_tail = 0;   // (h->mu) the cut's ring tails while it is written
+    // AGR_CFG_DELTA_SNAPSHOT (and a restore that applies deltas): the compare cut's dirty bits (word blocks, then the completed
+    // and failed logs' blocks at snap_bit_off[1], [2]) and digest, the pinned copy the writer reads them from (the two log
+    // lengths and the digest first), the device block list and the staging buffer of the block gather / scatter
+    uint32_t* d_snap_bits = nullptr; unsigned long long* d_snap_digest = nullptr; uint8_t* h_snap_bits = nullptr;
+    size_t snap_bit_off[3] = {}, snap_bit_words = 0;
+    uint32_t* d_snap_list = nullptr; uint8_t* d_snap_stage = nullptr; size_t snap_stage_bytes = 0;
+    snap_chain chain;                                        // (snap_mu) empty: the next snapshot is a full file
 };
 #define AGR_TIMING_RING 1024
 
@@ -704,6 +729,8 @@ static int create_impl(const agr_config* cfg_in, agr_handle* h) {
     if (c.flags == 0) c.flags = AGR_CFG_PERSISTENCE;
     if (c.slab_rows == 0) c.slab_rows = 1ull << 20;
     if (c.slab_rows >= 0x7fffffffull) return fail(AGR_EINVAL, "slab_rows must be < 2^31");
+    if ((c.flags & AGR_CFG_DELTA_SNAPSHOT) && !(c.flags & AGR_CFG_ONLINE_SNAPSHOT))
+        return fail(AGR_EINVAL, "AGR_CFG_DELTA_SNAPSHOT needs AGR_CFG_ONLINE_SNAPSHOT (the delta is taken by the online cut)");
     const bool mint = (c.flags & AGR_CFG_MINT_IDS) != 0;
     if (mint) c.table_slots = 64;                               // no dedupe index in this mode (a stub keeps pointers valid)
     if (c.table_slots == 0) c.table_slots = next_pow2(c.slab_rows * 2);
@@ -1866,11 +1893,6 @@ int agr_get_record_json(agr_handle* h, const char* agent_id, const uint8_t reque
 }
 
 // ------------------------------------------------------------------------------------------ durability
-struct snap_header {
-    char magic[8];                 // "AGRSNAP3"
-    uint32_t flags, n_agents, shard, gen;
-    uint64_t rows_used, vused, log_len[2], id_secret, scan_lo, resp_used, expired_total, tail, released_total, slab_rows, vtail, vcap, resp_tail, resp_cap;
-};
 static int dump_dev(agr_handle* h, FILE* f, void* dsrc, size_t bytes) {
     const size_t chunk = h->bounce_bytes;
     for (size_t o = 0; o < bytes; o += chunk) {
@@ -1939,6 +1961,152 @@ static int snap_sections(agr_handle* h, const snap_header& hd, FILE* f, int (*io
     return 0;
 }
 
+// ---- AGR_CFG_DELTA_SNAPSHOT
+// A delta file (AGRDELT1): this header; the parent's absolute path; the agent table, as in a full file; the appended slab rows
+// (record bytes with AGR_CFG_VARLEN) [rows_lo, rows_hi), then the appended response bytes [resp_lo, resp_hi), both in physical
+// order, in one run or two where the ring wraps; the ascending list of dirty word blocks (u32), then each listed block's slice
+// of every SNAP_WORDS section of snap_table, in table order; then per log (completed, failed) the same for its dirty log
+// blocks.  Only the last block of a section may be short.  The digests are the compare cut's keyed sums over the word
+// sections [0, R) and the log prefixes of the parent's cut and of this one.
+#define SNAP_BLOCK_ROWS 256u
+#define SNAP_LOG_BLOCK 1024u
+struct delta_header {
+    char magic[8];                 // "AGRDELT1"
+    snap_header cut;               // the state this file brings a restore to
+    uint64_t file_bytes;           // a restore refuses a shorter file
+    unsigned long long parent_digest[2], digest[2];
+    uint32_t block_rows, log_block;
+    uint64_t rows_lo, rows_hi, resp_lo, resp_hi;
+    uint64_t n_blocks, n_log_blocks[2];
+    uint32_t parent_path_len, pad;
+};
+static_assert(sizeof(delta_header) == 264 && sizeof(snap_header) == 144, "delta_header is a file layout");
+
+// Everything the compare cut, the gather and the scatter use; allocated at agr_create (or by the restore of a delta chain)
+static int snap_delta_alloc(agr_handle* h) {
+    if (h->d_snap_stage) return 0;
+    const size_t nwb = (h->cfg.slab_rows + SNAP_BLOCK_ROWS - 1) / SNAP_BLOCK_ROWS, nlb = (h->d.log_cap + SNAP_LOG_BLOCK - 1) / SNAP_LOG_BLOCK;
+    h->snap_bit_off[1] = (nwb + 31) / 32; h->snap_bit_off[2] = h->snap_bit_off[1] + (nlb + 31) / 32;
+    h->snap_bit_words = h->snap_bit_off[2] + (nlb + 31) / 32;
+    TRY(dev_alloc(h, &h->d_snap_bits, h->snap_bit_words, false));
+    TRY(dev_alloc(h, &h->d_snap_digest, (size_t)2, false));
+    TRY(host_alloc(h, &h->h_snap_bits, 32 + h->snap_bit_words * 4));
+    TRY(dev_alloc(h, &h->d_snap_list, std::max<size_t>(std::max(nwb, nlb), 1), false));
+    h->snap_stage_bytes = std::max<size_t>(h->bounce_bytes, (size_t)1 << 20);   // >= one block of every section
+    TRY(dev_alloc(h, &h->d_snap_stage, h->snap_stage_bytes, false));
+    return 0;
+}
+static size_t snap_full_bytes(agr_handle* h, const snap_header& hd) {
+    snap_section sec[SNAP_NSEC];
+    snap_table(h, hd, sec);
+    size_t n = sizeof(snap_header) + (size_t)hd.n_agents * (AGR_AGENT_ID_BYTES + 1);
+    for (int k = 0; k < SNAP_NSEC; ++k) n += sec[k].bytes;
+    return n;
+}
+// The compare cut's sections: the SNAP_WORDS ones that hold bytes, then the two logs (whose lengths the kernel reads on the
+// device unless lens_from_host).  A word block is 256 rows: 16 * width pieces of 16 B; a log block 1024 entries: 256 pieces.
+static void snap_cmp_params(agr_handle* h, const snap_header& hd, bool lens_from_host, agr_snap_cmp& c) {
+    snap_section sec[SNAP_NSEC];
+    snap_table(h, hd, sec);
+    const size_t R = snap_rows(hd);
+    c = agr_snap_cmp{};
+    c.shadow = h->d_shadow; c.bits = h->d_snap_bits; c.digest = h->d_snap_digest; c.key = h->d.id_secret;
+    c.lens_from_host = lens_from_host ? 1u : 0u;
+    int logs[2], nlog = 0;
+    for (int k = 0; k < SNAP_NSEC; ++k) {
+        if (sec[k].kind == SNAP_LOG) logs[nlog++] = k;
+        if (sec[k].kind != SNAP_WORDS || sec[k].bytes == 0) continue;
+        const uint32_t n = c.nrow++;
+        c.src[n] = (const uint8_t*)sec[k].p; c.dst_off[n] = h->shadow_off[k]; c.bytes[n] = sec[k].bytes;
+        c.pshift[n] = (uint32_t)__builtin_ctzll(16 * (sec[k].bytes / R)); c.bit_off[n] = 0; c.sec_id[n] = (uint32_t)k;
+    }
+    for (int j = 0; j < 2; ++j) {
+        const uint32_t n = c.nrow + j;
+        c.src[n] = (const uint8_t*)sec[logs[j]].p; c.dst_off[n] = h->shadow_off[logs[j]]; c.bytes[n] = sec[logs[j]].bytes;
+        c.pshift[n] = 8; c.bit_off[n] = (uint32_t)h->snap_bit_off[1 + j]; c.sec_id[n] = (uint32_t)logs[j];
+    }
+}
+// the compare cut (caller holds HLock): the cut of snap_cut_locked that also marks the blocks that differ from the previous
+// cut and sums the digest of this one
+static int snap_cmp_cut_locked(agr_handle* h, const snap_header& hd) {
+    agr_snap_cmp c;
+    snap_cmp_params(h, hd, false, c);
+    CK(cudaMemsetAsync(h->d_snap_bits, 0, h->snap_bit_words * 4, h->stream));
+    CK(cudaMemsetAsync(h->d_snap_digest, 0, 16, h->stream));
+    TRY(op_time_begin(h, 3));
+    agr_launch_snap_cmp(h->d, c, true, h->sm_count, h->stream);
+    CK(cudaGetLastError());
+    TRY(op_time_end(h, 3));
+    CK(cudaEventRecord(h->snap_ev[0], h->stream));
+    return 0;
+}
+// (restore) the digest of the live arrays as hd describes them.  seed: through the compare cut, which also leaves them in the
+// shadow, so that the next snapshot of an AGR_CFG_DELTA_SNAPSHOT engine compares against the restored state
+static int snap_digest_locked(agr_handle* h, const snap_header& hd, bool seed, unsigned long long out[2]) {
+    agr_snap_cmp c;
+    snap_cmp_params(h, hd, !seed, c);
+    if (seed) CK(cudaMemsetAsync(h->d_snap_bits, 0, h->snap_bit_words * 4, h->stream));
+    CK(cudaMemsetAsync(h->d_snap_digest, 0, 16, h->stream));
+    agr_launch_snap_cmp(h->d, c, seed, h->sm_count, h->stream);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(h->h_snap_bits, h->d_snap_digest, 16, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    memcpy(out, h->h_snap_bits, 16);
+    return 0;
+}
+// The block tables of a delta: the word sections of hd (256 rows per block), or log j (1024 entries per block), in the shadow
+// (the writer) or the live arrays (restore)
+static agr_snap_blocks snap_word_blocks(agr_handle* h, const snap_header& hd, bool shadow) {
+    snap_section sec[SNAP_NSEC];
+    snap_table(h, hd, sec);
+    agr_snap_blocks g{};
+    g.block_rows = SNAP_BLOCK_ROWS; g.rows = snap_rows(hd);
+    for (int k = 0; k < SNAP_NSEC; ++k) {
+        if (sec[k].kind != SNAP_WORDS || sec[k].bytes == 0) continue;
+        g.arr[g.nsec] = shadow ? h->d_shadow + h->shadow_off[k] : (uint8_t*)sec[k].p;
+        g.width[g.nsec] = (uint32_t)(sec[k].bytes / g.rows);
+        g.rec_bytes += (unsigned long long)g.width[g.nsec] * SNAP_BLOCK_ROWS;
+        g.nsec++;
+    }
+    return g;
+}
+static agr_snap_blocks snap_log_blocks(agr_handle* h, const snap_header& hd, int j, bool shadow) {
+    snap_section sec[SNAP_NSEC];
+    snap_table(h, hd, sec);
+    agr_snap_blocks g{};
+    for (int k = 0, seen = 0; k < SNAP_NSEC; ++k) {
+        if (sec[k].kind != SNAP_LOG || seen++ != j) continue;
+        g.arr[0] = shadow ? h->d_shadow + h->shadow_off[k] : (uint8_t*)sec[k].p;
+    }
+    g.nsec = 1; g.width[0] = 4; g.block_rows = SNAP_LOG_BLOCK; g.rows = hd.log_len[j]; g.rec_bytes = 4ull * SNAP_LOG_BLOCK;
+    return g;
+}
+// bytes of the slices of n listed blocks (only the table's last block may be short)
+static uint64_t snap_blocks_bytes(const agr_snap_blocks& g, const uint32_t* list, size_t n) {
+    if (!n) return 0;
+    const uint64_t last = list[n - 1], r0 = last * g.block_rows;
+    return (n - 1) * g.rec_bytes + std::min<uint64_t>(g.block_rows, g.rows - r0) * (g.rec_bytes / g.block_rows);
+}
+// the physical runs (start, count) of the logical range [lo, hi) of a ring of cap units (one run without AGR_CFG_RING)
+static int snap_runs(uint64_t lo, uint64_t hi, uint64_t cap, bool ring, uint64_t run[2][2]) {
+    if (hi <= lo) return 0;
+    const uint64_t p = ring ? lo % cap : lo, n0 = ring ? std::min(hi - lo, cap - p) : hi - lo;
+    run[0][0] = p; run[0][1] = n0;
+    if (hi - lo == n0) return 1;
+    run[1][0] = 0; run[1][1] = hi - lo - n0;
+    return 2;
+}
+// the absolute name a chain keeps of a file: realpath of its directory, then its name ("" if the directory does not resolve)
+static std::string snap_abs_path(const std::string& p) {
+    const size_t cut = p.rfind('/');
+    const std::string dir = cut == std::string::npos ? "." : (cut == 0 ? "/" : p.substr(0, cut));
+    char buf[PATH_MAX];
+    if (!realpath(dir.c_str(), buf)) return "";
+    std::string out(buf);
+    if (out.back() != '/') out += '/';
+    return out + (cut == std::string::npos ? p : p.substr(cut + 1));
+}
+
 // ---- AGR_CFG_ONLINE_SNAPSHOT
 // The shadow holds every section rewritten in place at full capacity (slab_rows rows, log_entries entries), each at a 256 B
 // boundary behind a 256 B area with the two log lengths the cut read.  Everything is allocated here: nothing is allocated or
@@ -1962,6 +2130,7 @@ static int snap_online_create(agr_handle* h) {
     for (auto& e : h->snap_ev) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
     // non-blocking: a stream that synchronised with the legacy default stream would also wait behind the resident kernel
     CK(cudaStreamCreateWithFlags(&h->snap_stream, cudaStreamNonBlocking));
+    if (h->cfg.flags & AGR_CFG_DELTA_SNAPSHOT) TRY(snap_delta_alloc(h));
     return 0;
 }
 // the cut: one kernel copies the per-row words of rows [0, R) and the two log prefixes into the shadow (caller holds HLock)
@@ -2015,14 +2184,111 @@ static void snap_fill_header(agr_handle* h, snap_header& hd) {
     hd.rows_used = h->rows_used; hd.vused = h->vused; hd.id_secret = h->d.id_secret; hd.scan_lo = h->scan_lo;
     hd.resp_used = h->resp_used; hd.expired_total = h->expired_total; hd.tail = h->tail; hd.released_total = h->released_total; hd.slab_rows = h->cfg.slab_rows; hd.vtail = h->vtail; hd.vcap = h->vcap; hd.resp_tail = h->resp_tail; hd.resp_cap = h->resp_cap;
 }
+// the writer: the list, then the listed blocks of g, packed on the writer stream into the staging buffer (stream order keeps
+// a chunk's copies ahead of the next chunk's gather) and streamed through the pinned buffers
+static int dump_blocks(agr_handle* h, FILE* f, agr_snap_blocks g, const std::vector<uint32_t>& list) {
+    TRY(snap_drain(h, f));
+    if (list.empty()) return 0;
+    if (fwrite(list.data(), 4, list.size(), f) != list.size()) return fail(AGR_EINVAL, "snapshot: short write");
+    CK(cudaMemcpyAsync(h->d_snap_list, list.data(), list.size() * 4, cudaMemcpyHostToDevice, h->snap_stream));
+    const size_t per = h->snap_stage_bytes / g.rec_bytes;
+    g.stage = h->d_snap_stage;
+    for (size_t j = 0; j < list.size(); j += per) {
+        const size_t n = std::min(per, list.size() - j);
+        g.list = h->d_snap_list + j;
+        agr_launch_snap_blocks(g, (uint32_t)n, true, h->snap_stream);
+        CK(cudaGetLastError());
+        TRY(dump_online(h, f, h->d_snap_stage, snap_blocks_bytes(g, list.data() + j, n)));
+    }
+    return 0;
+}
+// AGR_CFG_DELTA_SNAPSHOT: reads the compare cut's log lengths, digest and dirty bits, then writes a delta on the chain's last
+// file, or a full file when there is no chain, path is one of its files, or the deltas would outgrow a full file
+static int snap_write_chain(agr_handle* h, FILE* f, const char* path, snap_header& hd, const std::vector<char>& agents, uint64_t bound) {
+    if (cudaStreamWaitEvent(h->snap_stream, h->snap_ev[0], 0) != cudaSuccess ||
+        cudaMemcpyAsync(h->h_snap_bits, h->d_shadow, 16, cudaMemcpyDeviceToHost, h->snap_stream) != cudaSuccess ||
+        cudaMemcpyAsync(h->h_snap_bits + 16, h->d_snap_digest, 16, cudaMemcpyDeviceToHost, h->snap_stream) != cudaSuccess ||
+        cudaMemcpyAsync(h->h_snap_bits + 32, h->d_snap_bits, h->snap_bit_words * 4, cudaMemcpyDeviceToHost, h->snap_stream) != cudaSuccess ||
+        cudaStreamSynchronize(h->snap_stream) != cudaSuccess) return fail(AGR_ECUDA, "snapshot: cut");
+    memcpy(hd.log_len, h->h_snap_bits, 16);
+    unsigned long long digest[2];
+    memcpy(digest, h->h_snap_bits + 16, 16);
+    const uint32_t* bits = reinterpret_cast<const uint32_t*>(h->h_snap_bits + 32);
+    const std::string at = snap_abs_path(path);
+    if (at.empty()) return fail(AGR_EINVAL, std::string("snapshot: cannot resolve the directory of ") + path);
+    snap_chain& ch = h->chain;
+    const size_t full = snap_full_bytes(h, hd);
+    bool delta = !ch.paths.empty() && std::find(ch.paths.begin(), ch.paths.end(), at) == ch.paths.end();
+    delta_header dh{};
+    std::vector<uint32_t> wl, ll[2];
+    const bool var = (hd.flags & AGR_CFG_VARLEN) != 0, ring = (hd.flags & AGR_CFG_RING) != 0;
+    const uint64_t unit = var ? 1 : AGR_REC;
+    agr_snap_blocks gw = snap_word_blocks(h, hd, true), gl[2] = {snap_log_blocks(h, hd, 0, true), snap_log_blocks(h, hd, 1, true)};
+    if (delta) {
+        const snap_header& b = ch.base;
+        memcpy(dh.magic, "AGRDELT1", 8);
+        dh.cut = hd;
+        memcpy(dh.parent_digest, ch.digest, 16); memcpy(dh.digest, digest, 16);
+        dh.block_rows = SNAP_BLOCK_ROWS; dh.log_block = SNAP_LOG_BLOCK;
+        // appended since the parent's cut: from the first row (byte) it did not hold yet, clipped to this cut's window
+        dh.rows_hi = var ? hd.vused : hd.rows_used;
+        dh.rows_lo = std::min(dh.rows_hi, std::max(var ? b.vused : ch.base_bound, var ? hd.vtail : hd.tail));
+        dh.resp_hi = hd.resp_used;
+        dh.resp_lo = std::min(dh.resp_hi, std::max(b.resp_used, hd.resp_tail));
+        // dirty blocks, and every block that reaches past what the parent's cut held (the shadow has nothing of it there)
+        const uint64_t R = snap_rows(hd), first_new = snap_rows(b) / SNAP_BLOCK_ROWS;
+        for (uint64_t k = 0; k * SNAP_BLOCK_ROWS < R; ++k)
+            if (k >= first_new || ((bits[k >> 5] >> (k & 31)) & 1u)) wl.push_back((uint32_t)k);
+        for (int j = 0; j < 2; ++j) {
+            const uint32_t* lb = bits + h->snap_bit_off[1 + j];
+            const uint64_t lnew = b.log_len[j] / SNAP_LOG_BLOCK;
+            for (uint64_t k = 0; k * SNAP_LOG_BLOCK < hd.log_len[j]; ++k)
+                if (k >= lnew || ((lb[k >> 5] >> (k & 31)) & 1u)) ll[j].push_back((uint32_t)k);
+        }
+        dh.n_blocks = wl.size(); dh.n_log_blocks[0] = ll[0].size(); dh.n_log_blocks[1] = ll[1].size();
+        dh.parent_path_len = (uint32_t)ch.paths.back().size();
+        dh.file_bytes = sizeof dh + dh.parent_path_len + agents.size() + (dh.rows_hi - dh.rows_lo) * unit + (dh.resp_hi - dh.resp_lo)
+                        + 4 * wl.size() + snap_blocks_bytes(gw, wl.data(), wl.size());
+        for (int j = 0; j < 2; ++j) dh.file_bytes += 4 * ll[j].size() + snap_blocks_bytes(gl[j], ll[j].data(), ll[j].size());
+        delta = ch.delta_bytes + dh.file_bytes <= full;              // else a full file: a restore reads at most ~2 full files
+    }
+    if (!delta) {
+        if (fwrite(&hd, sizeof hd, 1, f) != 1 || fwrite(agents.data(), 1, agents.size(), f) != agents.size())
+            return fail(AGR_EINVAL, "snapshot: short write");
+        TRY(snap_sections(h, hd, f, dump_online, h->d_shadow));
+        TRY(snap_drain(h, f));
+        ch = snap_chain{};
+        ch.full_bytes = full;
+    } else {
+        const std::string& parent = ch.paths.back();
+        if (fwrite(&dh, sizeof dh, 1, f) != 1 || fwrite(parent.data(), 1, parent.size(), f) != parent.size() ||
+            fwrite(agents.data(), 1, agents.size(), f) != agents.size()) return fail(AGR_EINVAL, "snapshot: short write");
+        uint64_t run[2][2];
+        for (int n = snap_runs(dh.rows_lo, dh.rows_hi, var ? hd.vcap : hd.slab_rows, ring, run), j = 0; j < n; ++j)
+            TRY(dump_online(h, f, h->d.slab + run[j][0] * unit, run[j][1] * unit));
+        for (int n = snap_runs(dh.resp_lo, dh.resp_hi, hd.resp_cap, ring, run), j = 0; j < n; ++j)
+            TRY(dump_online(h, f, h->d_resp + run[j][0], run[j][1]));
+        TRY(dump_blocks(h, f, gw, wl));
+        for (int j = 0; j < 2; ++j) TRY(dump_blocks(h, f, gl[j], ll[j]));
+        TRY(snap_drain(h, f));
+        ch.delta_bytes += dh.file_bytes;
+    }
+    ch.paths.push_back(at);
+    ch.base = hd; ch.base_bound = bound;
+    memcpy(ch.digest, digest, 16);
+    return 0;
+}
+
 // The handle is held only while the cut is enqueued; the file is written afterwards while every other call goes on.
 static int snapshot_online(agr_handle* h, const char* path) {
     std::lock_guard<std::mutex> one(h->snap_mu);
     CK(cudaSetDevice(h->device));
     FILE* f = fopen(path, "wb");
     if (!f) return fail(AGR_EINVAL, std::string("snapshot: cannot open ") + path);
+    const bool chain = (h->cfg.flags & AGR_CFG_DELTA_SNAPSHOT) != 0;
     snap_header hd{};
     std::vector<char> agents;                                  // the agent table as it was at the cut
+    uint64_t bound = 0;                                        // rows below were ingested at the cut
     {
         HLock lk(h);
         snap_fill_header(h, hd);
@@ -2032,8 +2298,9 @@ static int snapshot_online(agr_handle* h, const char* path) {
             strncpy(e, h->agent_names[a].c_str(), AGR_AGENT_ID_BYTES - 1);
             e[AGR_AGENT_ID_BYTES] = (char)h->agent_status[a];
         }
-        const int rc = snap_cut_locked(h, hd);
-        if (rc < 0) { fclose(f); return rc; }
+        bound = ingested_bound(h);
+        const int rc = chain ? snap_cmp_cut_locked(h, hd) : snap_cut_locked(h, hd);
+        if (rc < 0) { fclose(f); h->chain = snap_chain{}; return rc; }
         if (is_ring(h)) { h->pinned = true; h->pin_tail = h->tail; h->pin_vtail = h->vtail; h->pin_resp_tail = h->resp_tail; }
     }
     auto done = [&](int r) {
@@ -2042,9 +2309,11 @@ static int snapshot_online(agr_handle* h, const char* path) {
         h->snap_pend = 0; h->snap_cur = 0;
         { std::lock_guard<std::mutex> g(h->mu); h->pinned = false; }
         if (fclose(f) != 0 && r == 0) { keep = "snapshot: close failed"; r = AGR_EINVAL; }
+        if (r != 0) h->chain = snap_chain{};                    // a file that failed is no base: the next one is full
         g_err = keep;
         return r;
     };
+    if (chain) return done(snap_write_chain(h, f, path, hd, agents, bound));
     // the writer stream starts behind the cut; the header's log lengths are the ones the cut read
     if (cudaStreamWaitEvent(h->snap_stream, h->snap_ev[0], 0) != cudaSuccess ||
         cudaMemcpyAsync(h->snap_buf[0], h->d_shadow, 16, cudaMemcpyDeviceToHost, h->snap_stream) != cudaSuccess ||
@@ -2082,11 +2351,158 @@ int agr_snapshot(agr_handle* h, const char* path) {
     return done(0);
 }
 
+// ---- restore: a full file, then the deltas of its chain, oldest first
+// The agent table of a file: entry a is slot a.  An agent the engine already has (registered before the parent's cut) keeps its
+// name and slot, and only its status changes; a new one is registered in table order, so that the slots match.
+static int restore_agents_locked(agr_handle* h, FILE* f, uint32_t n) {
+    for (uint32_t a = 0; a < n; ++a) {
+        char name[AGR_AGENT_ID_BYTES]; uint8_t st;
+        if (fread(name, 1, AGR_AGENT_ID_BYTES, f) != AGR_AGENT_ID_BYTES || fread(&st, 1, 1, f) != 1) return fail(AGR_EINVAL, "restore: short read");
+        name[AGR_AGENT_ID_BYTES - 1] = 0;
+        const bool removed = (st == AG_STATUS_REMOVED), known = a < h->agent_names.size();
+        if (known && h->agent_names[a] != name) return fail(AGR_EINVAL, "restore: the agent table of a delta does not extend its parent's");
+        if (!known || !removed) {
+            const int s = set_agent_state_locked(h, name, removed ? (uint8_t)AGR_AGENT_STOPPED : st, true);
+            if (s < 0) return s;
+            if ((uint32_t)s != a) return fail(AGR_EINVAL, "restore: an agent appears twice in the agent table");
+        }
+        if (removed) { h->agent_status[a] = AG_STATUS_REMOVED; TRY(push_agent_status(h, a, AG_STATUS_REMOVED)); }
+    }
+    return 0;
+}
+// the scatter: n listed blocks of g, read from the file chunk by chunk into the staging buffer and placed into the live arrays
+static int load_blocks(agr_handle* h, FILE* f, agr_snap_blocks g, uint64_t n) {
+    const uint64_t nb = (g.rows + g.block_rows - 1) / g.block_rows;
+    if (n > nb) return fail(AGR_EINVAL, "restore: corrupt delta (more blocks listed than its sections have)");
+    std::vector<uint32_t> list(n);
+    if (n && fread(list.data(), 4, n, f) != n) return fail(AGR_EINVAL, "restore: short read");
+    for (size_t j = 0; j < n; ++j)
+        if (list[j] >= nb || (j && list[j] <= list[j - 1])) return fail(AGR_EINVAL, "restore: corrupt delta (block list)");
+    if (!n) return 0;
+    CK(cudaMemcpyAsync(h->d_snap_list, list.data(), n * 4, cudaMemcpyHostToDevice, h->stream));
+    const size_t per = h->snap_stage_bytes / g.rec_bytes;
+    g.stage = h->d_snap_stage;
+    for (size_t j = 0; j < n; j += per) {
+        const size_t m = std::min<size_t>(per, n - j);
+        TRY(load_dev(h, f, h->d_snap_stage, snap_blocks_bytes(g, list.data() + j, m)));   // (stream-ordered after the last scatter)
+        g.list = h->d_snap_list + j;
+        agr_launch_snap_blocks(g, (uint32_t)m, false, h->stream);
+        CK(cudaGetLastError());
+    }
+    CK(cudaStreamSynchronize(h->stream));
+    return 0;
+}
+// applies one delta (f is past its header and parent path) to the live arrays; the header fields are set by the caller
+static int restore_delta_locked(agr_handle* h, FILE* f, const delta_header& dh) {
+    const snap_header& hd = dh.cut;
+    const bool var = (hd.flags & AGR_CFG_VARLEN) != 0, ring = (hd.flags & AGR_CFG_RING) != 0;
+    const uint64_t unit = var ? 1 : AGR_REC;
+    TRY(restore_agents_locked(h, f, hd.n_agents));
+    uint64_t run[2][2];
+    for (int n = snap_runs(dh.rows_lo, dh.rows_hi, var ? hd.vcap : hd.slab_rows, ring, run), j = 0; j < n; ++j)
+        TRY(load_dev(h, f, h->d.slab + run[j][0] * unit, run[j][1] * unit));
+    for (int n = snap_runs(dh.resp_lo, dh.resp_hi, hd.resp_cap, ring, run), j = 0; j < n; ++j)
+        TRY(load_dev(h, f, h->d_resp + run[j][0], run[j][1]));
+    TRY(load_blocks(h, f, snap_word_blocks(h, hd, false), dh.n_blocks));
+    for (int j = 0; j < 2; ++j) TRY(load_blocks(h, f, snap_log_blocks(h, hd, j, false), dh.n_log_blocks[j]));
+    if ((uint64_t)ftello(f) != dh.file_bytes) return fail(AGR_EINVAL, "restore: corrupt delta (its sections do not add up to its size)");
+    return 0;
+}
+// Follows the parent paths from path back to a full file: files[0] is that file, files[k] (k >= 1) the delta dh[k - 1].
+static int restore_chain(const char* path, std::vector<std::string>& files, std::vector<delta_header>& dh) {
+    std::string p = path;
+    for (;;) {
+        const std::string of = files.empty() ? "" : ", the parent of " + files.front();
+        if (files.size() > 65536) return fail(AGR_EINVAL, "restore: the chain of parents does not end in a full file");
+        FILE* f = fopen(p.c_str(), "rb");
+        if (!f) return fail(AGR_EINVAL, "restore: cannot open " + p + of);
+        char magic[8] = {0};
+        const bool got = fread(magic, 1, 8, f) == 8;
+        if (got && memcmp(magic, "AGRSNAP3", 8) == 0) { fclose(f); files.insert(files.begin(), p); return 0; }
+        if (!got || memcmp(magic, "AGRDELT1", 8) != 0) { fclose(f); return fail(AGR_EINVAL, files.empty() ? "restore: not a snapshot" : "restore: " + p + of + ", is not a snapshot"); }
+        delta_header d{};
+        struct stat st{};
+        rewind(f);
+        const bool ok = fread(&d, sizeof d, 1, f) == 1 && fstat(fileno(f), &st) == 0;
+        std::string parent(ok && d.parent_path_len <= PATH_MAX ? d.parent_path_len : 0, '\0');
+        const bool named = ok && d.parent_path_len && d.parent_path_len <= PATH_MAX && fread(&parent[0], 1, parent.size(), f) == parent.size();
+        fclose(f);
+        if (!ok || (uint64_t)st.st_size < d.file_bytes) return fail(AGR_EINVAL, "restore: " + p + of + " is shorter than its header says (truncated)");
+        const bool var = (d.cut.flags & AGR_CFG_VARLEN) != 0;
+        if (!named || d.block_rows != SNAP_BLOCK_ROWS || d.log_block != SNAP_LOG_BLOCK || d.rows_lo > d.rows_hi ||
+            d.rows_hi != (var ? d.cut.vused : d.cut.rows_used) || d.resp_lo > d.resp_hi || d.resp_hi != d.cut.resp_used ||
+            d.rows_hi - d.rows_lo > (var ? d.cut.vcap : d.cut.slab_rows) || d.resp_hi - d.resp_lo > d.cut.resp_cap)
+            return fail(AGR_EINVAL, "restore: " + p + of + " is not a valid delta");
+        files.insert(files.begin(), p);
+        dh.insert(dh.begin(), d);
+        p = parent;
+    }
+}
+// The state of the whole chain into h: the full file (f, past its header), each delta after a check that the state so far
+// is its parent's cut (digest), then the header fields, the log lengths, the dedupe index and the chain an
+// AGR_CFG_DELTA_SNAPSHOT engine continues, once.
+static int restore_locked(agr_handle* h, FILE* f, const snap_header& full, const std::vector<std::string>& files, const std::vector<delta_header>& dh) {
+    HLock lk(h);
+    CK(cudaSetDevice(h->device));
+    TRY(restore_agents_locked(h, f, full.n_agents));
+    TRY(snap_sections(h, full, f, load_dev));
+    const bool chain = (h->cfg.flags & AGR_CFG_DELTA_SNAPSHOT) != 0;
+    if (!dh.empty()) TRY(snap_delta_alloc(h));
+    const snap_header* at = &full;
+    unsigned long long dg[2] = {0, 0};
+    for (size_t k = 0; k < dh.size(); ++k) {
+        TRY(snap_digest_locked(h, *at, false, dg));
+        if (memcmp(dg, dh[k].parent_digest, 16) != 0)
+            return fail(AGR_EINVAL, "restore: " + files[k] + " is not the snapshot " + files[k + 1] + " was written on (digest differs): was it replaced?");
+        FILE* g = fopen(files[k + 1].c_str(), "rb");
+        if (!g) return fail(AGR_EINVAL, "restore: cannot open " + files[k + 1]);
+        int rc = fseeko(g, (off_t)(sizeof(delta_header) + dh[k].parent_path_len), SEEK_SET) == 0 ? restore_delta_locked(h, g, dh[k])
+                                                                                                : fail(AGR_EINVAL, "restore: short read");
+        fclose(g);
+        TRY(rc);
+        at = &dh[k].cut;
+    }
+    const snap_header& hd = *at;
+    const size_t R = snap_rows(hd);
+    h->resp_used = hd.resp_used; h->resp_tail = hd.resp_tail; h->expired_total = hd.expired_total;
+    unsigned long long lens[2] = {hd.log_len[0], hd.log_len[1]};
+    if (cudaMemcpy(h->d.log_len, lens, sizeof lens, cudaMemcpyHostToDevice) != cudaSuccess) return fail(AGR_ECUDA, "restore: log_len");
+    h->rows_used = hd.rows_used; h->vused = hd.vused; h->vtail = hd.vtail; h->scan_lo = hd.scan_lo;
+    h->d.shard_id = hd.shard; h->d.id_gen = hd.gen; h->tail = hd.tail; h->released_total = hd.released_total; sync_window(h);
+    h->d.idx_base = h->tail;
+    cudaMemsetAsync(h->d.cmin, 0, (size_t)(h->cfg.slab_rows / AGR_CHUNK_ROWS + 2) * 8, h->stream);       // time bounds unknown: the first sweep recomputes them
+    if (!(hd.flags & AGR_CFG_MINT_IDS) && R) {        // hash-id mode: rebuild the dedupe index from the restored rows
+        agr_launch_reindex(h->d, (uint32_t)R, h->stream);
+        h->k1_launches += 1;
+        if (cudaStreamSynchronize(h->stream) != cudaSuccess) return fail(AGR_ECUDA, "restore: reindex");
+    }
+    if (chain || !dh.empty()) {
+        TRY(snap_digest_locked(h, hd, chain, dg));    // an AGR_CFG_DELTA_SNAPSHOT engine: also seeds the shadow
+        if (!dh.empty() && memcmp(dg, dh.back().digest, 16) != 0)
+            return fail(AGR_EINVAL, "restore: the state after " + files.back() + " differs from the one it was written from (digest)");
+    }
+    if (chain) {
+        snap_chain& ch = h->chain;
+        ch = snap_chain{};
+        ch.paths = files;
+        ch.paths.back() = snap_abs_path(files.back());   // (the parents' paths are absolute already)
+        ch.full_bytes = snap_full_bytes(h, full);
+        for (const auto& d : dh) ch.delta_bytes += d.file_bytes;
+        ch.base = hd; ch.base_bound = hd.rows_used;
+        memcpy(ch.digest, dg, 16);
+        if (ch.paths.back().empty()) ch = snap_chain{};
+    }
+    return 0;
+}
+
 int agr_restore(const agr_config* cfg, const char* path, agr_handle** out) {
     if (!cfg || !path || !out) return fail(AGR_EINVAL, "NULL argument");
     *out = nullptr;
-    FILE* f = fopen(path, "rb");
-    if (!f) return fail(AGR_EINVAL, std::string("restore: cannot open ") + path);
+    std::vector<std::string> files;
+    std::vector<delta_header> dh;
+    TRY(restore_chain(path, files, dh));
+    FILE* f = fopen(files[0].c_str(), "rb");
+    if (!f) return fail(AGR_EINVAL, "restore: cannot open " + files[0]);
     snap_header hd{};
     if (fread(&hd, sizeof hd, 1, f) != 1 || memcmp(hd.magic, "AGRSNAP3", 8) != 0) { fclose(f); return fail(AGR_EINVAL, "restore: not a snapshot"); }
     agr_config c = *cfg;
@@ -2095,40 +2511,28 @@ int agr_restore(const agr_config* cfg, const char* path, agr_handle** out) {
     if ((c.flags & mode_bits) != (hd.flags & mode_bits)) { fclose(f); return fail(AGR_EINVAL, "restore: id mode / record form differ from the snapshot"); }
     if (c.id_secret == 0) c.id_secret = hd.id_secret;
     if (c.id_secret != hd.id_secret) { fclose(f); return fail(AGR_EINVAL, "restore: id_secret differs from the snapshot"); }
+    for (size_t k = 0; k < dh.size(); ++k)
+        if ((dh[k].cut.flags & mode_bits) != (hd.flags & mode_bits) || dh[k].cut.id_secret != hd.id_secret || dh[k].cut.slab_rows != hd.slab_rows) {
+            fclose(f);
+            return fail(AGR_EINVAL, "restore: " + files[k + 1] + " and its full file " + files[0] + " come from different engines");
+        }
     agr_handle* h = nullptr;
     int rc = agr_create(&c, &h);
     if (rc < 0) { fclose(f); return rc; }
     auto bail = [&](int r) { std::string keep = g_err; fclose(f); agr_destroy(h); g_err = keep; return r; };
-    const bool snap_ring = (hd.flags & AGR_CFG_RING) != 0;
-    if (!snap_ring && hd.resp_used > h->resp_cap) return bail(fail(AGR_ENOSPC, "restore: stored responses larger than resp_bytes"));
-    if (snap_ring && hd.resp_cap != h->resp_cap) return bail(fail(AGR_EINVAL, "restore: a ring snapshot needs the same resp_bytes"));
-    if (snap_ring && (hd.flags & AGR_CFG_VARLEN) && hd.vcap != h->vcap) return bail(fail(AGR_EINVAL, "restore: a ring snapshot needs the same vslab_bytes"));
-    if (snap_ring && hd.slab_rows != h->cfg.slab_rows) return bail(fail(AGR_EINVAL, "restore: a ring snapshot needs the same slab_rows (rows live at logical mod slab_rows)"));
-    if ((!snap_ring && hd.rows_used > h->cfg.slab_rows) || hd.log_len[0] > h->d.log_cap || hd.log_len[1] > h->d.log_cap || ((hd.flags & AGR_CFG_VARLEN) && !snap_ring && hd.vused > h->vcap))
-        return bail(fail(AGR_ENOSPC, "restore: snapshot larger than the configured capacities"));
-    for (uint32_t a = 0; a < hd.n_agents; ++a) {
-        char name[AGR_AGENT_ID_BYTES]; uint8_t st;
-        if (fread(name, 1, AGR_AGENT_ID_BYTES, f) != AGR_AGENT_ID_BYTES || fread(&st, 1, 1, f) != 1) return bail(fail(AGR_EINVAL, "restore: short read"));
-        name[AGR_AGENT_ID_BYTES - 1] = 0;
-        const bool removed = (st == AG_STATUS_REMOVED);
-        if ((rc = agr_set_agent_state(h, name, removed ? (uint8_t)AGR_AGENT_STOPPED : st)) < 0) return bail(rc);
-        if (removed) { HLock lk(h); h->agent_status[a] = AG_STATUS_REMOVED; if ((rc = push_agent_status(h, a, AG_STATUS_REMOVED)) < 0) return bail(rc); }
-    }
-    HLock lk(h);
-    const size_t R = snap_rows(hd);
-    if ((rc = snap_sections(h, hd, f, load_dev)) < 0) return bail(rc);
-    h->resp_used = hd.resp_used; h->resp_tail = hd.resp_tail; h->expired_total = hd.expired_total;
-    unsigned long long lens[2] = {hd.log_len[0], hd.log_len[1]};
-    if (cudaMemcpy(h->d.log_len, lens, sizeof lens, cudaMemcpyHostToDevice) != cudaSuccess) return bail(fail(AGR_ECUDA, "restore: log_len"));
-    h->rows_used = hd.rows_used; h->vused = hd.vused; h->vtail = hd.vtail; h->scan_lo = hd.scan_lo;
-    h->d.shard_id = hd.shard; h->d.id_gen = hd.gen; h->tail = hd.tail; h->released_total = hd.released_total; sync_window(h);
-    h->d.idx_base = h->tail;
-    cudaMemsetAsync(h->d.cmin, 0, (size_t)(h->cfg.slab_rows / AGR_CHUNK_ROWS + 2) * 8, h->stream);       // time bounds unknown: the first sweep recomputes them
-    if (!(hd.flags & AGR_CFG_MINT_IDS) && R) {        // hash-id mode: rebuild the dedupe index from the restored rows
-        agr_launch_reindex(h->d, (uint32_t)R, h->stream);
-        h->k1_launches += 1;
-        if (cudaStreamSynchronize(h->stream) != cudaSuccess) return bail(fail(AGR_ECUDA, "restore: reindex"));
-    }
+    auto fits = [&](const snap_header& s) -> int {
+        const bool snap_ring = (s.flags & AGR_CFG_RING) != 0;
+        if (!snap_ring && s.resp_used > h->resp_cap) return fail(AGR_ENOSPC, "restore: stored responses larger than resp_bytes");
+        if (snap_ring && s.resp_cap != h->resp_cap) return fail(AGR_EINVAL, "restore: a ring snapshot needs the same resp_bytes");
+        if (snap_ring && (s.flags & AGR_CFG_VARLEN) && s.vcap != h->vcap) return fail(AGR_EINVAL, "restore: a ring snapshot needs the same vslab_bytes");
+        if (snap_ring && s.slab_rows != h->cfg.slab_rows) return fail(AGR_EINVAL, "restore: a ring snapshot needs the same slab_rows (rows live at logical mod slab_rows)");
+        if ((!snap_ring && s.rows_used > h->cfg.slab_rows) || s.log_len[0] > h->d.log_cap || s.log_len[1] > h->d.log_cap || ((s.flags & AGR_CFG_VARLEN) && !snap_ring && s.vused > h->vcap))
+            return fail(AGR_ENOSPC, "restore: snapshot larger than the configured capacities");
+        return 0;
+    };
+    if ((rc = fits(hd)) < 0) return bail(rc);
+    for (const auto& d : dh) if ((rc = fits(d.cut)) < 0) return bail(rc);
+    if ((rc = restore_locked(h, f, hd, files, dh)) < 0) return bail(rc);
     fclose(f);
     *out = h;
     return 0;

@@ -1077,6 +1077,107 @@ void agr_launch_snap_cut(const agr_dev& d, const agr_snap_cut& c, int sm_count, 
     k_snap_cut<<<dim3(bx, c.nrow + 2), 256, 0, st>>>(d, c);
 }
 
+// ------------------------------------------------------------------------------------------------ delta snapshot cut
+// The same grid as k_snap_cut.  Each warp takes 32 consecutive pieces, aligned to 32: 512 B, inside one block of any section
+// (blocks are 1, 2 or 4 KiB), so a warp sets at most one bit, with one atomicOr, and only when a lane differs.  A piece at the
+// end of a section (< 16 B) is read and written by words and zero-padded for the sum.
+__device__ __forceinline__ uint4 snap_load_piece(const uint8_t* p, unsigned long long i, unsigned long long bytes) {
+    if ((i + 1) * 16 <= bytes) return reinterpret_cast<const uint4*>(p)[i];
+    uint32_t w[4] = {0, 0, 0, 0};
+    for (unsigned k = 0; k < 4 && i * 16 + k * 4 < bytes; ++k) w[k] = reinterpret_cast<const uint32_t*>(p)[i * 4 + k];
+    return make_uint4(w[0], w[1], w[2], w[3]);
+}
+__device__ __forceinline__ void snap_store_piece(uint8_t* p, unsigned long long i, unsigned long long bytes, uint4 v) {
+    if ((i + 1) * 16 <= bytes) { reinterpret_cast<uint4*>(p)[i] = v; return; }
+    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+    for (unsigned k = 0; k < 4 && i * 16 + k * 4 < bytes; ++k) reinterpret_cast<uint32_t*>(p)[i * 4 + k] = w[k];
+}
+template <bool COMPARE>
+__global__ void __launch_bounds__(256) k_snap_cmp(const agr_dev d, const agr_snap_cmp c) {
+    __shared__ unsigned long long part[2][8];
+    const uint32_t s = blockIdx.y, lane = threadIdx.x & 31u;
+    unsigned long long bytes = c.bytes[s];
+    if (s >= c.nrow && !c.lens_from_host) {
+        const unsigned long long n = d.log_len[s - c.nrow];
+        bytes = (n < d.log_cap ? n : d.log_cap) * 4ull;
+        if (COMPARE && blockIdx.x == 0 && threadIdx.x == 0) reinterpret_cast<unsigned long long*>(c.shadow)[s - c.nrow] = n;
+    }
+    const uint8_t* __restrict__ src = c.src[s];
+    uint8_t* __restrict__ dst = COMPARE ? c.shadow + c.dst_off[s] : nullptr;
+    const unsigned long long np = (bytes + 15) >> 4, stride = (unsigned long long)gridDim.x * blockDim.x;
+    const unsigned long long skey = agr_fmix64(c.key ^ ((unsigned long long)(c.sec_id[s] + 1) << 56));
+    unsigned long long h0 = 0, h1 = 0;
+    for (unsigned long long i0 = (unsigned long long)blockIdx.x * blockDim.x + (threadIdx.x & ~31u); i0 < np; i0 += stride) {
+        const unsigned long long i = i0 + lane;
+        bool differ = false;
+        if (i < np) {
+            const uint4 v = snap_load_piece(src, i, bytes);
+            if (COMPARE) {
+                const uint4 o = snap_load_piece(dst, i, bytes);
+                differ = (v.x != o.x) | (v.y != o.y) | (v.z != o.z) | (v.w != o.w);
+                if (differ) snap_store_piece(dst, i, bytes, v);
+            }
+            const unsigned long long a = ((unsigned long long)v.y << 32) | v.x, b = ((unsigned long long)v.w << 32) | v.z;
+            const unsigned long long t = agr_fmix64(skey + i * 0x9e3779b97f4a7c15ULL);
+            h0 += agr_fmix64(agr_fmix64(t ^ a) ^ b);
+            h1 += agr_fmix64(agr_fmix64((t + 0x632be59bd9b4e019ULL) ^ b) ^ a);
+        }
+        if (COMPARE && __ballot_sync(0xffffffffu, differ) != 0u && lane == 0) {
+            const unsigned long long blk = i0 >> c.pshift[s];
+            atomicOr(c.bits + c.bit_off[s] + (blk >> 5), 1u << (blk & 31u));
+        }
+    }
+    for (int o = 16; o > 0; o >>= 1) { h0 += __shfl_xor_sync(0xffffffffu, h0, o); h1 += __shfl_xor_sync(0xffffffffu, h1, o); }
+    if (lane == 0) { part[0][threadIdx.x >> 5] = h0; part[1][threadIdx.x >> 5] = h1; }
+    __syncthreads();
+    if (threadIdx.x < 2) {
+        unsigned long long sum = 0;
+        for (int w = 0; w < 8; ++w) sum += part[threadIdx.x][w];
+        atomicAdd(c.digest + threadIdx.x, sum);
+    }
+}
+void agr_launch_snap_cmp(const agr_dev& d, const agr_snap_cmp& c, bool compare, int sm_count, cudaStream_t st) {
+    unsigned long long most = 0;
+    for (uint32_t s = 0; s < c.nrow + 2; ++s) most = c.bytes[s] > most ? c.bytes[s] : most;
+    if (d.log_cap * 4ull > most) most = d.log_cap * 4ull;
+    const unsigned long long want = (most / 16 + 1023) / 1024;
+    const uint32_t bx = (uint32_t)(want < 1 ? 1 : want > (unsigned long long)sm_count * 2 ? (unsigned long long)sm_count * 2 : want);
+    if (compare) k_snap_cmp<true><<<dim3(bx, c.nrow + 2), 256, 0, st>>>(d, c);
+    else k_snap_cmp<false><<<dim3(bx, c.nrow + 2), 256, 0, st>>>(d, c);
+}
+
+// One CTA per listed block.  A full block's slices are whole multiples of 1 KiB: 16 B moves; the short last block by words.
+template <bool GATHER>
+__global__ void __launch_bounds__(256) k_snap_blocks(const agr_snap_blocks g) {
+    const uint32_t b = g.list[blockIdx.x];
+    const unsigned long long r0 = (unsigned long long)b * g.block_rows;
+    const unsigned long long nr = g.rows - r0 < g.block_rows ? g.rows - r0 : g.block_rows;
+    uint8_t* rec = g.stage + (unsigned long long)blockIdx.x * g.rec_bytes;
+    unsigned long long at = 0;
+    for (uint32_t s = 0; s < g.nsec; ++s) {
+        const unsigned long long n = nr * g.width[s];
+        uint8_t* a = g.arr[s] + r0 * g.width[s];
+        uint8_t* st = rec + at;
+        if (nr == g.block_rows) {
+            for (unsigned long long k = threadIdx.x; k < n / 16; k += blockDim.x) {
+                if (GATHER) reinterpret_cast<uint4*>(st)[k] = reinterpret_cast<const uint4*>(a)[k];
+                else reinterpret_cast<uint4*>(a)[k] = reinterpret_cast<const uint4*>(st)[k];
+            }
+        } else {
+            for (unsigned long long k = threadIdx.x; k < n / 4; k += blockDim.x) {
+                if (GATHER) reinterpret_cast<uint32_t*>(st)[k] = reinterpret_cast<const uint32_t*>(a)[k];
+                else reinterpret_cast<uint32_t*>(a)[k] = reinterpret_cast<const uint32_t*>(st)[k];
+            }
+        }
+        at += n;
+    }
+}
+void agr_launch_snap_blocks(const agr_snap_blocks& g, uint32_t n, bool gather, cudaStream_t st) {
+    if (!n) return;
+    if (gather) k_snap_blocks<true><<<n, 256, 0, st>>>(g);
+    else k_snap_blocks<false><<<n, 256, 0, st>>>(g);
+}
+
 // ------------------------------------------------------------------------------------------------ synthetic stream
 __global__ void __launch_bounds__(128) k_synth(uint8_t* dst, const agr_synth_dev s, const unsigned long long first_index, const uint32_t n) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;

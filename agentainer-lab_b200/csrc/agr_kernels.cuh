@@ -230,3 +230,37 @@ struct agr_snap_cut {
     uint32_t nrow;
 };
 void agr_launch_snap_cut(const agr_dev& d, const agr_snap_cut& c, int sm_count, cudaStream_t st);
+
+// Delta snapshots (AGR_CFG_DELTA_SNAPSHOT).  The compare cut is the cut above that also compares each 16 B piece with what the
+// shadow held (the previous cut) before it overwrites it: a piece that differs sets the bit of its block (256 rows of a word
+// section, 1024 entries of a log) in bits, and every piece, live or not, goes into a 128-bit keyed sum (digest[2], added to).
+// Section s covers bytes[s] bytes (sections nrow and nrow + 1, the logs, as in agr_snap_cut unless lens_from_host); its
+// block of piece i is i >> pshift[s], its bit word bit_off[s] + block / 32.  The digest-only pass (compare = false) reads
+// src alone: no shadow, no bits.  The sum does not depend on the grid: it adds one keyed hash per (section, piece).
+struct agr_snap_cmp {
+    const uint8_t* src[AGR_SNAP_CUT_MAX];
+    unsigned long long dst_off[AGR_SNAP_CUT_MAX];
+    unsigned long long bytes[AGR_SNAP_CUT_MAX];
+    uint32_t pshift[AGR_SNAP_CUT_MAX];
+    uint32_t bit_off[AGR_SNAP_CUT_MAX];
+    uint32_t sec_id[AGR_SNAP_CUT_MAX];     // the section's index in the file's table: part of each piece's key
+    uint8_t* shadow;
+    uint32_t* bits;
+    unsigned long long* digest;
+    unsigned long long key;
+    uint32_t nrow;
+    uint32_t lens_from_host;               // 1: the logs' byte counts are bytes[nrow], bytes[nrow + 1] (restore-time checks)
+};
+void agr_launch_snap_cmp(const agr_dev& d, const agr_snap_cmp& c, bool compare, int sm_count, cudaStream_t st);
+// Block gather / scatter: block list[j] of a section table (arr[s], width[s] bytes per row, rows rows in all, block_rows rows
+// per block) is packed at stage + j * rec_bytes as each section's slice in table order; the last block of the table may be
+// short.  gather: arrays -> stage (the writer packs dirty blocks from the shadow); scatter: stage -> arrays (restore).
+struct agr_snap_blocks {
+    uint8_t* arr[AGR_SNAP_CUT_MAX];
+    uint32_t width[AGR_SNAP_CUT_MAX];
+    uint32_t nsec, block_rows;
+    unsigned long long rows, rec_bytes;
+    const uint32_t* list;
+    uint8_t* stage;
+};
+void agr_launch_snap_blocks(const agr_snap_blocks& g, uint32_t n, bool gather, cudaStream_t st);

@@ -115,6 +115,11 @@ typedef struct agr_record {
                                        agr_create returns AGR_ENOMEM when that does not fit. */
 #define AGR_CFG_DIAG_NO_INDEX  0x100u /* DIAGNOSTIC ONLY (results invalid): K1 skips the dedupe-index insert, to attribute kernel time */
 #define AGR_CFG_DIAG_NO_CKSUM  0x200u /* DIAGNOSTIC ONLY (results invalid): K1 skips the record checksum */
+#define AGR_CFG_DELTA_SNAPSHOT 0x400u /* needs AGR_CFG_ONLINE_SNAPSHOT (else agr_create / agr_restore return AGR_EINVAL): agr_snapshot
+                                       writes a DELTA file — only what changed since the engine's previous completed snapshot, and the
+                                       absolute path of that file — whenever it can, else a full file (see agr_snapshot).  Files must
+                                       stay where they were written: a restore follows the paths back.  Costs a dirty bitmap (1 bit
+                                       per 256 rows and per 1024 log entries) and a staging buffer of at most 32 MiB. */
 #define AGR_CFG_SKIP_INFLIGHT 0x2u  /* EXTENSION, off in parity mode: replay scan skips records whose forward is still in flight (fixes Q16) */
 
 typedef struct agr_config {
@@ -403,7 +408,21 @@ int agr_json_decode(const uint8_t* json, uint32_t len, uint8_t* record, uint32_t
  * empty, as it treats what a blocking snapshot writes there) for rows that hold no record at the cut — rows outside
  * [rows_tail, rows_used), rows skipped at the end of a lap, rows reserved and not ingested — and for byte-ring bytes outside
  * the record bytes' and the response bytes' live ranges.  agr_snapshot returns once the file is written; a failure at any
- * point releases the pinned window. */
+ * point releases the pinned window.
+ * With AGR_CFG_DELTA_SNAPSHOT as well, the cut also compares the per-row words and the logs with the previous cut and marks the
+ * blocks that changed, and agr_snapshot writes one of two kinds of file; the first 8 bytes tell them apart:
+ *   "AGRSNAP3"  a full file, the layout above, byte for byte;
+ *   "AGRDELT1"  a delta on the engine's previous completed snapshot (its PARENT): the cut's header, the absolute path of the
+ *               parent, the agent table, the slab rows / record bytes and response bytes appended since the parent's cut, and
+ *               the blocks of per-row words and log entries that changed (layout: DESIGN.md section 5).
+ * It writes a full file when there is no completed snapshot to build on (the first one after agr_create, or the next one after
+ * a write that failed), when path names a file of the current chain (the last full file and every delta since: the usual
+ * "write path.tmp, rename over path" recipe gets a full file every time), or when the deltas since the last full file plus
+ * this one would be larger than a full file of this cut (a restore then reads at most about twice a full file).
+ * agr_restore accepts either kind.  Given a delta it follows the parent paths back to the full file, loads it and applies the
+ * deltas oldest first; a parent that is missing, replaced by another file or shorter than its header says fails with
+ * AGR_EINVAL.  So the files of a chain must stay where they were written until a newer full file exists.  An engine restored
+ * with the flag continues the chain: its next agr_snapshot is a delta on the file it was restored from. */
 int agr_snapshot(agr_handle* h, const char* path);
 int agr_restore(const agr_config* cfg, const char* path, agr_handle** out);
 /* The 24 h TTL of the record keys (SET ... EX 24h at requests.go:106,175,270; every SET restarts it, Q11).  Times are the
@@ -472,7 +491,7 @@ int agr_kernel_time(agr_handle* h, double* sum_ms, uint64_t* launches);
 /* With AGR_CFG_TIMING: device time (CUDA events on the launching stream) of the most recent kernel group:
  * which = 0 the K2 kernels of the last agr_complete, 1 the K3 select kernels of the last scan / pending / list,
  * 2 the K5 kernels of the last JSON encode (measure + scan + emit, including the host's read of the total between them),
- * 3 the cut of the last agr_snapshot with AGR_CFG_ONLINE_SNAPSHOT. */
+ * 3 the cut of the last agr_snapshot with AGR_CFG_ONLINE_SNAPSHOT (the compare cut with AGR_CFG_DELTA_SNAPSHOT). */
 int agr_op_time(agr_handle* h, int which, double* ms);
 void* agr_slab_ptr(agr_handle* h, uint64_t rid); /* device address of a slab row */
 
