@@ -190,8 +190,8 @@ struct agr_handle {
     std::mutex snap_mu;                                      // one online snapshot at a time: there is one shadow
     bool pinned = false; uint64_t pin_tail = 0, pin_vtail = 0, pin_resp_tail = 0;   // (h->mu) the cut's ring tails while it is written
     // AGR_CFG_DELTA_SNAPSHOT (and a restore that applies deltas): the compare cut's dirty bits (word blocks, then the completed
-    // and failed logs' blocks at snap_bit_off[1], [2]) and digest, the pinned copy the writer reads them from (the two log
-    // lengths and the digest first), the device block list and the staging buffer of the block gather / scatter
+    // and failed logs' blocks at snap_bit_off[1], [2]) and digest, the pinned copy the writer reads them from (the digest at
+    // offset 16, the bits at 32), the device block list and the staging buffer of the block gather / scatter
     uint32_t* d_snap_bits = nullptr; unsigned long long* d_snap_digest = nullptr; uint8_t* h_snap_bits = nullptr;
     size_t snap_bit_off[3] = {}, snap_bit_words = 0;
     uint32_t* d_snap_list = nullptr; uint8_t* d_snap_stage = nullptr; size_t snap_stage_bytes = 0;
@@ -1977,7 +1977,7 @@ struct delta_header {
     unsigned long long parent_digest[2], digest[2];
     uint32_t block_rows, log_block;
     uint64_t rows_lo, rows_hi, resp_lo, resp_hi;
-    uint64_t n_blocks, n_log_blocks[2];
+    uint64_t n_blocks[3];          // listed blocks per table of snap_block_tables
     uint32_t parent_path_len, pad;
 };
 static_assert(sizeof(delta_header) == 264 && sizeof(snap_header) == 144, "delta_header is a file layout");
@@ -2003,9 +2003,9 @@ static size_t snap_full_bytes(agr_handle* h, const snap_header& hd) {
     for (int k = 0; k < SNAP_NSEC; ++k) n += sec[k].bytes;
     return n;
 }
-// The compare cut's sections: the SNAP_WORDS ones that hold bytes, then the two logs (whose lengths the kernel reads on the
-// device unless lens_from_host).  A word block is 256 rows: 16 * width pieces of 16 B; a log block 1024 entries: 256 pieces.
-static void snap_cmp_params(agr_handle* h, const snap_header& hd, bool lens_from_host, agr_snap_cmp& c) {
+// The cut's sections: the SNAP_WORDS ones that hold bytes, then the two logs (whose lengths the kernel reads on the device
+// unless lens_from_host).  A word block is 256 rows: 16 * width pieces of 16 B; a log block 1024 entries: 256 pieces.
+static void snap_cut_params(agr_handle* h, const snap_header& hd, bool lens_from_host, agr_snap_cmp& c) {
     snap_section sec[SNAP_NSEC];
     snap_table(h, hd, sec);
     const size_t R = snap_rows(hd);
@@ -2026,15 +2026,18 @@ static void snap_cmp_params(agr_handle* h, const snap_header& hd, bool lens_from
         c.pshift[n] = 8; c.bit_off[n] = (uint32_t)h->snap_bit_off[1 + j]; c.sec_id[n] = (uint32_t)logs[j];
     }
 }
-// the compare cut (caller holds HLock): the cut of snap_cut_locked that also marks the blocks that differ from the previous
-// cut and sums the digest of this one
-static int snap_cmp_cut_locked(agr_handle* h, const snap_header& hd) {
+// the cut (caller holds HLock): one kernel copies the per-row words of rows [0, R) and the two log prefixes into the shadow;
+// with compare, it also marks the blocks that differ from the previous cut and sums the digest of this one
+static int snap_cut_locked(agr_handle* h, const snap_header& hd, bool compare) {
     agr_snap_cmp c;
-    snap_cmp_params(h, hd, false, c);
-    CK(cudaMemsetAsync(h->d_snap_bits, 0, h->snap_bit_words * 4, h->stream));
-    CK(cudaMemsetAsync(h->d_snap_digest, 0, 16, h->stream));
+    snap_cut_params(h, hd, false, c);
+    if (compare) {
+        CK(cudaMemsetAsync(h->d_snap_bits, 0, h->snap_bit_words * 4, h->stream));
+        CK(cudaMemsetAsync(h->d_snap_digest, 0, 16, h->stream));
+    }
     TRY(op_time_begin(h, 3));
-    agr_launch_snap_cmp(h->d, c, true, h->sm_count, h->stream);
+    if (compare) agr_launch_snap_cmp(h->d, c, true, h->sm_count, h->stream);
+    else agr_launch_snap_cut(h->d, c, h->sm_count, h->stream);
     CK(cudaGetLastError());
     TRY(op_time_end(h, 3));
     CK(cudaEventRecord(h->snap_ev[0], h->stream));
@@ -2044,7 +2047,7 @@ static int snap_cmp_cut_locked(agr_handle* h, const snap_header& hd) {
 // shadow, so that the next snapshot of an AGR_CFG_DELTA_SNAPSHOT engine compares against the restored state
 static int snap_digest_locked(agr_handle* h, const snap_header& hd, bool seed, unsigned long long out[2]) {
     agr_snap_cmp c;
-    snap_cmp_params(h, hd, !seed, c);
+    snap_cut_params(h, hd, !seed, c);
     if (seed) CK(cudaMemsetAsync(h->d_snap_bits, 0, h->snap_bit_words * 4, h->stream));
     CK(cudaMemsetAsync(h->d_snap_digest, 0, 16, h->stream));
     agr_launch_snap_cmp(h->d, c, seed, h->sm_count, h->stream);
@@ -2054,32 +2057,26 @@ static int snap_digest_locked(agr_handle* h, const snap_header& hd, bool seed, u
     memcpy(out, h->h_snap_bits, 16);
     return 0;
 }
-// The block tables of a delta: the word sections of hd (256 rows per block), or log j (1024 entries per block), in the shadow
-// (the writer) or the live arrays (restore)
-static agr_snap_blocks snap_word_blocks(agr_handle* h, const snap_header& hd, bool shadow) {
+// The block tables of a delta, in file order: [0] the word sections of hd (256 rows per block), [1] and [2] the completed and
+// failed logs (1024 entries per block), in the shadow (the writer) or the live arrays (restore).  Table t's bits start at
+// snap_bit_off[t].
+static void snap_block_tables(agr_handle* h, const snap_header& hd, bool shadow, agr_snap_blocks g[3]) {
     snap_section sec[SNAP_NSEC];
     snap_table(h, hd, sec);
-    agr_snap_blocks g{};
-    g.block_rows = SNAP_BLOCK_ROWS; g.rows = snap_rows(hd);
-    for (int k = 0; k < SNAP_NSEC; ++k) {
-        if (sec[k].kind != SNAP_WORDS || sec[k].bytes == 0) continue;
-        g.arr[g.nsec] = shadow ? h->d_shadow + h->shadow_off[k] : (uint8_t*)sec[k].p;
-        g.width[g.nsec] = (uint32_t)(sec[k].bytes / g.rows);
-        g.rec_bytes += (unsigned long long)g.width[g.nsec] * SNAP_BLOCK_ROWS;
-        g.nsec++;
+    for (int t = 0; t < 3; ++t) g[t] = agr_snap_blocks{};
+    g[0].block_rows = SNAP_BLOCK_ROWS; g[0].rows = snap_rows(hd);
+    for (int k = 0, j = 0; k < SNAP_NSEC; ++k) {
+        uint8_t* a = shadow ? h->d_shadow + h->shadow_off[k] : (uint8_t*)sec[k].p;
+        if (sec[k].kind == SNAP_LOG) {
+            agr_snap_blocks& l = g[1 + j];
+            l.arr[0] = a; l.nsec = 1; l.width[0] = 4; l.block_rows = SNAP_LOG_BLOCK; l.rows = hd.log_len[j++]; l.rec_bytes = 4ull * SNAP_LOG_BLOCK;
+        } else if (sec[k].kind == SNAP_WORDS && sec[k].bytes) {
+            agr_snap_blocks& w = g[0];
+            w.arr[w.nsec] = a; w.width[w.nsec] = (uint32_t)(sec[k].bytes / w.rows);
+            w.rec_bytes += (unsigned long long)w.width[w.nsec] * SNAP_BLOCK_ROWS;
+            w.nsec++;
+        }
     }
-    return g;
-}
-static agr_snap_blocks snap_log_blocks(agr_handle* h, const snap_header& hd, int j, bool shadow) {
-    snap_section sec[SNAP_NSEC];
-    snap_table(h, hd, sec);
-    agr_snap_blocks g{};
-    for (int k = 0, seen = 0; k < SNAP_NSEC; ++k) {
-        if (sec[k].kind != SNAP_LOG || seen++ != j) continue;
-        g.arr[0] = shadow ? h->d_shadow + h->shadow_off[k] : (uint8_t*)sec[k].p;
-    }
-    g.nsec = 1; g.width[0] = 4; g.block_rows = SNAP_LOG_BLOCK; g.rows = hd.log_len[j]; g.rec_bytes = 4ull * SNAP_LOG_BLOCK;
-    return g;
 }
 // bytes of the slices of n listed blocks (only the table's last block may be short)
 static uint64_t snap_blocks_bytes(const agr_snap_blocks& g, const uint32_t* list, size_t n) {
@@ -2087,14 +2084,22 @@ static uint64_t snap_blocks_bytes(const agr_snap_blocks& g, const uint32_t* list
     const uint64_t last = list[n - 1], r0 = last * g.block_rows;
     return (n - 1) * g.rec_bytes + std::min<uint64_t>(g.block_rows, g.rows - r0) * (g.rec_bytes / g.block_rows);
 }
-// the physical runs (start, count) of the logical range [lo, hi) of a ring of cap units (one run without AGR_CFG_RING)
-static int snap_runs(uint64_t lo, uint64_t hi, uint64_t cap, bool ring, uint64_t run[2][2]) {
-    if (hi <= lo) return 0;
-    const uint64_t p = ring ? lo % cap : lo, n0 = ring ? std::min(hi - lo, cap - p) : hi - lo;
-    run[0][0] = p; run[0][1] = n0;
-    if (hi - lo == n0) return 1;
-    run[1][0] = 0; run[1][1] = hi - lo - n0;
-    return 2;
+// The appended pieces of a delta, in file order: the slab rows (record bytes with AGR_CFG_VARLEN) [rows_lo, rows_hi), then the
+// response bytes [resp_lo, resp_hi), each in one physical run or two where its ring wraps, as (live device array, bytes)
+struct snap_piece { uint8_t* p; uint64_t bytes; };
+static int snap_delta_pieces(agr_handle* h, const delta_header& dh, snap_piece out[4]) {
+    const snap_header& hd = dh.cut;
+    const bool var = (hd.flags & AGR_CFG_VARLEN) != 0, ring = (hd.flags & AGR_CFG_RING) != 0;
+    const struct { uint64_t lo, hi, cap; uint8_t* base; uint64_t unit; } spans[2] = {
+        {dh.rows_lo, dh.rows_hi, var ? hd.vcap : hd.slab_rows, h->d.slab, var ? 1ull : (uint64_t)AGR_REC}, {dh.resp_lo, dh.resp_hi, hd.resp_cap, h->d_resp, 1}};
+    int n = 0;
+    for (const auto& s : spans) {
+        if (s.hi <= s.lo) continue;
+        const uint64_t p = ring ? s.lo % s.cap : s.lo, n0 = ring ? std::min(s.hi - s.lo, s.cap - p) : s.hi - s.lo;
+        out[n++] = {s.base + p * s.unit, n0 * s.unit};
+        if (s.hi - s.lo > n0) out[n++] = {s.base, (s.hi - s.lo - n0) * s.unit};
+    }
+    return n;
 }
 // the absolute name a chain keeps of a file: realpath of its directory, then its name ("" if the directory does not resolve)
 static std::string snap_abs_path(const std::string& p) {
@@ -2133,25 +2138,15 @@ static int snap_online_create(agr_handle* h) {
     if (h->cfg.flags & AGR_CFG_DELTA_SNAPSHOT) TRY(snap_delta_alloc(h));
     return 0;
 }
-// the cut: one kernel copies the per-row words of rows [0, R) and the two log prefixes into the shadow (caller holds HLock)
-static int snap_cut_locked(agr_handle* h, const snap_header& hd) {
-    snap_section sec[SNAP_NSEC];
-    snap_table(h, hd, sec);
-    agr_snap_cut c{};
-    c.shadow = h->d_shadow;
-    int logs[2], nlog = 0;
-    for (int k = 0; k < SNAP_NSEC; ++k) {
-        if (sec[k].kind == SNAP_LOG) logs[nlog++] = k;
-        if (sec[k].kind != SNAP_WORDS || sec[k].bytes == 0) continue;
-        c.src[c.nrow] = (const uint8_t*)sec[k].p; c.dst_off[c.nrow] = h->shadow_off[k]; c.bytes[c.nrow] = sec[k].bytes;
-        c.nrow++;
-    }
-    for (int j = 0; j < 2; ++j) { c.src[c.nrow + j] = (const uint8_t*)sec[logs[j]].p; c.dst_off[c.nrow + j] = h->shadow_off[logs[j]]; }
-    TRY(op_time_begin(h, 3));
-    agr_launch_snap_cut(h->d, c, h->sm_count, h->stream);
-    CK(cudaGetLastError());
-    TRY(op_time_end(h, 3));
-    CK(cudaEventRecord(h->snap_ev[0], h->stream));
+// the writer stream starts behind the cut; reads what the cut left: the log lengths it read (into hd), and with compare the
+// digest and the dirty bits (into h_snap_bits + 16 and + 32)
+static int snap_read_cut(agr_handle* h, snap_header& hd, bool compare) {
+    if (cudaStreamWaitEvent(h->snap_stream, h->snap_ev[0], 0) != cudaSuccess ||
+        cudaMemcpyAsync(h->snap_buf[0], h->d_shadow, 16, cudaMemcpyDeviceToHost, h->snap_stream) != cudaSuccess ||
+        (compare && (cudaMemcpyAsync(h->h_snap_bits + 16, h->d_snap_digest, 16, cudaMemcpyDeviceToHost, h->snap_stream) != cudaSuccess ||
+                     cudaMemcpyAsync(h->h_snap_bits + 32, h->d_snap_bits, h->snap_bit_words * 4, cudaMemcpyDeviceToHost, h->snap_stream) != cudaSuccess)) ||
+        cudaStreamSynchronize(h->snap_stream) != cudaSuccess) return fail(AGR_ECUDA, "snapshot: cut");
+    memcpy(hd.log_len, h->snap_buf[0], 16);
     return 0;
 }
 // writes the chunk waiting in the buffer the next chunk does not use, once its copy has landed
@@ -2184,6 +2179,31 @@ static void snap_fill_header(agr_handle* h, snap_header& hd) {
     hd.rows_used = h->rows_used; hd.vused = h->vused; hd.id_secret = h->d.id_secret; hd.scan_lo = h->scan_lo;
     hd.resp_used = h->resp_used; hd.expired_total = h->expired_total; hd.tail = h->tail; hd.released_total = h->released_total; hd.slab_rows = h->cfg.slab_rows; hd.vtail = h->vtail; hd.vcap = h->vcap; hd.resp_tail = h->resp_tail; hd.resp_cap = h->resp_cap;
 }
+// the agent table as a file holds it: per agent its NUL-padded name (AGR_AGENT_ID_BYTES), then its status byte
+static std::vector<char> snap_agents(agr_handle* h) {
+    std::vector<char> agents(h->agent_names.size() * (AGR_AGENT_ID_BYTES + 1), 0);
+    for (size_t a = 0; a < h->agent_names.size(); ++a) {
+        char* e = agents.data() + a * (AGR_AGENT_ID_BYTES + 1);
+        strncpy(e, h->agent_names[a].c_str(), AGR_AGENT_ID_BYTES - 1);
+        e[AGR_AGENT_ID_BYTES] = (char)h->agent_status[a];
+    }
+    return agents;
+}
+// A full file (AGRSNAP3): the header, the agent table, then the sections through io (dump_dev, or dump_online with the cut's
+// shadow as in snap_sections) and the drain of the last chunk (nothing is pending after dump_dev)
+static int snap_write_full(agr_handle* h, FILE* f, const snap_header& hd, const std::vector<char>& agents,
+                           int (*io)(agr_handle*, FILE*, void*, size_t), uint8_t* shadow = nullptr) {
+    if (fwrite(&hd, sizeof hd, 1, f) != 1 || fwrite(agents.data(), 1, agents.size(), f) != agents.size())
+        return fail(AGR_EINVAL, "snapshot: short write");
+    TRY(snap_sections(h, hd, f, io, shadow));
+    return snap_drain(h, f);
+}
+// closes a file a snapshot wrote; a failed close (the last buffered bytes did not reach the file) fails a snapshot that had not
+// failed already
+static int snap_close(FILE* f, int r) {
+    if (fclose(f) != 0 && r == 0) return fail(AGR_EINVAL, "snapshot: close failed");
+    return r;
+}
 // the writer: the list, then the listed blocks of g, packed on the writer stream into the staging buffer (stream order keeps
 // a chunk's copies ahead of the next chunk's gather) and streamed through the pinned buffers
 static int dump_blocks(agr_handle* h, FILE* f, agr_snap_blocks g, const std::vector<uint32_t>& list) {
@@ -2202,15 +2222,9 @@ static int dump_blocks(agr_handle* h, FILE* f, agr_snap_blocks g, const std::vec
     }
     return 0;
 }
-// AGR_CFG_DELTA_SNAPSHOT: reads the compare cut's log lengths, digest and dirty bits, then writes a delta on the chain's last
-// file, or a full file when there is no chain, path is one of its files, or the deltas would outgrow a full file
-static int snap_write_chain(agr_handle* h, FILE* f, const char* path, snap_header& hd, const std::vector<char>& agents, uint64_t bound) {
-    if (cudaStreamWaitEvent(h->snap_stream, h->snap_ev[0], 0) != cudaSuccess ||
-        cudaMemcpyAsync(h->h_snap_bits, h->d_shadow, 16, cudaMemcpyDeviceToHost, h->snap_stream) != cudaSuccess ||
-        cudaMemcpyAsync(h->h_snap_bits + 16, h->d_snap_digest, 16, cudaMemcpyDeviceToHost, h->snap_stream) != cudaSuccess ||
-        cudaMemcpyAsync(h->h_snap_bits + 32, h->d_snap_bits, h->snap_bit_words * 4, cudaMemcpyDeviceToHost, h->snap_stream) != cudaSuccess ||
-        cudaStreamSynchronize(h->snap_stream) != cudaSuccess) return fail(AGR_ECUDA, "snapshot: cut");
-    memcpy(hd.log_len, h->h_snap_bits, 16);
+// AGR_CFG_DELTA_SNAPSHOT: writes a delta on the chain's last file, or a full file when there is no chain, path is one of its
+// files, or the deltas would outgrow a full file (hd, the digest and the dirty bits are what the compare cut left)
+static int snap_write_chain(agr_handle* h, FILE* f, const char* path, const snap_header& hd, const std::vector<char>& agents, uint64_t bound) {
     unsigned long long digest[2];
     memcpy(digest, h->h_snap_bits + 16, 16);
     const uint32_t* bits = reinterpret_cast<const uint32_t*>(h->h_snap_bits + 32);
@@ -2220,12 +2234,14 @@ static int snap_write_chain(agr_handle* h, FILE* f, const char* path, snap_heade
     const size_t full = snap_full_bytes(h, hd);
     bool delta = !ch.paths.empty() && std::find(ch.paths.begin(), ch.paths.end(), at) == ch.paths.end();
     delta_header dh{};
-    std::vector<uint32_t> wl, ll[2];
-    const bool var = (hd.flags & AGR_CFG_VARLEN) != 0, ring = (hd.flags & AGR_CFG_RING) != 0;
-    const uint64_t unit = var ? 1 : AGR_REC;
-    agr_snap_blocks gw = snap_word_blocks(h, hd, true), gl[2] = {snap_log_blocks(h, hd, 0, true), snap_log_blocks(h, hd, 1, true)};
+    std::vector<uint32_t> list[3];
+    agr_snap_blocks g[3];
+    snap_piece pc[4];
+    int npc = 0;
+    snap_block_tables(h, hd, true, g);
     if (delta) {
         const snap_header& b = ch.base;
+        const bool var = (hd.flags & AGR_CFG_VARLEN) != 0;
         memcpy(dh.magic, "AGRDELT1", 8);
         dh.cut = hd;
         memcpy(dh.parent_digest, ch.digest, 16); memcpy(dh.digest, digest, 16);
@@ -2235,41 +2251,33 @@ static int snap_write_chain(agr_handle* h, FILE* f, const char* path, snap_heade
         dh.rows_lo = std::min(dh.rows_hi, std::max(var ? b.vused : ch.base_bound, var ? hd.vtail : hd.tail));
         dh.resp_hi = hd.resp_used;
         dh.resp_lo = std::min(dh.resp_hi, std::max(b.resp_used, hd.resp_tail));
-        // dirty blocks, and every block that reaches past what the parent's cut held (the shadow has nothing of it there)
-        const uint64_t R = snap_rows(hd), first_new = snap_rows(b) / SNAP_BLOCK_ROWS;
-        for (uint64_t k = 0; k * SNAP_BLOCK_ROWS < R; ++k)
-            if (k >= first_new || ((bits[k >> 5] >> (k & 31)) & 1u)) wl.push_back((uint32_t)k);
-        for (int j = 0; j < 2; ++j) {
-            const uint32_t* lb = bits + h->snap_bit_off[1 + j];
-            const uint64_t lnew = b.log_len[j] / SNAP_LOG_BLOCK;
-            for (uint64_t k = 0; k * SNAP_LOG_BLOCK < hd.log_len[j]; ++k)
-                if (k >= lnew || ((lb[k >> 5] >> (k & 31)) & 1u)) ll[j].push_back((uint32_t)k);
-        }
-        dh.n_blocks = wl.size(); dh.n_log_blocks[0] = ll[0].size(); dh.n_log_blocks[1] = ll[1].size();
         dh.parent_path_len = (uint32_t)ch.paths.back().size();
-        dh.file_bytes = sizeof dh + dh.parent_path_len + agents.size() + (dh.rows_hi - dh.rows_lo) * unit + (dh.resp_hi - dh.resp_lo)
-                        + 4 * wl.size() + snap_blocks_bytes(gw, wl.data(), wl.size());
-        for (int j = 0; j < 2; ++j) dh.file_bytes += 4 * ll[j].size() + snap_blocks_bytes(gl[j], ll[j].data(), ll[j].size());
+        dh.file_bytes = sizeof dh + dh.parent_path_len + agents.size();
+        npc = snap_delta_pieces(h, dh, pc);
+        for (int j = 0; j < npc; ++j) dh.file_bytes += pc[j].bytes;
+        // dirty blocks, and every block that reaches past what the parent's cut held (the shadow has nothing of it there)
+        agr_snap_blocks pg[3];
+        snap_block_tables(h, b, true, pg);
+        for (int t = 0; t < 3; ++t) {
+            const uint32_t* tb = bits + h->snap_bit_off[t];
+            const uint64_t first_new = pg[t].rows / pg[t].block_rows;
+            for (uint64_t k = 0; k * g[t].block_rows < g[t].rows; ++k)
+                if (k >= first_new || ((tb[k >> 5] >> (k & 31)) & 1u)) list[t].push_back((uint32_t)k);
+            dh.n_blocks[t] = list[t].size();
+            dh.file_bytes += 4 * list[t].size() + snap_blocks_bytes(g[t], list[t].data(), list[t].size());
+        }
         delta = ch.delta_bytes + dh.file_bytes <= full;              // else a full file: a restore reads at most ~2 full files
     }
     if (!delta) {
-        if (fwrite(&hd, sizeof hd, 1, f) != 1 || fwrite(agents.data(), 1, agents.size(), f) != agents.size())
-            return fail(AGR_EINVAL, "snapshot: short write");
-        TRY(snap_sections(h, hd, f, dump_online, h->d_shadow));
-        TRY(snap_drain(h, f));
+        TRY(snap_write_full(h, f, hd, agents, dump_online, h->d_shadow));
         ch = snap_chain{};
         ch.full_bytes = full;
     } else {
         const std::string& parent = ch.paths.back();
         if (fwrite(&dh, sizeof dh, 1, f) != 1 || fwrite(parent.data(), 1, parent.size(), f) != parent.size() ||
             fwrite(agents.data(), 1, agents.size(), f) != agents.size()) return fail(AGR_EINVAL, "snapshot: short write");
-        uint64_t run[2][2];
-        for (int n = snap_runs(dh.rows_lo, dh.rows_hi, var ? hd.vcap : hd.slab_rows, ring, run), j = 0; j < n; ++j)
-            TRY(dump_online(h, f, h->d.slab + run[j][0] * unit, run[j][1] * unit));
-        for (int n = snap_runs(dh.resp_lo, dh.resp_hi, hd.resp_cap, ring, run), j = 0; j < n; ++j)
-            TRY(dump_online(h, f, h->d_resp + run[j][0], run[j][1]));
-        TRY(dump_blocks(h, f, gw, wl));
-        for (int j = 0; j < 2; ++j) TRY(dump_blocks(h, f, gl[j], ll[j]));
+        for (int j = 0; j < npc; ++j) TRY(dump_online(h, f, pc[j].p, pc[j].bytes));
+        for (int t = 0; t < 3; ++t) TRY(dump_blocks(h, f, g[t], list[t]));
         TRY(snap_drain(h, f));
         ch.delta_bytes += dh.file_bytes;
     }
@@ -2292,38 +2300,20 @@ static int snapshot_online(agr_handle* h, const char* path) {
     {
         HLock lk(h);
         snap_fill_header(h, hd);
-        agents.assign((size_t)hd.n_agents * (AGR_AGENT_ID_BYTES + 1), 0);
-        for (uint32_t a = 0; a < hd.n_agents; ++a) {
-            char* e = agents.data() + (size_t)a * (AGR_AGENT_ID_BYTES + 1);
-            strncpy(e, h->agent_names[a].c_str(), AGR_AGENT_ID_BYTES - 1);
-            e[AGR_AGENT_ID_BYTES] = (char)h->agent_status[a];
-        }
+        agents = snap_agents(h);
         bound = ingested_bound(h);
-        const int rc = chain ? snap_cmp_cut_locked(h, hd) : snap_cut_locked(h, hd);
+        const int rc = snap_cut_locked(h, hd, chain);
         if (rc < 0) { fclose(f); h->chain = snap_chain{}; return rc; }
         if (is_ring(h)) { h->pinned = true; h->pin_tail = h->tail; h->pin_vtail = h->vtail; h->pin_resp_tail = h->resp_tail; }
     }
-    auto done = [&](int r) {
-        std::string keep = g_err;
-        if (cudaStreamSynchronize(h->snap_stream) != cudaSuccess && r == 0) { keep = "snapshot: writer stream"; r = AGR_ECUDA; }
-        h->snap_pend = 0; h->snap_cur = 0;
-        { std::lock_guard<std::mutex> g(h->mu); h->pinned = false; }
-        if (fclose(f) != 0 && r == 0) { keep = "snapshot: close failed"; r = AGR_EINVAL; }
-        if (r != 0) h->chain = snap_chain{};                    // a file that failed is no base: the next one is full
-        g_err = keep;
-        return r;
-    };
-    if (chain) return done(snap_write_chain(h, f, path, hd, agents, bound));
-    // the writer stream starts behind the cut; the header's log lengths are the ones the cut read
-    if (cudaStreamWaitEvent(h->snap_stream, h->snap_ev[0], 0) != cudaSuccess ||
-        cudaMemcpyAsync(h->snap_buf[0], h->d_shadow, 16, cudaMemcpyDeviceToHost, h->snap_stream) != cudaSuccess ||
-        cudaStreamSynchronize(h->snap_stream) != cudaSuccess) return done(fail(AGR_ECUDA, "snapshot: cut"));
-    memcpy(hd.log_len, h->snap_buf[0], 16);
-    if (fwrite(&hd, sizeof hd, 1, f) != 1 || fwrite(agents.data(), 1, agents.size(), f) != agents.size())
-        return done(fail(AGR_EINVAL, "snapshot: short write"));
-    int rc = snap_sections(h, hd, f, dump_online, h->d_shadow);
-    if (rc == 0) rc = snap_drain(h, f);
-    return done(rc);
+    int rc = snap_read_cut(h, hd, chain);
+    if (rc == 0) rc = chain ? snap_write_chain(h, f, path, hd, agents, bound) : snap_write_full(h, f, hd, agents, dump_online, h->d_shadow);
+    if (cudaStreamSynchronize(h->snap_stream) != cudaSuccess && rc == 0) rc = fail(AGR_ECUDA, "snapshot: writer stream");
+    h->snap_pend = 0; h->snap_cur = 0;
+    { std::lock_guard<std::mutex> g(h->mu); h->pinned = false; }
+    rc = snap_close(f, rc);
+    if (rc != 0) h->chain = snap_chain{};                      // a file that failed is no base: the next one is full
+    return rc;
 }
 
 int agr_snapshot(agr_handle* h, const char* path) {
@@ -2336,19 +2326,11 @@ int agr_snapshot(agr_handle* h, const char* path) {
     if (!f) return fail(AGR_EINVAL, std::string("snapshot: cannot open ") + path);
     snap_header hd{};
     snap_fill_header(h, hd);
-    unsigned long long lens[2];
-    int rc = 0;
-    auto done = [&](int r) { fclose(f); return r; };
-    if (cudaMemcpy(lens, h->d.log_len, sizeof lens, cudaMemcpyDeviceToHost) != cudaSuccess) return done(fail(AGR_ECUDA, "snapshot: log_len"));
+    unsigned long long lens[2] = {0, 0};
+    int rc = read_log_lens(h, lens);
     hd.log_len[0] = lens[0]; hd.log_len[1] = lens[1];
-    if (fwrite(&hd, sizeof hd, 1, f) != 1) return done(fail(AGR_EINVAL, "snapshot: short write"));
-    for (uint32_t a = 0; a < hd.n_agents; ++a) {
-        char name[AGR_AGENT_ID_BYTES] = {0};
-        strncpy(name, h->agent_names[a].c_str(), AGR_AGENT_ID_BYTES - 1);
-        fwrite(name, 1, AGR_AGENT_ID_BYTES, f); fwrite(&h->agent_status[a], 1, 1, f);
-    }
-    if ((rc = snap_sections(h, hd, f, dump_dev)) < 0) return done(rc);
-    return done(0);
+    if (rc == 0) rc = snap_write_full(h, f, hd, snap_agents(h), dump_dev);
+    return snap_close(f, rc);
 }
 
 // ---- restore: a full file, then the deltas of its chain, oldest first
@@ -2394,17 +2376,12 @@ static int load_blocks(agr_handle* h, FILE* f, agr_snap_blocks g, uint64_t n) {
 }
 // applies one delta (f is past its header and parent path) to the live arrays; the header fields are set by the caller
 static int restore_delta_locked(agr_handle* h, FILE* f, const delta_header& dh) {
-    const snap_header& hd = dh.cut;
-    const bool var = (hd.flags & AGR_CFG_VARLEN) != 0, ring = (hd.flags & AGR_CFG_RING) != 0;
-    const uint64_t unit = var ? 1 : AGR_REC;
-    TRY(restore_agents_locked(h, f, hd.n_agents));
-    uint64_t run[2][2];
-    for (int n = snap_runs(dh.rows_lo, dh.rows_hi, var ? hd.vcap : hd.slab_rows, ring, run), j = 0; j < n; ++j)
-        TRY(load_dev(h, f, h->d.slab + run[j][0] * unit, run[j][1] * unit));
-    for (int n = snap_runs(dh.resp_lo, dh.resp_hi, hd.resp_cap, ring, run), j = 0; j < n; ++j)
-        TRY(load_dev(h, f, h->d_resp + run[j][0], run[j][1]));
-    TRY(load_blocks(h, f, snap_word_blocks(h, hd, false), dh.n_blocks));
-    for (int j = 0; j < 2; ++j) TRY(load_blocks(h, f, snap_log_blocks(h, hd, j, false), dh.n_log_blocks[j]));
+    TRY(restore_agents_locked(h, f, dh.cut.n_agents));
+    snap_piece pc[4];
+    for (int n = snap_delta_pieces(h, dh, pc), j = 0; j < n; ++j) TRY(load_dev(h, f, pc[j].p, pc[j].bytes));
+    agr_snap_blocks g[3];
+    snap_block_tables(h, dh.cut, false, g);
+    for (int t = 0; t < 3; ++t) TRY(load_blocks(h, f, g[t], dh.n_blocks[t]));
     if ((uint64_t)ftello(f) != dh.file_bytes) return fail(AGR_EINVAL, "restore: corrupt delta (its sections do not add up to its size)");
     return 0;
 }

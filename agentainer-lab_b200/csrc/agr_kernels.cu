@@ -1046,7 +1046,7 @@ void agr_launch_drop_agent(const agr_dev& d, uint32_t slot, unsigned long long r
 // ------------------------------------------------------------------------------------------------ online snapshot cut
 // blockIdx.y = section; the blocks of a section stride over it in 16 B pieces, four independent loads in flight per thread,
 // and block 0 copies the tail (< 16 B).  The log lengths are read here, on the device, so the host never waits to learn them.
-__global__ void __launch_bounds__(256) k_snap_cut(const agr_dev d, const agr_snap_cut c) {
+__global__ void __launch_bounds__(256) k_snap_cut(const agr_dev d, const agr_snap_cmp c) {
     const uint32_t s = blockIdx.y;
     unsigned long long bytes = c.bytes[s];
     if (s >= c.nrow) {
@@ -1068,7 +1068,7 @@ __global__ void __launch_bounds__(256) k_snap_cut(const agr_dev d, const agr_sna
         c.shadow[c.dst_off[s] + t] = c.src[s][t];
     }
 }
-void agr_launch_snap_cut(const agr_dev& d, const agr_snap_cut& c, int sm_count, cudaStream_t st) {
+void agr_launch_snap_cut(const agr_dev& d, const agr_snap_cmp& c, int sm_count, cudaStream_t st) {
     unsigned long long most = 0;                      // (the logs are at most log_cap entries)
     for (uint32_t s = 0; s < c.nrow; ++s) most = c.bytes[s] > most ? c.bytes[s] : most;
     if (d.log_cap * 4ull > most) most = d.log_cap * 4ull;

@@ -220,23 +220,16 @@ void agr_launch_synth(uint8_t* dst, agr_synth_dev s, unsigned long long first_in
 // Online snapshot (AGR_CFG_ONLINE_SNAPSHOT): the cut copies the sections that later calls rewrite in place (per-row words, the
 // completed / failed logs) into a device shadow.  Every destination is 256 B-aligned; every source is the start of its array.
 // Sections [0, nrow) have the byte counts given here; sections nrow and nrow + 1 are the completed and failed logs, whose
-// lengths the kernel reads from d.log_len and stores as two u64 at the start of the shadow.
-#define AGR_SNAP_CUT_MAX 16
-struct agr_snap_cut {
-    const uint8_t* src[AGR_SNAP_CUT_MAX];
-    unsigned long long dst_off[AGR_SNAP_CUT_MAX];
-    unsigned long long bytes[AGR_SNAP_CUT_MAX];
-    uint8_t* shadow;
-    uint32_t nrow;
-};
-void agr_launch_snap_cut(const agr_dev& d, const agr_snap_cut& c, int sm_count, cudaStream_t st);
-
+// lengths the kernel reads from d.log_len and stores as two u64 at the start of the shadow.  The cut reads src, dst_off,
+// bytes[0, nrow), shadow and nrow of agr_snap_cmp below.
+//
 // Delta snapshots (AGR_CFG_DELTA_SNAPSHOT).  The compare cut is the cut above that also compares each 16 B piece with what the
 // shadow held (the previous cut) before it overwrites it: a piece that differs sets the bit of its block (256 rows of a word
 // section, 1024 entries of a log) in bits, and every piece, live or not, goes into a 128-bit keyed sum (digest[2], added to).
-// Section s covers bytes[s] bytes (sections nrow and nrow + 1, the logs, as in agr_snap_cut unless lens_from_host); its
+// Section s covers bytes[s] bytes (sections nrow and nrow + 1, the logs, as in the cut unless lens_from_host); its
 // block of piece i is i >> pshift[s], its bit word bit_off[s] + block / 32.  The digest-only pass (compare = false) reads
 // src alone: no shadow, no bits.  The sum does not depend on the grid: it adds one keyed hash per (section, piece).
+#define AGR_SNAP_CUT_MAX 16
 struct agr_snap_cmp {
     const uint8_t* src[AGR_SNAP_CUT_MAX];
     unsigned long long dst_off[AGR_SNAP_CUT_MAX];
@@ -251,6 +244,7 @@ struct agr_snap_cmp {
     uint32_t nrow;
     uint32_t lens_from_host;               // 1: the logs' byte counts are bytes[nrow], bytes[nrow + 1] (restore-time checks)
 };
+void agr_launch_snap_cut(const agr_dev& d, const agr_snap_cmp& c, int sm_count, cudaStream_t st);
 void agr_launch_snap_cmp(const agr_dev& d, const agr_snap_cmp& c, bool compare, int sm_count, cudaStream_t st);
 // Block gather / scatter: block list[j] of a section table (arr[s], width[s] bytes per row, rows rows in all, block_rows rows
 // per block) is packed at stage + j * rec_bytes as each section's slice in table order; the last block of the table may be

@@ -42,13 +42,15 @@ class Restarting:
 
 @pytest.mark.parametrize("mode", sorted(MODES))
 @pytest.mark.parametrize("seed", [1, 2])
-def test_restart_in_mid_stream_is_invisible(mode, seed, tmp_path):
+@pytest.mark.parametrize("online", [False, True], ids=["blocking", "online"])
+def test_restart_in_mid_stream_is_invisible(mode, seed, online, tmp_path):
     ev = random_scenario(400 + seed, n_events=500, n_agents=5, p_replay=0.15)
     if mode == "var":
         from test_varlen_gpu import with_bodies
         ev = with_bodies(ev, seed)
     ref = run_oracle(ev)
-    r = Restarting(MODES[mode], str(tmp_path / "agr.snap"), restart_after_calls=12 + seed)
+    flags = MODES[mode] | (K.AGR_CFG_ONLINE_SNAPSHOT if online else 0)
+    r = Restarting(flags, str(tmp_path / "agr.snap"), restart_after_calls=12 + seed)
     try:
         got = run_engine(r, ev, max_batch=40)
         assert r.restarts == 1
@@ -57,6 +59,20 @@ def test_restart_in_mid_stream_is_invisible(mode, seed, tmp_path):
         assert rows > 100 and bad == 0
     finally:
         r.close()
+
+
+@pytest.mark.parametrize("online", [False, True], ids=["blocking", "online"])
+def test_a_failed_flush_fails_the_snapshot(online):
+    """The file of a small engine fits stdio's buffer whole, so its bytes reach the device only when the file is closed:
+    /dev/full takes every write and refuses that flush.  The snapshot must report it, not succeed."""
+    from scenario import Req, rid_of, make_records
+    flags = MODES["mint"] | (K.AGR_CFG_ONLINE_SNAPSHOT if online else 0)
+    with A.Engine(slab_rows=1 << 10, max_agents=16, flags=flags) as eng:
+        eng.set_agent_state("agent-1", "running")
+        eng.ingest(make_records([Req("agent-1", rid_of(i), i) for i in range(1, 5)]))   # 4 rows: ~2.5 KiB of file
+        with pytest.raises(A.AgrError) as e:
+            eng.snapshot("/dev/full")
+        assert e.value.code == K.AGR_EINVAL
 
 
 def test_verify_detects_a_flipped_bit(tmp_path):

@@ -1,5 +1,5 @@
 """AGR_CFG_DELTA_SNAPSHOT: agr_snapshot writes a delta (AGRDELT1) on the engine's previous snapshot whenever it can, and
-agr_restore follows a delta's parents back to the full file.  A plain reader below applies each delta to the parsed sections
+agr_restore follows a delta's parents back to the full file.  A plain reader (snapfile.py) applies each delta to the parsed sections
 of its parent; at every step the result must be what a twin engine without the flags writes as a full file at the same point,
 and the chain must restore to the twin's state."""
 import os
@@ -11,122 +11,19 @@ import pytest
 import agentainer_lab_b200 as A
 from agentainer_lab_b200 import constants as K
 from jsoncase import make_requests, records_array, var_batch
-from test_snapshot_online_gpu import (AGENTS, HEADER, MODES, RESP, RING_ROWS, VSLAB, WORDS, Driver, PipeSnapshot, SECRET, STEP,
-                                      T0, M, P, R, V,
-                                      engine_kw, outcomes, parse, referenced, sections, submit_ingest, while_writing)
+from snapfile import BLOCK_ROWS, WORDS, apply, expected_blocks, parse, parse_delta, referenced
+from test_snapshot_online_gpu import (AGENTS, MODES, RESP, RING_ROWS, VSLAB, Driver, PipeSnapshot, SECRET, STEP, T0, M, P, R, V,
+                                      assert_same_engine, engine_kw, outcomes, submit_ingest, while_writing)
 
 pytestmark = pytest.mark.gpu
 
 DELTA_FLAGS = K.AGR_CFG_ONLINE_SNAPSHOT | K.AGR_CFG_DELTA_SNAPSHOT
-BLOCK_ROWS, LOG_BLOCK = 256, 1024
-# mirrors struct delta_header in csrc/agr_engine.cu
-DELTA = np.dtype([("magic", "S8"), ("cut", HEADER), ("file_bytes", "<u8"), ("parent_digest", "<u8", (2,)), ("digest", "<u8", (2,)),
-                  ("block_rows", "<u4"), ("log_block", "<u4"), ("rows_lo", "<u8"), ("rows_hi", "<u8"), ("resp_lo", "<u8"),
-                  ("resp_hi", "<u8"), ("n_blocks", "<u8"), ("n_log_blocks", "<u8", (2,)), ("parent_path_len", "<u4"), ("pad", "<u4")])
 
 
 def delta_kw(flags):
     kw = engine_kw(flags, True)
     kw["flags"] |= K.AGR_CFG_DELTA_SNAPSHOT
     return kw
-
-
-def runs(lo, hi, cap, ring):
-    if hi <= lo:
-        return []
-    p = lo % cap if ring else lo
-    n0 = min(hi - lo, cap - p) if ring else hi - lo
-    return [(p, n0)] + ([(0, hi - lo - n0)] if hi - lo > n0 else [])
-
-
-def parse_delta(data: bytes):
-    """The fields of an AGRDELT1 file; every byte of it is accounted for."""
-    dh = np.frombuffer(data, dtype=DELTA, count=1)[0]
-    assert dh["magic"] == b"AGRDELT1" and int(dh["file_bytes"]) == len(data)
-    assert (int(dh["block_rows"]), int(dh["log_block"])) == (BLOCK_ROWS, LOG_BLOCK)
-    hd = dh["cut"]
-    ring, var = bool(hd["flags"] & R), bool(hd["flags"] & V)
-    at = DELTA.itemsize
-    n = int(dh["parent_path_len"])
-    out = {"dh": dh, "hd": hd, "parent": data[at: at + n].decode()}
-    at += n
-    out["agents"] = data[at: at + 33 * int(hd["n_agents"])]
-    at += len(out["agents"])
-    unit = 1 if var else 512
-    cap = int(hd["vcap"]) if var else int(hd["slab_rows"])
-    out["rows"] = []
-    for p, k in runs(int(dh["rows_lo"]), int(dh["rows_hi"]), cap, ring):
-        out["rows"].append((p * unit, data[at: at + k * unit])); at += k * unit
-    out["resp"] = []
-    for p, k in runs(int(dh["resp_lo"]), int(dh["resp_hi"]), int(hd["resp_cap"]), ring):
-        out["resp"].append((p, data[at: at + k])); at += k
-    secs = {name: (dt, count) for name, dt, count in sections(hd)}
-    words = [w for w in WORDS if secs[w][1]]
-    rows = secs["state"][1]
-
-    def blocks(names, count, per, nb):
-        nonlocal at
-        lst = np.frombuffer(data, dtype="<u4", count=nb, offset=at).astype(np.int64)
-        at += 4 * nb
-        assert np.all(np.diff(lst) > 0) and (nb == 0 or lst[-1] * per < count)
-        got = []
-        for b in lst:
-            r = min(per, count - b * per)
-            sl = {}
-            for w in names:
-                dt = np.dtype(secs[w][0])
-                sl[w] = np.frombuffer(data, dtype=dt, count=r, offset=at); at += r * dt.itemsize
-            got.append((int(b), sl))
-        return lst, got
-    out["wl"], out["words"] = blocks(words, rows, BLOCK_ROWS, int(dh["n_blocks"]))
-    out["ll"], out["logs"] = [], []
-    for j, name in enumerate(("completed_log", "failed_log")):
-        lst, got = blocks([name], secs[name][1], LOG_BLOCK, int(dh["n_log_blocks"][j]))
-        out["ll"].append(lst); out["logs"].append(got)
-    assert at == len(data)
-    return out
-
-
-def apply(sec_p, d):
-    """The sections the delta brings its parent's sections (sec_p) to."""
-    sec = {}
-    for name, dt, count in sections(d["hd"]):
-        a = np.zeros(count, dtype=dt)
-        old = sec_p[name]
-        k = min(count, len(old))
-        a[:k] = old[:k]
-        sec[name] = a
-    for name, pieces in (("slab", d["rows"]), ("resp", d["resp"])):
-        for p, b in pieces:
-            sec[name][p: p + len(b)] = np.frombuffer(b, dtype=np.uint8)
-    for b, sl in d["words"]:
-        for w, v in sl.items():
-            sec[w][b * BLOCK_ROWS: b * BLOCK_ROWS + len(v)] = v
-    for j, name in enumerate(("completed_log", "failed_log")):
-        for b, sl in d["logs"][j]:
-            v = sl[name]
-            sec[name][b * LOG_BLOCK: b * LOG_BLOCK + len(v)] = v
-    return sec
-
-
-def expected_blocks(sec_a, hd_a, sec_b, hd_b):
-    """Blocks where two consecutive full files differ, plus those reaching past the earlier file's rows / log length."""
-    Ra, Rb = len(sec_a["state"]), len(sec_b["state"])
-    dirty = set(range(Ra // BLOCK_ROWS, (Rb + BLOCK_ROWS - 1) // BLOCK_ROWS))
-    for w in WORDS:
-        a, b = sec_a[w], sec_b[w]
-        if len(b) == 0:
-            continue
-        diff = np.nonzero(a[: min(len(a), len(b))] != b[: len(a)])[0]
-        dirty |= set((diff // BLOCK_ROWS).tolist())
-    logs = []
-    for name in ("completed_log", "failed_log"):
-        a, b = sec_a[name], sec_b[name]
-        d = set(range(len(a) // LOG_BLOCK, (len(b) + LOG_BLOCK - 1) // LOG_BLOCK))
-        k = min(len(a), len(b))
-        d |= set((np.nonzero(a[:k] != b[:k])[0] // LOG_BLOCK).tolist())
-        logs.append(sorted(d))
-    return sorted(b for b in dirty if b * BLOCK_ROWS < Rb), logs
 
 
 def assert_same_sections(hd, agents, sec, hd_t, agents_t, sec_t, var):
@@ -137,26 +34,6 @@ def assert_same_sections(hd, agents, sec, hd_t, agents_t, sec_t, var):
     slab_m, resp_m, live = referenced(sec_t, hd_t, var)
     assert np.array_equal(sec["slab"][slab_m], sec_t["slab"][slab_m])
     assert np.array_equal(sec["resp"][resp_m], sec_t["resp"][resp_m])
-
-
-def assert_same_engine(back, twin, drv, used, var):
-    assert back.verify()[1] == 0
-    for a in AGENTS:
-        for which in (K.AGR_LIST_PENDING, K.AGR_LIST_COMPLETED, K.AGR_LIST_FAILED):
-            assert np.array_equal(back.list(a, which), twin.list(a, which)), (a, which)
-        if not var:
-            assert back.pending(a).tobytes() == twin.pending(a).tobytes()
-    for L, (a, rid) in drv.ids.items():
-        if L >= used:
-            continue
-        assert back.get_record_json(a, rid) == twin.get_record_json(a, rid), L
-        assert back.get_response_body(a, rid) == twin.get_response_body(a, rid), L
-    if var:
-        got, want = back.replay_scan_var(), twin.replay_scan_var()
-        assert all(np.array_equal(x, y) for x, y in zip(got, want))
-    else:
-        got, want = back.replay_scan(), twin.replay_scan()
-        assert got[0].tobytes() == want[0].tobytes() and got[1].tobytes() == want[1].tobytes()
 
 
 def traffic(drv, engines, step, combine, ttl=3 * STEP):

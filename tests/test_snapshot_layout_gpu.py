@@ -9,6 +9,7 @@ import pytest
 import agentainer_lab_b200 as A
 from agentainer_lab_b200 import constants as K
 from jsoncase import make_requests, records_array, var_batch
+from snapfile import parse
 
 pytestmark = pytest.mark.gpu
 
@@ -24,40 +25,7 @@ MODES = {"hash": K.AGR_CFG_PERSISTENCE, "mint": K.AGR_CFG_PERSISTENCE | K.AGR_CF
          "ring": K.AGR_CFG_PERSISTENCE | K.AGR_CFG_MINT_IDS | K.AGR_CFG_RING,
          "var_ring": K.AGR_CFG_PERSISTENCE | K.AGR_CFG_VARLEN | K.AGR_CFG_MINT_IDS | K.AGR_CFG_RING}
 
-# mirrors struct snap_header in csrc/agr_engine.cu
-HEADER = np.dtype([("magic", "S8"), ("flags", "<u4"), ("n_agents", "<u4"), ("shard", "<u4"), ("gen", "<u4"),
-                   ("rows_used", "<u8"), ("vused", "<u8"), ("log_len", "<u8", (2,)), ("id_secret", "<u8"), ("scan_lo", "<u8"),
-                   ("resp_used", "<u8"), ("expired_total", "<u8"), ("tail", "<u8"), ("released_total", "<u8"), ("slab_rows", "<u8"),
-                   ("vtail", "<u8"), ("vcap", "<u8"), ("resp_tail", "<u8"), ("resp_cap", "<u8")])
 AGENT_ENTRY = 32 + 1                      # NUL-padded agent id, status byte
-
-
-def sections(hd):
-    """(name, dtype, count) of every section after the agent table, in file order: mirrors snap_sections in
-    csrc/agr_engine.cu."""
-    ring, var = bool(hd["flags"] & K.AGR_CFG_RING), bool(hd["flags"] & K.AGR_CFG_VARLEN)
-    rows = int(min(hd["rows_used"], hd["slab_rows"])) if ring else int(hd["rows_used"])
-    slab = (int(min(hd["vused"], hd["vcap"])) if ring else int(hd["vused"])) if var else rows * 512
-    resp = int(min(hd["resp_used"], hd["resp_cap"])) if ring else int(hd["resp_used"])
-    return [("slab", np.uint8, slab), ("state", "<u4", rows), ("route", "<u4", rows), ("aux", "<u4", rows), ("cksum", "<u8", rows),
-            ("voff", "<u8", rows if var else 0), ("vlen", "<u4", rows if var else 0),
-            ("completed_log", "<u4", int(hd["log_len"][0])), ("failed_log", "<u4", int(hd["log_len"][1])),
-            ("resp", np.uint8, resp), ("resp_off", "<u8", rows), ("resp_len", "<u4", rows), ("resp_hlen", "<u4", rows),
-            ("err_off", "<u8", rows), ("err_len", "<u4", rows), ("ptime", "<u8", rows), ("mtime", "<u8", rows)]
-
-
-def parse(data: bytes):
-    hd = np.frombuffer(data, dtype=HEADER, count=1)[0]
-    at = HEADER.itemsize
-    agents = []
-    for _ in range(int(hd["n_agents"])):
-        agents.append((data[at: at + 32].rstrip(b"\0").decode(), data[at + 32]))
-        at += AGENT_ENTRY
-    sec = {}
-    for name, dt, count in sections(hd):
-        sec[name] = np.frombuffer(data, dtype=dt, count=count, offset=at)
-        at += sec[name].nbytes
-    return hd, agents, sec, at
 
 
 def device_bytes(ptr: int, n: int) -> bytes:
@@ -147,15 +115,15 @@ def test_snapshot_sections_match_the_engine(mode, tmp_path):
         path = str(tmp_path / f"{mode}.snap")
         eng.snapshot(path)
         data = open(path, "rb").read()
-        hd, agents, sec, end = parse(data)
+        hd, agents, sec = parse(data)                         # (parse asserts that the sections account for every byte of the file)
 
-        assert end == len(data)                               # the sections account for every byte of the file
         assert hd["magic"] == b"AGRSNAP3"
         assert int(hd["flags"]) == flags & (K.AGR_CFG_PERSISTENCE | K.AGR_CFG_MINT_IDS | K.AGR_CFG_VARLEN | K.AGR_CFG_RING)
         assert int(hd["id_secret"]) == SECRET and int(hd["slab_rows"]) == S
         used, tail = int(hd["rows_used"]), int(hd["tail"])
         assert used == st["rows_used"] and tail == st["rows_tail"]
-        assert agents == [(a, K.AGENT_STATUS_CODES[s]) for a, s in zip(AGENTS, STATUS)]
+        entries = [agents[at: at + AGENT_ENTRY] for at in range(0, len(agents), AGENT_ENTRY)]
+        assert [(e[:32].rstrip(b"\0").decode(), e[32]) for e in entries] == [(a, K.AGENT_STATUS_CODES[s]) for a, s in zip(AGENTS, STATUS)]
         if ring:                                              # each ring has gone round: its sections hold one lap
             assert used > S and tail > 0 and int(hd["resp_used"]) > int(hd["resp_cap"]) == RESP
             assert not var or int(hd["vused"]) > int(hd["vcap"]) == VSLAB

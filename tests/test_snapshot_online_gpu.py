@@ -13,7 +13,7 @@ import pytest
 import agentainer_lab_b200 as A
 from agentainer_lab_b200 import constants as K
 from jsoncase import make_requests, records_array, var_batch
-from scenario import run_oracle, run_engine, assert_same, random_scenario
+from snapfile import HEADER, WORDS, parse, referenced
 
 pytestmark = pytest.mark.gpu
 
@@ -28,38 +28,6 @@ P, M, V, R = K.AGR_CFG_PERSISTENCE, K.AGR_CFG_MINT_IDS, K.AGR_CFG_VARLEN, K.AGR_
 MODES = {"hash": P, "mint": P | M, "var": P | V | M, "ring": P | M | R, "var_ring": P | V | M | R,
          "ring_combine": P | M | R | K.AGR_CFG_COMBINE}
 JOIN_S = 120                                  # the traffic during a write finishes long before this unless the writer holds the engine
-
-# mirrors struct snap_header in csrc/agr_engine.cu
-HEADER = np.dtype([("magic", "S8"), ("flags", "<u4"), ("n_agents", "<u4"), ("shard", "<u4"), ("gen", "<u4"),
-                   ("rows_used", "<u8"), ("vused", "<u8"), ("log_len", "<u8", (2,)), ("id_secret", "<u8"), ("scan_lo", "<u8"),
-                   ("resp_used", "<u8"), ("expired_total", "<u8"), ("tail", "<u8"), ("released_total", "<u8"), ("slab_rows", "<u8"),
-                   ("vtail", "<u8"), ("vcap", "<u8"), ("resp_tail", "<u8"), ("resp_cap", "<u8")])
-WORDS = ("state", "route", "aux", "cksum", "voff", "vlen", "resp_off", "resp_len", "resp_hlen", "err_off", "err_len", "ptime", "mtime")
-
-
-def sections(hd):
-    """(name, dtype, count) of every section after the agent table, in file order (the AGRSNAP3 layout)."""
-    ring, var = bool(hd["flags"] & R), bool(hd["flags"] & V)
-    rows = int(min(hd["rows_used"], hd["slab_rows"])) if ring else int(hd["rows_used"])
-    slab = (int(min(hd["vused"], hd["vcap"])) if ring else int(hd["vused"])) if var else rows * 512
-    resp = int(min(hd["resp_used"], hd["resp_cap"])) if ring else int(hd["resp_used"])
-    return [("slab", np.uint8, slab), ("state", "<u4", rows), ("route", "<u4", rows), ("aux", "<u4", rows), ("cksum", "<u8", rows),
-            ("voff", "<u8", rows if var else 0), ("vlen", "<u4", rows if var else 0),
-            ("completed_log", "<u4", int(hd["log_len"][0])), ("failed_log", "<u4", int(hd["log_len"][1])),
-            ("resp", np.uint8, resp), ("resp_off", "<u8", rows), ("resp_len", "<u4", rows), ("resp_hlen", "<u4", rows),
-            ("err_off", "<u8", rows), ("err_len", "<u4", rows), ("ptime", "<u8", rows), ("mtime", "<u8", rows)]
-
-
-def parse(data: bytes):
-    hd = np.frombuffer(data, dtype=HEADER, count=1)[0]
-    at = HEADER.itemsize + 33 * int(hd["n_agents"])
-    agents = data[HEADER.itemsize: at]
-    sec = {}
-    for name, dt, count in sections(hd):
-        sec[name] = np.frombuffer(data, dtype=dt, count=count, offset=at)
-        at += sec[name].nbytes
-    assert at == len(data)
-    return hd, agents, sec
 
 
 def outcomes(rows):
@@ -218,25 +186,24 @@ def while_writing(snap, fn):
     return box.get("out")
 
 
-def referenced(sec, hd, var):
-    """Byte masks of the slab and the response bytes that some row of the cut's window refers to (everything else there
-    is unspecified: outside the window, skipped at a lap's end, or never written by either engine, such as 16 B padding)."""
-    ring = bool(hd["flags"] & R)
-    S, used, tail = int(hd["slab_rows"]), int(hd["rows_used"]), int(hd["tail"])
-    live = [(L % S) if ring else L for L in range(tail, used)]
-    live = [p for p in live if sec["state"][p] != 0]
-    slab = np.zeros(len(sec["slab"]), dtype=bool)
-    resp = np.zeros(len(sec["resp"]), dtype=bool)
-    for p in live:
-        if var:
-            o = int(sec["voff"][p]); slab[o: o + int(sec["vlen"][p])] = True
-        else:
-            slab[p * 512: (p + 1) * 512] = True
-        for off, ln in (("resp_off", "resp_len"), ("err_off", "err_len")):
-            n = int(sec[ln][p])
-            if n:
-                o = int(sec[off][p]); resp[o: o + n] = True
-    return slab, resp, live
+def assert_same_engine(back, twin, drv, used, var):
+    assert back.verify()[1] == 0
+    for a in AGENTS:
+        for which in (K.AGR_LIST_PENDING, K.AGR_LIST_COMPLETED, K.AGR_LIST_FAILED):
+            assert np.array_equal(back.list(a, which), twin.list(a, which)), (a, which)
+        if not var:
+            assert back.pending(a).tobytes() == twin.pending(a).tobytes()
+    for L, (a, rid) in drv.ids.items():
+        if L >= used:
+            continue
+        assert back.get_record_json(a, rid) == twin.get_record_json(a, rid), L
+        assert back.get_response_body(a, rid) == twin.get_response_body(a, rid), L
+    if var:
+        got, want = back.replay_scan_var(), twin.replay_scan_var()
+        assert all(np.array_equal(x, y) for x, y in zip(got, want))
+    else:
+        got, want = back.replay_scan(), twin.replay_scan()
+        assert got[0].tobytes() == want[0].tobytes() and got[1].tobytes() == want[1].tobytes()
 
 
 @pytest.mark.parametrize("mode", sorted(MODES))
@@ -304,23 +271,7 @@ def test_online_file_is_the_cut_and_restores_like_the_twin(mode, tmp_path):
 
         # restored from the online file: the same state as the twin
         with A.Engine(restore_from=_save(tmp_path, data), **engine_kw(flags, False)) as back:
-            assert back.verify()[1] == 0
-            for a in AGENTS:
-                for which in (K.AGR_LIST_PENDING, K.AGR_LIST_COMPLETED, K.AGR_LIST_FAILED):
-                    assert np.array_equal(back.list(a, which), twin.list(a, which)), (a, which)
-                if not var:
-                    assert back.pending(a).tobytes() == twin.pending(a).tobytes()
-            for L, (a, rid) in drv.ids.items():
-                if L >= used:
-                    continue
-                assert back.get_record_json(a, rid) == twin.get_record_json(a, rid), L
-                assert back.get_response_body(a, rid) == twin.get_response_body(a, rid), L
-            if var:
-                got, want = back.replay_scan_var(), twin.replay_scan_var()
-                assert all(np.array_equal(x, y) for x, y in zip(got, want))
-            else:
-                got, want = back.replay_scan(), twin.replay_scan()
-                assert got[0].tobytes() == want[0].tobytes() and got[1].tobytes() == want[1].tobytes()
+            assert_same_engine(back, twin, drv, used, var)
 
 
 def _save(tmp_path, data):
@@ -447,46 +398,3 @@ def test_cut_time_is_reported(tmp_path):
             eng.op_time(3)                                         # no cut yet
         eng.snapshot(str(tmp_path / "t.snap"))
         assert eng.op_time(3) > 0
-
-
-# ---- the restart-in-mid-stream scenario of the blocking path, with the flag, against the oracle
-class Restarting:
-    def __init__(self, flags, path, restart_after_calls):
-        self.kw = dict(slab_rows=1 << 15, max_agents=256, flags=flags, vslab_bytes=64 << 20)
-        self.eng, self.path, self.left = A.Engine(**self.kw), path, restart_after_calls
-        self.mint, self.varlen = self.eng.mint, self.eng.varlen
-        self.restarts = 0
-
-    def __getattr__(self, name):
-        target = getattr(self.eng, name)
-        if name in ("ingest", "ingest_var", "complete") and self.left is not None:
-            self.left -= 1
-            if self.left == 0:
-                self.left = None
-                self.eng.snapshot(self.path)
-                self.eng.close()
-                self.eng = A.Engine(restore_from=self.path, **self.kw)
-                self.restarts += 1
-                target = getattr(self.eng, name)
-        return target
-
-    def close(self):
-        self.eng.close()
-
-
-@pytest.mark.parametrize("mode", ["hash", "mint", "var"])
-def test_restart_in_mid_stream_with_online_snapshot(mode, tmp_path):
-    ev = random_scenario(401, n_events=500, n_agents=5, p_replay=0.15)
-    if mode == "var":
-        from test_varlen_gpu import with_bodies
-        ev = with_bodies(ev, 1)
-    ref = run_oracle(ev)
-    r = Restarting(MODES[mode] | K.AGR_CFG_ONLINE_SNAPSHOT, str(tmp_path / "agr.snap"), restart_after_calls=13)
-    try:
-        got = run_engine(r, ev, max_batch=40)
-        assert r.restarts == 1
-        assert_same(ref, got)
-        rows, bad = r.eng.verify()
-        assert rows > 100 and bad == 0
-    finally:
-        r.close()
