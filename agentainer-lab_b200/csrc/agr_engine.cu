@@ -1,38 +1,11 @@
-// agr_engine.cu — host side of the engine and the C-ABI of include/agentainer_gpu.h.
+// agr_engine.cu — host side of the engine and the C-ABI of include/agentainer_gpu.h: the core (the other parts: agr_engine.h).
 //
 // One agr_handle == one GPU shard: HBM slab + SoA state + dedupe index + logs + agent-table mirror, one stream.
 // Calls are linearised by the handle mutex; the order in which calls take it is the event order the state
 // machine sees (the reference's serialisation point is the single-threaded Redis server).
 // There is NO CPU fallback: every state transition happens in the kernels of agr_kernels.cu.
-#include <cuda_runtime.h>
-#include <dlfcn.h>
 #include <sys/random.h>
-#include <nccl.h>      // types only: every NCCL symbol is resolved with dlopen/dlsym at run time
-#include <limits.h>
-#include <stdint.h>
-#include <stdio.h>
-#include <stdlib.h>
-#include <sys/stat.h>
-#include <string.h>
-
-#include <algorithm>
-#include <thread>
-#include <condition_variable>
-#include <mutex>
-#include <string>
-#include <unordered_map>
-#include <vector>
-
-#include "../../include/agentainer_gpu.h"
-#include "agr_kernels.cuh"
-#include "agr_svc.h"
-#include <atomic>
-#include <chrono>
-#include <immintrin.h>
-#include <sched.h>
-#include <time.h>
-#include <sys/prctl.h>
-#include "agr_ring.hpp"
+#include "agr_engine.h"
 
 static_assert(sizeof(agr_record) == 512, "agr_record must be 512 B");
 static_assert(sizeof(agr_outcome) == 64, "agr_outcome must be 64 B");
@@ -43,202 +16,10 @@ static_assert(sizeof(agr_agent_key) == 48, "agr_agent_key must be 48 B");
 static_assert(sizeof(agr_dop) == 32, "agr_dop must be 32 B");
 static_assert(sizeof(agr_k2op) == 16, "agr_k2op must be 16 B");
 
-static thread_local std::string g_err;
-static int fail(int code, const std::string& msg) { g_err = msg; return code; }
-
-#define CK(call)                                                                                     \
-    do {                                                                                             \
-        cudaError_t e_ = (call);                                                                     \
-        if (e_ != cudaSuccess)                                                                       \
-            return fail(AGR_ECUDA, std::string(#call) + ": " + cudaGetErrorString(e_));              \
-    } while (0)
-
-// One exchange over a batch: K4's launch parameters, the per-peer send / receive counts, and their offsets.  Send offsets are
-// owner-major (in-place mode: the peers' segments only), receive offsets source-major.
-struct exchange_plan {
-    agr_k4_params p{};
-    uint32_t G = 1, me = 0, scnt[32], rcnt[32], soff[33], roff[33], n_local = 0, n_recv = 0;
-    uint32_t recv_res_base = 0;      // index of the first received item's result in the result array
-};
-
-// grow-only scratch: a buffer and the element count it was allocated with (regrow sets both)
-template <typename T>
-struct scratch {
-    T* p = nullptr;
-    size_t cap = 0;
-};
-
-// the header of a full snapshot file (agr_snapshot); a delta file carries the one of its cut
-struct snap_header {
-    char magic[8];                 // "AGRSNAP3"
-    uint32_t flags, n_agents, shard, gen;
-    uint64_t rows_used, vused, log_len[2], id_secret, scan_lo, resp_used, expired_total, tail, released_total, slab_rows, vtail, vcap, resp_tail, resp_cap;
-};
-// AGR_CFG_DELTA_SNAPSHOT: what the next snapshot builds on — the files since the last full one (absolute paths, oldest
-// first), the full file's size and the deltas' total, the last cut's header, its ingested bound and its digest
-struct snap_chain {
-    std::vector<std::string> paths;
-    uint64_t full_bytes = 0, delta_bytes = 0;
-    snap_header base{};
-    uint64_t base_bound = 0;
-    unsigned long long digest[2] = {0, 0};
-};
-
-struct agr_handle {
-    std::mutex mu;
-    agr_config cfg{};
-    int device = 0;
-    int sm_count = 132;
-    cudaStream_t stream = nullptr;
-    cudaStream_t copy_stream = nullptr;        // H2D of chunk k+1 overlaps K1 of chunk k (agr_ingest pipeline)
-    std::vector<cudaEvent_t> chunk_ev;
-    cudaStream_t d2h_stream = nullptr;         // verdicts / ids of chunk k go back while chunk k+1 comes in (PCIe is full duplex)
-    std::vector<cudaEvent_t> out_ev;
-    agr_verdict* d_verdicts = nullptr;         // [max_batch], written by k1_post
-    agr_verdict* h_verdicts = nullptr;         // pinned [max_batch]
-    uint8_t* d_ids = nullptr;                  // [max_batch][16] Request.ID per record (agr_ingest_ex)
-    uint8_t* h_ids = nullptr;                  // pinned
-    agr_dev d{};
-    uint64_t rows_used = 0;   // LOGICAL rows handed out so far (ring: includes the rows skipped at a wrap)
-    uint64_t tail = 0;        // ring: first logical row that has not been released
-    uint32_t* d_log_scratch = nullptr; uint32_t* d_lc_chunks = nullptr;   // ring: log compaction
-    uint64_t released_total = 0;
-    uint32_t* d_reclaim_scratch = nullptr;                        // k_first_live: {offset found, ticket}
-    uint8_t* d_reclaim = nullptr; uint8_t* h_reclaim = nullptr;   // agr_reclaim's scan result (device scratch / pinned copy)
-    cudaEvent_t reclaim_ev = nullptr; bool reclaim_pending = false; uint64_t reclaim_bound = 0;
-    uint32_t* dupfix_base = nullptr; uint32_t batch_phase = 0;   // two sets of per-batch words, used alternately
-    uint64_t scan_lo = 0;     // every row below has left its pending list for good
-    uint64_t sweep_clean = 0; // append-only slab: rows below were ingested when agr_expire last ran (their chunks' time bounds are exact)
-    // host agent map + mirror
-    std::unordered_map<std::string, uint32_t> slot_of;
-    std::vector<std::string> agent_names;
-    std::vector<uint8_t> agent_status;
-    std::vector<agr_agent_key> akeys_host;
-    std::vector<uint32_t> akey_index;          // slot -> index of its entry in the open-addressing key table
-    // staging
-    uint8_t* bounce[2] = {nullptr, nullptr};   // pinned, for pageable caller buffers
-    cudaEvent_t bounce_ev[2] = {nullptr, nullptr};
-    size_t bounce_bytes = 0;
-    agr_dop* h_ops = nullptr;                  // pinned [16] (single-key lookups)
-    agr_outcome* h_outs = nullptr;             // pinned [max_batch]
-    agr_outcome* d_outs = nullptr;             // [max_batch]
-    int32_t* h_results = nullptr;              // pinned [max_batch]
-    agr_k2_scratch k2{};
-    uint32_t* d_hrid = nullptr;                // rows found by the single-key resolve (k_resolve)
-    uint32_t* h_k2flag = nullptr;              // pinned: k2_append's overflow flag of the last batch
-    agr_dop* d_ops = nullptr;
-    std::vector<std::pair<uint64_t, uint64_t>> resv;   // rows handed out by agr_reserve_rows and not ingested yet: [first, end)
-    // K3
-    scratch<uint32_t> d_matrix, d_cta_matrix;
-    scratch<uint32_t> d_selmask;               // one selection bit per scanned item (k3_mark -> k3_place)
-    uint32_t* d_gtotal = nullptr; uint32_t* d_goff = nullptr;
-    scratch<uint32_t> d_out_rid, d_out_slot;
-    uint32_t* d_min_inq = nullptr;
-    scratch<uint8_t> d_gather, h_gather;       // (h_gather pinned)
-    uint32_t* h_small = nullptr;               // pinned scratch (>= 64 words)
-    scratch<unsigned long long> d_cdf;
-    // launch accounting
-    uint64_t k1_launches = 0, k2_launches = 0, k3_launches = 0, k4_launches = 0;
-    uint64_t replay_scans = 0, replay_dispatched = 0;
-    std::vector<void*> dev_allocs, host_allocs;
-    alignas(64) unsigned char tmap[128];       // CUtensorMap of the slab for the TMA K1 variants
-    // stored responses: byte slab + per-row (offset, length), written off the hot path
-    uint8_t* d_resp = nullptr; uint64_t resp_used = 0, resp_cap = 0;   // bytes appended so far (ring: logical, pads included) / capacity
-    uint64_t resp_tail = 0;                    // ring: logical offset of the oldest byte a live row still refers to
-    unsigned long long* d_resp_off = nullptr; uint32_t* d_resp_len = nullptr;
-    uint32_t* d_resp_hlen = nullptr;           // leading bytes of the stored response that are its flattened headers
-    unsigned long long* d_err_off = nullptr; uint32_t* d_err_len = nullptr;   // Request.Error text, same byte slab
-    // agr_complete_ex staging, allocated on first use: per-op offsets / slab places / header lengths, and the batch's bytes
-    unsigned long long *h_boff = nullptr, *d_boff = nullptr, *h_bdst = nullptr, *d_bdst = nullptr;
-    uint32_t *h_bhlen = nullptr, *d_bhlen = nullptr;
-    scratch<uint8_t> h_bsrc, d_bsrc;           // (h_bsrc pinned)
-    // K5 (JSON wire form) scratch
-    scratch<uint32_t> d_jlen; scratch<unsigned long long> d_joff, d_jchunk;
-    scratch<uint8_t> d_json;
-    uint64_t k5_launches = 0;
-    uint64_t expired_total = 0;                // records dropped by agr_expire so far
-    // single-request front end (AGR_CFG_COMBINE): pinned op ring + dispatcher thread + resident service kernel (agr_svc.h)
-    struct svc_host* svc = nullptr;
-    // variable-length mode
-    uint64_t vused = 0, vcap = 0;               // bytes appended so far (ring: logical, pads included) / capacity
-    uint64_t vtail = 0;                        // ring: logical offset of the first byte that has not been released
-    uint32_t* d_voffsets = nullptr; uint32_t* d_tile_first = nullptr;   // per-batch offsets [max_batch+1], tile index
-    uint32_t* h_voffsets = nullptr;
-    scratch<uint32_t> d_lens; scratch<unsigned long long> d_goffs;      // gather scratch
-    // multi-GPU exchange (K4)
-    ncclComm_t comm = nullptr; int rank = 0, world = 1;
-    uint8_t* d_stage = nullptr;                // incoming batch before binning [max_batch * 512]
-    uint8_t* d_send = nullptr;                 // owner-major send buffer [max_batch * 512]
-    uint8_t* d_owner = nullptr; uint32_t* d_perm = nullptr;
-    uint32_t* d_k4matrix = nullptr; uint32_t k4_nwarps = 0;
-    uint32_t* d_k4cnt = nullptr;               // [4][32]: gtotal, goff(33 → second row pair), recv counts
-    agr_verdict* d_xverd = nullptr;            // verdicts of local + received rows [2 * max_batch]
-    agr_verdict* d_vback = nullptr;            // verdicts returned by owners, owner-major [max_batch]
-    agr_verdict* d_vout = nullptr;             // caller-order verdicts [max_batch]
-    exchange_plan xdbg{}; uint64_t xdbg_first = 0; uint32_t xdbg_n = 0; bool xdbg_open = false;   // agr_debug_exchange_begin -> _end
-    // AGR_CFG_TIMING: CUDA-event pairs around the dominant K1 kernel, on the launching stream
-    std::vector<cudaEvent_t> tev; uint64_t tev_next = 0, tev_read = 0, timing_calls = 0;
-    cudaEvent_t op_ev[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // [0,1] last K2 group, [2,3] last K3 select group, [4,5] last K5 encode, [6,7] last snapshot cut
-    bool op_timed[4] = {false, false, false, false};
-    // AGR_CFG_ONLINE_SNAPSHOT: the cut's device shadow of the sections rewritten in place (the two log lengths at offset 0, then
-    // every such section at shadow_off), the writer's own stream, its two pinned buffers, and the pins (agr_snapshot)
-    uint8_t* d_shadow = nullptr; size_t shadow_off[17] = {};
-    cudaStream_t snap_stream = nullptr;
-    cudaEvent_t snap_ev[3] = {nullptr, nullptr, nullptr};   // [0] the cut, [1 + b] the last copy into snap_buf[b]
-    uint8_t* snap_buf[2] = {nullptr, nullptr}; size_t snap_buf_bytes = 0;
-    int snap_cur = 0; size_t snap_pend = 0;                 // buffer of the next chunk; bytes of the chunk waiting in the other one
-    std::mutex snap_mu;                                      // one online snapshot at a time: there is one shadow
-    bool pinned = false; uint64_t pin_tail = 0, pin_vtail = 0, pin_resp_tail = 0;   // (h->mu) the cut's ring tails while it is written
-    // AGR_CFG_DELTA_SNAPSHOT (and a restore that applies deltas): the compare cut's dirty bits (word blocks, then the completed
-    // and failed logs' blocks at snap_bit_off[1], [2]) and digest, the pinned copy the writer reads them from (the digest at
-    // offset 16, the bits at 32), the device block list and the staging buffer of the block gather / scatter
-    uint32_t* d_snap_bits = nullptr; unsigned long long* d_snap_digest = nullptr; uint8_t* h_snap_bits = nullptr;
-    size_t snap_bit_off[3] = {}, snap_bit_words = 0;
-    uint32_t* d_snap_list = nullptr; uint8_t* d_snap_stage = nullptr; size_t snap_stage_bytes = 0;
-    snap_chain chain;                                        // (snap_mu) empty: the next snapshot is a full file
-};
-#define AGR_TIMING_RING 1024
-
-template <typename T>
-static int dev_alloc(agr_handle* h, T** p, size_t count, bool zero) {
-    void* q = nullptr;
-    cudaError_t e = cudaMalloc(&q, count * sizeof(T));
-    if (e != cudaSuccess) return fail(AGR_ENOMEM, std::string("cudaMalloc ") + std::to_string(count * sizeof(T)) + " B: " + cudaGetErrorString(e));
-    if (zero) { e = cudaMemsetAsync(q, 0, count * sizeof(T), h->stream); if (e != cudaSuccess) return fail(AGR_ECUDA, cudaGetErrorString(e)); }
-    h->dev_allocs.push_back(q);
-    *p = (T*)q;
-    return 0;
-}
-template <typename T>
-static int host_alloc(agr_handle* h, T** p, size_t count) {
-    void* q = nullptr;
-    cudaError_t e = cudaHostAlloc(&q, count * sizeof(T), cudaHostAllocDefault);
-    if (e != cudaSuccess) return fail(AGR_ENOMEM, std::string("cudaHostAlloc: ") + cudaGetErrorString(e));
-    h->host_allocs.push_back(q);
-    *p = (T*)q;
-    return 0;
-}
-#define TRY(x) do { int r_ = (x); if (r_ < 0) return r_; } while (0)
-// replaces s by a buffer of count elements (device memory, or pinned host memory) and releases the old one (every user of
-// the old buffer has been synchronised by then: the callers hold the handle mutex and the previous operation ended with a
-// stream sync)
-template <typename T>
-static int regrow(agr_handle* h, scratch<T>& s, size_t count, bool pinned = false) {
-    T* old = s.p;
-    TRY(pinned ? host_alloc(h, &s.p, count) : dev_alloc(h, &s.p, count, false));
-    s.cap = count;
-    if (old) {
-        cudaStreamSynchronize(h->stream);
-        std::vector<void*>& allocs = pinned ? h->host_allocs : h->dev_allocs;
-        auto it = std::find(allocs.begin(), allocs.end(), (void*)old);
-        if (it != allocs.end()) allocs.erase(it);
-        if (pinned) cudaFreeHost(old); else cudaFree(old);
-    }
-    return 0;
-}
-
+namespace agr_impl __attribute__((visibility("hidden"))) {
+thread_local std::string g_err;
 // K2 scratch for up to n outcomes per batch
-static int k2_scratch_alloc(agr_handle* h, size_t n) {
+int k2_scratch_alloc(agr_handle* h, size_t n) {
     TRY(dev_alloc(h, &h->k2.ops, n, false));
     TRY(dev_alloc(h, &h->k2.nxt, n, false));
     TRY(dev_alloc(h, &h->k2.eff, n + 8, false));
@@ -252,32 +33,6 @@ static int k2_scratch_alloc(agr_handle* h, size_t n) {
     return 0;
 }
 
-// ---- logical rows (arrival numbers, what the API speaks) vs physical rows (where the record lives; see agr_dev)
-static inline bool is_ring(const agr_handle* h) { return (h->cfg.flags & AGR_CFG_RING) != 0; }
-static inline uint64_t phys_row(const agr_handle* h, uint64_t l) { return is_ring(h) ? l % h->cfg.slab_rows : l; }
-static inline uint64_t rows_span(const agr_handle* h) {       // physical rows that have ever been handed out
-    return is_ring(h) ? std::min<uint64_t>(h->rows_used, h->cfg.slab_rows) : h->rows_used;
-}
-static inline void sync_svc_rows(agr_handle* h);
-static inline void sync_window(agr_handle* h) {               // the live window the kernels check decoded ids against
-    h->d.tail = h->tail; h->d.head_l = h->rows_used;
-    h->d.ring_rows = is_ring(h) ? (uint32_t)h->cfg.slab_rows : 0u;
-    h->d.tail_phys = is_ring(h) ? (uint32_t)(h->tail % h->cfg.slab_rows) : 0u;
-    sync_svc_rows(h);
-}
-
-struct nccl_api {
-    void* lib = nullptr;
-    ncclResult_t (*GetUniqueId)(ncclUniqueId*) = nullptr;
-    ncclResult_t (*CommInitRank)(ncclComm_t*, int, ncclUniqueId, int) = nullptr;
-    ncclResult_t (*CommDestroy)(ncclComm_t) = nullptr;
-    ncclResult_t (*Send)(const void*, size_t, ncclDataType_t, int, ncclComm_t, cudaStream_t) = nullptr;
-    ncclResult_t (*Recv)(void*, size_t, ncclDataType_t, int, ncclComm_t, cudaStream_t) = nullptr;
-    ncclResult_t (*GroupStart)() = nullptr;
-    ncclResult_t (*GroupEnd)() = nullptr;
-    const char* (*GetErrorString)(ncclResult_t) = nullptr;
-};
-static nccl_api g_nccl;
 // pageable -> pinned staging copy.  One core moves ~13 GB/s, a quarter of what the link takes; big pieces are split over a
 // few short-lived threads (the pinned path, agr_host_alloc, needs none of this).
 static void par_memcpy(void* dst, const void* src, size_t bytes) {
@@ -294,7 +49,7 @@ static void par_memcpy(void* dst, const void* src, size_t bytes) {
     memcpy(dst, src, std::min(slice, bytes));
     for (auto& x : th) x.join();
 }
-static bool is_pinned(const void* p) {
+bool is_pinned(const void* p) {
     cudaPointerAttributes attr;
     if (cudaPointerGetAttributes(&attr, p) == cudaSuccess) return attr.type == cudaMemoryTypeHost;
     cudaGetLastError();
@@ -306,9 +61,16 @@ static int h2d_staged(agr_handle* h, void* dst, const void* src, size_t bytes, v
     CK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, h->stream));
     return 0;
 }
+// device -> host on the compute stream through the pinned stage, then into dst (NULL: the bytes stay in the stage)
+int d2h_staged(agr_handle* h, void* dst, const void* dsrc, size_t bytes, void* stage) {
+    CK(cudaMemcpyAsync(stage, dsrc, bytes, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    if (dst) memcpy(dst, stage, bytes);
+    return 0;
+}
 // caller records -> slab rows on the copy stream: pinned (or registered) memory is DMA'd in place, pageable memory goes
 // through the two pinned bounce buffers; bk is the bounce buffer to use next, carried from one call to the next
-static int upload_rows(agr_handle* h, uint8_t* dst, const uint8_t* src, size_t bytes, bool src_pinned, int& bk) {
+int upload_rows(agr_handle* h, uint8_t* dst, const uint8_t* src, size_t bytes, bool src_pinned, int& bk) {
     if (src_pinned) {
         CK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, h->copy_stream));
         return 0;
@@ -324,7 +86,7 @@ static int upload_rows(agr_handle* h, uint8_t* dst, const uint8_t* src, size_t b
     return 0;
 }
 // the lengths of the completed and failed logs
-static int read_log_lens(agr_handle* h, unsigned long long lens[2]) {
+int read_log_lens(agr_handle* h, unsigned long long lens[2]) {
     CK(cudaMemcpyAsync(lens, h->d.log_len, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
     return 0;
@@ -336,6 +98,16 @@ static int read_count(agr_handle* h, unsigned long long* v) {
     CK(cudaStreamSynchronize(h->stream));
     return 0;
 }
+// grows an event pool to k events (without timing); the ones it has are kept
+int grow_events(std::vector<cudaEvent_t>& ev, size_t k) {
+    while (ev.size() < k) { cudaEvent_t e; CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming)); ev.push_back(e); }
+    return 0;
+}
+// every chunk's time bounds "unknown" (after a restore, or a jump of the arrival counter): the next agr_expire recomputes them
+int chunk_bounds_unknown(agr_handle* h) {
+    CK(cudaMemsetAsync(h->d.cmin, 0, (size_t)(h->cfg.slab_rows / AGR_CHUNK_ROWS + 2) * 8, h->stream));
+    return 0;
+}
 
 static uint64_t next_pow2(uint64_t v) { uint64_t p = 1; while (p < v) p <<= 1; return p; }
 
@@ -345,355 +117,7 @@ static void pack_agent_id(const char* id, unsigned long long w[4]) {
     strncpy(buf, id, AGR_AGENT_ID_BYTES - 1);
     memcpy(w, buf, 32);
 }
-
-
-// ------------------------------------------------------------------------------------------ single-request front end
-// Host side of agr_svc.h.  Lock-free for the callers: one fetch_add claims ring slots, the payload is written into pinned
-// device-mapped memory, a release store publishes it, and the caller waits on a word the GPU writes.  One dispatcher thread
-// per handle turns the published prefix of the ring into batch descriptors; the resident service kernel (k_svc) does the rest.
-extern "C" { static int reserve_rows_locked(agr_handle* h, uint32_t n, uint64_t* first); }
-extern "C" { static int resp_reserve_locked(agr_handle* h, uint64_t need, uint64_t len, unsigned long long* off); }
-cudaError_t agr_launch_svc(const agr_dev& d, const svc_dev& v, const agr_k2_scratch& k2, unsigned long long next_seq, cudaStream_t st);
-unsigned long long agr_svc_desc_check(const svc_desc* dsc);
-
-struct svc_host {
-    // ---- read-mostly (every caller reads these on every call; nothing here is written while callers run)
-    svc_desc* desc = nullptr; uint8_t* payload = nullptr; svc_res* res = nullptr; svc_ctl* ctl = nullptr;   // pinned, device-mapped
-    std::atomic<uint32_t>* ready = nullptr;             // [SVC_SLOTS] (lap + 1) << 2 | SVC_OP_* once the slot's payload is complete
-    uint32_t spin_cpus = 1;                             // how many waiters may spin (CPU allowance minus dispatcher and driver threads)
-    std::atomic<bool> shutdown{false}, sleeping{false}; // (sleeping flips only when the ring has been empty for 2 ms)
-    std::atomic<int> fatal{0};                          // a CUDA error in the dispatcher: every later call fails with it
-    // ---- the words the callers / the dispatcher keep writing: a cache line each
-    alignas(64) std::atomic<uint64_t> head{0};          // next ring slot to hand out (absolute number)
-    alignas(64) std::atomic<uint32_t> waiters{0};       // callers blocked in svc_wait right now
-    alignas(64) std::atomic<uint64_t> scanned{0};       // dispatcher: first slot whose ready word it has not consumed yet (>= taken)
-    std::atomic<uint64_t> rows_out{0};                  // = the handle's rows_used (sync_window): callers rebuild a row's high bits from it (svc_try)
-    // ---- the dispatcher's own
-    alignas(64) uint64_t taken = 0;                     // first slot not yet put into a batch
-    uint64_t seq = 0;                                   // last batch number published
-    bool running = false;                               // service kernel resident (changed under the handle mutex only)
-    std::chrono::steady_clock::time_point started;      // when it was launched
-    agr_k2_scratch k2{};                                // K2 scratch of the service kernel (SVC_MAX_OPS ops)
-    uint32_t* d_dupfix = nullptr;
-    unsigned long long *d_boff = nullptr, *d_bdst = nullptr; uint32_t* d_bhlen = nullptr;   // per-outcome byte places (svc_dev)
-    std::atomic<uint64_t> batches{0}, ops{0};
-    // diagnostics (AGR_SVC_DEBUG=1 prints them when the handle is destroyed)
-    uint64_t starts = 0, stops = 0, sleeps = 0, flow_waits = 0;
-    double cyc[4] = {0, 0, 0, 0}; uint64_t polls = 0;
-    std::thread thr;
-    alignas(64) std::mutex smu; std::condition_variable scv;   // the dispatcher sleeps here when the ring has been empty for a while
-};
-
-// (called under the handle mutex by every change of rows_used: reserve_rows_locked stores the new value before the dispatcher
-// publishes the batch whose answers name the rows)
-static inline void sync_svc_rows(agr_handle* h) {
-    if (h->svc) h->svc->rows_out.store(h->rows_used, std::memory_order_release);
-}
-
-static void svc_fail_ops(svc_host* s, uint64_t from, uint64_t to, int rc, bool records_only, const uint32_t* conts);
-// stops the resident kernel; the caller holds h->mu, so no new batch can be published meanwhile
-static int svc_stop_locked(agr_handle* h) {
-    svc_host* s = h->svc;
-    if (!s || !s->running) return 0;
-    s->ctl->stop = 1;
-    std::atomic_thread_fence(std::memory_order_seq_cst);
-    cudaError_t e = cudaStreamSynchronize(h->stream);
-    s->ctl->stop = 0;
-    s->running = false;
-    s->stops++;
-    s->cyc[0] += (double)s->ctl->cyc_wait; s->cyc[1] += (double)s->ctl->cyc_load; s->cyc[2] += (double)s->ctl->cyc_work; s->cyc[3] += (double)s->ctl->cyc_publish;
-    s->polls += s->ctl->heartbeat;
-    if (e != cudaSuccess) { s->fatal = AGR_ECUDA; return fail(AGR_ECUDA, std::string("service kernel: ") + cudaGetErrorString(e)); }
-    if (s->ctl->done_seq != s->seq) {
-        // (cannot happen while the dispatcher runs: it stops the kernel after 2 ms without traffic, the kernel's own idle exit is 2 s)
-        // whoever waits for an operation of those batches gets an error instead of waiting for ever
-        for (uint64_t q = s->ctl->done_seq + 1; q <= s->seq; ++q) {
-            const svc_desc* dsc = s->desc + (q % SVC_DESCS);
-            if (dsc->seq == q) svc_fail_ops(s, dsc->from, dsc->from + dsc->count, AGR_ECUDA, false, dsc->cont);
-        }
-        s->fatal = AGR_ECUDA;
-        return fail(AGR_ECUDA, "service kernel left with batches unprocessed");
-    }
-    return 0;
-}
-static int svc_start_locked(agr_handle* h) {
-    svc_host* s = h->svc;
-    if (s->running) return 0;
-    svc_dev v{};
-    v.desc = s->desc; v.payload = s->payload; v.res = s->res; v.ctl = s->ctl; v.dupfix = s->d_dupfix;
-    v.resp = h->d_resp; v.resp_off = h->d_resp_off; v.resp_len = h->d_resp_len; v.resp_hlen = h->d_resp_hlen;
-    v.err_off = h->d_err_off; v.err_len = h->d_err_len; v.b_off = s->d_boff; v.b_dst = s->d_bdst; v.b_hlen = s->d_bhlen;
-    v.idle_ns = 2000000000ULL;                                   // safety only: the dispatcher stops the kernel long before
-    s->ctl->state = 1; s->ctl->stop = 0;
-    std::atomic_thread_fence(std::memory_order_seq_cst);
-    sync_window(h);
-    // resume at the first batch the previous incarnation did not run (normally none is pending; a batch published right
-    // before this launch is)
-    cudaError_t e = agr_launch_svc(h->d, v, s->k2, s->ctl->done_seq + 1, h->stream);
-    if (e != cudaSuccess) { s->fatal = AGR_ECUDA; return fail(AGR_ECUDA, std::string("service kernel launch: ") + cudaGetErrorString(e)); }
-    s->running = true;
-    s->starts++;
-    s->ctl->cyc_wait = 0; s->ctl->cyc_load = 0; s->ctl->cyc_work = 0; s->ctl->cyc_publish = 0; s->ctl->heartbeat = 0;
-    s->started = std::chrono::steady_clock::now();
-    return 0;
-}
-
-// the handle lock every entry point other than the single-request path takes: the resident kernel owns the handle's stream
-// while it runs, so it is stopped first (it finishes the batches already published) and started again by the dispatcher
-struct HLock {
-    agr_handle* h;
-    explicit HLock(agr_handle* h_) : h(h_) {
-        h->mu.lock();
-        if (h->svc && h->svc->running) { cudaSetDevice(h->device); svc_stop_locked(h); }
-    }
-    ~HLock() { h->mu.unlock(); }
-    HLock(const HLock&) = delete; HLock& operator=(const HLock&) = delete;
-};
-
-// answers every op of [from, to) from the host side (slab full, CUDA error): the callers see rc.  conts: the batch's
-// continuation bits (relative to from), answered as already collected (nobody waits for them)
-static void svc_fail_ops(svc_host* s, uint64_t from, uint64_t to, int rc, bool records_only, const uint32_t* conts) {
-    for (uint64_t a = from; a < to; ++a) {
-        const uint32_t slot = (uint32_t)(a & (SVC_SLOTS - 1u));
-        const uint32_t rw = s->ready[slot].load(std::memory_order_relaxed), kd = rw & 3u;
-        const bool rec = kd == SVC_OP_RECORD, cont = (conts[(a - from) >> 5] >> ((a - from) & 31u)) & 1u;
-        // (a skipped slot has no waiter and keeps its old answer; it may even have been published again for the NEXT lap already)
-        if ((rw >> 2) != (uint32_t)(a / SVC_SLOTS) + 1u || kd == SVC_OP_SKIP || (records_only && !rec)) continue;
-        svc_res* r = s->res + slot;
-        r->w[0] = rec ? 0u : cont ? 0u : (uint32_t)rc; r->w[1] = rec ? (uint32_t)rc : 0u; r->w[2] = 0;
-        std::atomic_thread_fence(std::memory_order_release);
-        r->w[3] = (svc_tag(a) | (cont ? SVC_COLLECTED : 0u)) << 16;
-    }
-}
-
-static void svc_dispatcher(agr_handle* h) {
-    svc_host* s = h->svc;
-    cudaSetDevice(h->device);
-    auto last_work = std::chrono::steady_clock::now();
-    uint32_t spins = 0;
-    // the contiguous published prefix [taken, to), grown INCREMENTALLY: a slot is looked at until it is published and never again
-    // (re-reading the callers' ready words every iteration keeps pulling their cache lines away from the cores that write them)
-    uint64_t to = s->taken;
-    uint32_t nstaged = 0;                                        // records + outcomes with bytes: one 512 B stage slot of k_svc each
-    uint32_t kinds[SVC_MAX_OPS / 16] = {0}, conts[SVC_MAX_OPS / 32] = {0};
-    while (!s->shutdown.load(std::memory_order_acquire)) {
-        svc_scan(s, s->taken, &to, &nstaged, kinds, 128u, conts); // (csrc/agr_ring.hpp: shared with the CPU simulation of the ring)
-        const auto now = std::chrono::steady_clock::now();
-        if (to == s->taken) {
-            const auto idle = std::chrono::duration_cast<std::chrono::microseconds>(now - last_work).count();
-            if (idle > 2000) {
-                // nothing for 2 ms: give the GPU (and this core) back; the next caller wakes us up
-                { std::lock_guard<std::mutex> hl(h->mu); if (s->running) svc_stop_locked(h); }
-                std::unique_lock<std::mutex> lk(s->smu);
-                s->sleeping.store(true, std::memory_order_seq_cst);
-                s->sleeps++;
-                const uint32_t slot = (uint32_t)(s->taken & (SVC_SLOTS - 1u));
-                if ((s->ready[slot].load(std::memory_order_seq_cst) >> 2) != (uint32_t)(s->taken / SVC_SLOTS) + 1u && !s->shutdown.load())
-                    s->scv.wait_for(lk, std::chrono::milliseconds(50));
-                s->sleeping.store(false, std::memory_order_seq_cst);
-                last_work = std::chrono::steady_clock::now();
-            } else {
-                cpu_relax(spins);
-            }
-            continue;
-        }
-        last_work = now;
-        // Batching window = the kernel's own pace: at most two batches are outstanding (one being decided, one being pulled by
-        // the kernel's loader warps); while both are, keep collecting — whatever arrives meanwhile joins the next batch instead
-        // of queueing behind a train of one-request batches.
-        if (s->running && s->seq - s->ctl->done_seq >= 2 && to - s->taken < SVC_MAX_OPS) {
-            s->flow_waits++;
-            for (int k = 0; k < 8; ++k) _mm_pause();
-            continue;
-        }
-        spins = 0;
-        std::lock_guard<std::mutex> hl(h->mu);
-        if (s->fatal.load()) {
-            svc_fail_ops(s, s->taken, to, s->fatal.load(), false, conts);
-            s->taken = to; nstaged = 0; memset(kinds, 0, sizeof kinds); memset(conts, 0, sizeof conts);
-            continue;
-        }
-        if (s->running && s->ctl->state != 1u) {                // it left on its own (safety timeout): note it and start another
-            cudaStreamSynchronize(h->stream);
-            s->running = false;
-        }
-        // a resident kernel blocks device-wide synchronisations of other threads (cudaFree ...): let it go every 20 ms
-        if (s->running && std::chrono::duration_cast<std::chrono::milliseconds>(now - s->started).count() > 20) svc_stop_locked(h);
-        // records, and the outcomes with bytes with their segments' region (16 B-rounded, in ring order; a span's length is
-        // clamped to the slots the batch holds of it, as the kernel does)
-        const uint32_t count = (uint32_t)(to - s->taken);
-        uint32_t nrec = 0, nbytes = 0, ncont = 0;
-        uint64_t byte_total = 0;
-        for (uint32_t k = 0; k < count; ++k) {
-            const uint32_t kd = (kinds[k >> 4] >> ((k & 15u) * 2u)) & 3u;
-            if (kd == SVC_OP_RECORD) nrec++;
-            if ((conts[k >> 5] >> (k & 31u)) & 1u) { ncont++; continue; }
-            if (kd == SVC_OP_OUTCOME_BYTES) {                    // (the slot's payload is visible: its ready word was acquired)
-                uint32_t len;
-                memcpy(&len, s->payload + (size_t)((s->taken + k) & (SVC_SLOTS - 1u)) * SVC_PAYLOAD + SVC_BYTES_HDR + 4, 4);
-                byte_total += (svc_span_len(len, svc_conts_after(conts, k, count)) + 15u) & ~15u;
-                nbytes++;
-            }
-        }
-        uint64_t first = 0;
-        bool have_rows = true;
-        if (nrec) {
-            if (reserve_rows_locked(h, nrec, &first) < 0) { svc_fail_ops(s, s->taken, to, AGR_ENOSPC, true, conts); have_rows = false; }
-        }
-        svc_desc dsc{};
-        for (uint32_t k = 0; k < (uint32_t)(to - s->taken); ++k) {
-            uint32_t kd = (kinds[k >> 4] >> ((k & 15u) * 2u)) & 3u;
-            if (kd == SVC_OP_RECORD && !have_rows) kd = SVC_OP_SKIP;
-            dsc.kinds[k >> 4] |= kd << ((k & 15u) * 2u);
-        }
-        memcpy(dsc.cont, conts, sizeof conts);
-        dsc.resp_base = SVC_NO_BYTES;
-        if (nbytes) {
-            unsigned long long off;
-            if (resp_reserve_locked(h, byte_total, byte_total, &off) == 0) dsc.resp_base = off;
-        }
-        dsc.from = s->taken; dsc.count = count; dsc.n_records = have_rows ? nrec : 0u;
-        dsc.first_l = first; dsc.first_p = (uint32_t)phys_row(h, first);
-        dsc.tail = h->tail; dsc.head_l = h->rows_used; dsc.tail_phys = is_ring(h) ? (uint32_t)(h->tail % h->cfg.slab_rows) : 0u;
-        dsc.idx_base = h->d.idx_base;
-        dsc.seq = s->seq + 1;
-        dsc.check = agr_svc_desc_check(&dsc);
-        svc_desc* slot = s->desc + (dsc.seq % SVC_DESCS);
-        // the batch number goes last; the kernel also verifies the check word, so a torn read is never accepted
-        const uint64_t* src = reinterpret_cast<const uint64_t*>(&dsc);
-        volatile uint64_t* dst = reinterpret_cast<volatile uint64_t*>(slot);
-        for (int i = 0; i < 31; ++i) dst[i] = src[i];
-        std::atomic_thread_fence(std::memory_order_release);
-        dst[31] = src[31];
-        std::atomic_thread_fence(std::memory_order_seq_cst);
-        s->seq = dsc.seq;
-        s->taken = to;
-        s->batches.fetch_add(1, std::memory_order_relaxed);
-        s->ops.fetch_add(dsc.count - ncont, std::memory_order_relaxed);     // operations: a span counts once
-        h->k1_launches += nrec ? 1 : 0;                         // accounting: batches with records / with outcomes served by k_svc
-        h->k2_launches += (dsc.count > nrec) ? 1 : 0;
-        nstaged = 0; memset(kinds, 0, sizeof kinds); memset(conts, 0, sizeof conts);
-        if (!s->running && svc_start_locked(h) < 0) {
-            // could not launch: nothing will ever process this batch — fail it from here
-            svc_fail_ops(s, dsc.from, to, AGR_ECUDA, false, dsc.cont);
-        }
-    }
-    std::lock_guard<std::mutex> hl(h->mu);
-    cudaSetDevice(h->device);
-    svc_stop_locked(h);
-}
-
-// CPUs this process may keep busy: the cgroup CPU quota if there is one, else the online CPUs
-static uint32_t cpu_allowance() {
-    uint32_t n = std::max(1u, std::thread::hardware_concurrency());
-    if (FILE* f = fopen("/sys/fs/cgroup/cpu.max", "r")) {
-        char a[64]; unsigned long long period = 0;
-        if (fscanf(f, "%63s %llu", a, &period) == 2 && strcmp(a, "max") != 0 && period) {
-            const unsigned long long q = strtoull(a, nullptr, 10);
-            if (q) n = std::min<uint32_t>(n, (uint32_t)std::max<unsigned long long>(1, q / period));
-        }
-        fclose(f);
-    }
-    return n;
-}
-
-static int svc_create(agr_handle* h) {
-    svc_host* s = new svc_host();
-    h->svc = s;
-    auto pin = [&](void** p, size_t bytes) -> int {
-        cudaError_t e = cudaHostAlloc(p, bytes, cudaHostAllocMapped | cudaHostAllocPortable);
-        if (e != cudaSuccess) return fail(AGR_ENOMEM, std::string("cudaHostAlloc (request ring): ") + cudaGetErrorString(e));
-        memset(*p, 0, bytes);
-        h->host_allocs.push_back(*p);
-        return 0;
-    };
-    TRY(pin((void**)&s->desc, sizeof(svc_desc) * SVC_DESCS));
-    TRY(pin((void**)&s->payload, (size_t)SVC_SLOTS * SVC_PAYLOAD));
-    TRY(pin((void**)&s->res, sizeof(svc_res) * SVC_SLOTS));
-    TRY(pin((void**)&s->ctl, sizeof(svc_ctl)));
-    s->ready = new std::atomic<uint32_t>[SVC_SLOTS];
-    for (uint32_t i = 0; i < SVC_SLOTS; ++i) s->ready[i].store(0);
-    TRY(dev_alloc(h, &s->k2.ops, (size_t)SVC_MAX_OPS, false));
-    TRY(dev_alloc(h, &s->k2.nxt, (size_t)SVC_MAX_OPS, false));
-    TRY(dev_alloc(h, &s->k2.eff, (size_t)SVC_MAX_OPS + 8, false));
-    TRY(dev_alloc(h, &s->k2.results, (size_t)SVC_MAX_OPS, false));
-    TRY(dev_alloc(h, &s->d_dupfix, (size_t)4, true));
-    TRY(dev_alloc(h, &s->d_boff, (size_t)SVC_MAX_OPS + 1, false));
-    TRY(dev_alloc(h, &s->d_bdst, (size_t)SVC_MAX_OPS, false));
-    TRY(dev_alloc(h, &s->d_bhlen, (size_t)SVC_MAX_OPS, false));
-    CK(cudaStreamSynchronize(h->stream));
-    const uint32_t cpus = cpu_allowance();
-    s->spin_cpus = cpus > 6 ? cpus - 6 : 1;             // leave room for the dispatcher, the driver's threads and the nappers' wake-ups
-    s->thr = std::thread(svc_dispatcher, h);
-    return 0;
-}
-static void svc_destroy(agr_handle* h) {
-    svc_host* s = h->svc;
-    if (!s) return;
-    if (s->thr.joinable()) {
-        s->shutdown.store(true, std::memory_order_release);
-        { std::lock_guard<std::mutex> lk(s->smu); s->scv.notify_all(); }
-        s->thr.join();
-    }
-    if (getenv("AGR_SVC_DEBUG")) {
-        const double mhz = 1965.0, tot = s->cyc[0] + s->cyc[1] + s->cyc[2] + s->cyc[3];
-        const double nb = (double)std::max<uint64_t>(1, s->batches.load());
-        fprintf(stderr, "[agr svc] batches %llu ops %llu (%.1f/batch) | kernel starts %llu stops %llu, dispatcher sleeps %llu, flow waits %llu | "
-                        "per batch: wait %.2f us, load %.2f us, work %.2f us, publish %.2f us (kernel alive %.1f ms), polls %llu\n",
-                (unsigned long long)s->batches.load(), (unsigned long long)s->ops.load(), (double)s->ops.load() / nb,
-                (unsigned long long)s->starts, (unsigned long long)s->stops, (unsigned long long)s->sleeps, (unsigned long long)s->flow_waits,
-                s->cyc[0] / mhz / nb, s->cyc[1] / mhz / nb, s->cyc[2] / mhz / nb, s->cyc[3] / mhz / nb, tot / mhz / 1000.0, (unsigned long long)s->polls);
-    }
-    delete[] s->ready;
-    h->svc = nullptr;
-    delete s;
-}
-
-// (the callers' side of the ring — svc_submit_one, svc_try, svc_wait, svc_release — is csrc/agr_ring.hpp: the same code runs against a
-// stand-in for the dispatcher and the GPU in tests/ring_sim.cpp, on the CPU)
-// Request.ID of the record in ring slot a: minted from its row, or the caller's own (still in the slot's payload)
-static inline void svc_request_id(agr_handle* h, uint64_t a, uint64_t rid, uint8_t id[16]) {
-    if (h->cfg.flags & AGR_CFG_MINT_IDS) {
-        unsigned long long lo, hi;
-        agr_mint_id(rid, h->d.shard_id, h->d.id_gen, h->d.id_secret, lo, hi);
-        memcpy(id, &lo, 8); memcpy(id + 8, &hi, 8);
-    } else memcpy(id, h->svc->payload + (size_t)(a & (SVC_SLOTS - 1u)) * SVC_PAYLOAD, 16);
-}
-
-static int svc_ingest(agr_handle* h, const agr_record* recs, uint32_t n, agr_verdict* out, uint8_t (*ids)[16], uint64_t* first_rid) {
-    svc_host* s = h->svc;
-    uint64_t pos[SVC_MAX_CALL];
-    for (uint32_t i = 0; i < n; ++i) while (!svc_submit_one(s, SVC_OP_RECORD, &recs[i], sizeof(agr_record), &pos[i])) {}   // in call order
-    int rc = 0;
-    for (uint32_t i = 0; i < n; ++i) {
-        svc_answer r; svc_wait(s, pos[i], &r);
-        if ((r.w0 & 0xffu) == 0u) rc = (int)r.w1;
-        else {
-            if (out) { memcpy(&out[i], &r.w0, 4); memcpy((uint8_t*)&out[i] + 4, &r.w1, 4); }
-            const uint64_t row = svc_row(s, r);
-            if (ids) svc_request_id(h, pos[i], row, ids[i]);
-            if (i == 0 && first_rid) *first_rid = row;
-        }
-        svc_release(s, pos[i]);
-    }
-    if (rc < 0) return fail(rc, rc == AGR_ENOSPC ? "slab full" : "single-request front end: CUDA error");
-    return 0;
-}
-static int svc_complete(agr_handle* h, const agr_outcome* outs, uint32_t n, int32_t* results) {
-    svc_host* s = h->svc;
-    uint64_t pos[SVC_MAX_CALL];
-    for (uint32_t i = 0; i < n; ++i) while (!svc_submit_one(s, SVC_OP_OUTCOME, &outs[i], sizeof(agr_outcome), &pos[i])) {}
-    int rc = 0;
-    for (uint32_t i = 0; i < n; ++i) {
-        svc_answer r; svc_wait(s, pos[i], &r);
-        const int32_t res = (int32_t)r.w0;
-        if (res < 0 && res != AGR_ENOTFOUND) rc = res;
-        if (results) results[i] = res;
-        svc_release(s, pos[i]);
-    }
-    if (rc < 0) return fail(rc, "single-request front end: CUDA error");
-    return 0;
-}
+}  // namespace agr_impl
 
 extern "C" {
 
@@ -720,8 +144,6 @@ void* agr_host_alloc(size_t bytes) {
     return p;
 }
 void agr_host_free(void* p) { if (p) cudaFreeHost(p); }
-
-static int snap_online_create(agr_handle* h);
 
 static int create_impl(const agr_config* cfg_in, agr_handle* h) {
     agr_config c{};
@@ -883,11 +305,13 @@ void agr_destroy(agr_handle* h) {
     if (h->copy_stream) cudaStreamDestroy(h->copy_stream);
     if (h->d2h_stream) cudaStreamDestroy(h->d2h_stream);
     for (auto e : h->out_ev) cudaEventDestroy(e);
-    if (h->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(h->comm);
+    comm_destroy(h);
     if (h->stream) cudaStreamDestroy(h->stream);
     delete h;
 }
 
+}  // extern "C"
+namespace agr_impl __attribute__((visibility("hidden"))) {
 // ------------------------------------------------------------------------------------------ agent table
 static int agent_find(agr_handle* h, const char* id) {
     auto it = h->slot_of.find(std::string(id));
@@ -896,7 +320,7 @@ static int agent_find(agr_handle* h, const char* id) {
 
 // status lives in two places on the device: astatus[slot] (K3 reads it by slot) and the key entry (K1 reads it with
 // the key in one access); both copies are stream-ordered before the next kernel
-static int push_agent_status(agr_handle* h, uint32_t slot, uint8_t status) {
+int push_agent_status(agr_handle* h, uint32_t slot, uint8_t status) {
     const uint32_t idx = h->akey_index[slot];
     h->akeys_host[idx].status = status;
     CK(cudaMemcpyAsync(h->d.astatus + slot, &status, 1, cudaMemcpyHostToDevice, h->stream));
@@ -905,7 +329,7 @@ static int push_agent_status(agr_handle* h, uint32_t slot, uint8_t status) {
 }
 
 // core of agr_set_agent_state; `upload` = push the change to the device now (the bulk call uploads the tables once instead)
-static int set_agent_state_locked(agr_handle* h, const char* agent_id, uint8_t status, bool upload) {
+int set_agent_state_locked(agr_handle* h, const char* agent_id, uint8_t status, bool upload) {
     size_t len = strnlen(agent_id, AGR_AGENT_ID_BYTES);
     if (len == 0 || len >= AGR_AGENT_ID_BYTES) return fail(AGR_EINVAL, "agent id must be 1..31 bytes");
     if (status > AGR_AGENT_FAILED) return fail(AGR_EINVAL, "bad agent status");
@@ -937,6 +361,8 @@ static int set_agent_state_locked(agr_handle* h, const char* agent_id, uint8_t s
     }
     return slot;
 }
+}  // namespace agr_impl
+extern "C" {
 int agr_set_agent_state(agr_handle* h, const char* agent_id, uint8_t status) {
     if (!h || !agent_id) return fail(AGR_EINVAL, "NULL argument");
     HLock lk(h);
@@ -989,15 +415,17 @@ int agr_drop_agent(agr_handle* h, const char* agent_id) {
     return 0;
 }
 
+}  // extern "C"
+namespace agr_impl __attribute__((visibility("hidden"))) {
 // Rows handed out by agr_reserve_rows hold no record until agr_ingest_rows has run over them.  The replay scan, the pending
 // views and agr_reclaim stop at the first such row: otherwise a scan that finds "nothing pending" above its low-water mark
 // would move the mark past rows that K1 fills in later, and those requests would never be replayed.
-static uint64_t ingested_bound(const agr_handle* h) {
+uint64_t ingested_bound(const agr_handle* h) {
     uint64_t b = h->rows_used;
     for (const auto& r : h->resv) b = std::min(b, r.first);
     return b;
 }
-static void resv_remove(agr_handle* h, uint64_t first, uint64_t end) {
+void resv_remove(agr_handle* h, uint64_t first, uint64_t end) {
     std::vector<std::pair<uint64_t, uint64_t>> keep;
     for (const auto& r : h->resv) {
         if (r.second <= first || r.first >= end) { keep.push_back(r); continue; }
@@ -1024,7 +452,7 @@ static inline bool ring_fits_pinned(const agr_handle* h, uint64_t used, uint64_t
 }
 
 // ------------------------------------------------------------------------------------------ K1
-static int reserve_rows_locked(agr_handle* h, uint32_t n, uint64_t* first) {
+int reserve_rows_locked(agr_handle* h, uint32_t n, uint64_t* first) {
     if (!is_ring(h)) {
         if (h->rows_used + n > h->cfg.slab_rows) return fail(AGR_ENOSPC, "slab full");
         *first = h->rows_used;
@@ -1062,20 +490,20 @@ static int claim_k1_events(agr_handle* h, cudaEvent_t* e0, cudaEvent_t* e1) {
     return 0;
 }
 // AGR_CFG_TIMING: events around the last launch group g (0 = K2, 1 = K3 select, 2 = K5 encode, 3 = snapshot cut) that agr_op_time reads
-static int op_time_begin(agr_handle* h, int g) {
+int op_time_begin(agr_handle* h, int g) {
     if (!(h->cfg.flags & AGR_CFG_TIMING)) return 0;
     for (auto& e : h->op_ev) if (!e) CK(cudaEventCreate(&e));
     CK(cudaEventRecord(h->op_ev[2 * g], h->stream));
     return 0;
 }
-static int op_time_end(agr_handle* h, int g) {
+int op_time_end(agr_handle* h, int g) {
     if (!(h->cfg.flags & AGR_CFG_TIMING)) return 0;
     CK(cudaEventRecord(h->op_ev[2 * g + 1], h->stream));
     h->op_timed[g] = true;
     return 0;
 }
 
-static int launch_k1_locked(agr_handle* h, uint64_t first, uint32_t n, agr_verdict* d_out, uint8_t* d_ids = nullptr) {
+int launch_k1_locked(agr_handle* h, uint64_t first, uint32_t n, agr_verdict* d_out, uint8_t* d_ids) {
     sync_window(h);
     flip_batch_words(h);
     cudaEvent_t e0 = nullptr, e1 = nullptr;
@@ -1088,6 +516,8 @@ static int launch_k1_locked(agr_handle* h, uint64_t first, uint32_t n, agr_verdi
     CK(cudaGetLastError());
     return 0;
 }
+}  // namespace agr_impl
+extern "C" {
 
 static int ingest_rows_locked(agr_handle* h, uint64_t first, uint32_t n, agr_verdict* out, bool sync) {
     if (first + n > h->rows_used) return fail(AGR_EINVAL, "rows not reserved");
@@ -1096,9 +526,7 @@ static int ingest_rows_locked(agr_handle* h, uint64_t first, uint32_t n, agr_ver
     TRY(launch_k1_locked(h, first, n, out ? h->d_verdicts : nullptr));
     if (!h->resv.empty()) resv_remove(h, first, first + n);
     if (out) {
-        CK(cudaMemcpyAsync(h->h_verdicts, h->d_verdicts, (size_t)n * sizeof(agr_verdict), cudaMemcpyDeviceToHost, h->stream));
-        CK(cudaStreamSynchronize(h->stream));
-        memcpy(out, h->h_verdicts, (size_t)n * sizeof(agr_verdict));
+        TRY(d2h_staged(h, out, h->d_verdicts, (size_t)n * sizeof(agr_verdict), h->h_verdicts));
     } else if (sync) {
         CK(cudaStreamSynchronize(h->stream));
     }
@@ -1192,10 +620,7 @@ static int ingest_ex_locked(agr_handle* h, const agr_record* recs, uint32_t n, a
     const bool out_pinned = out && is_pinned(out);
     const bool ids_pinned = ids && is_pinned(ids);
     const uint32_t nchunks = (n + AGR_INGEST_CHUNK - 1) / AGR_INGEST_CHUNK;
-    while (h->chunk_ev.size() < nchunks + 1) {
-        cudaEvent_t e; CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-        h->chunk_ev.push_back(e);
-    }
+    TRY(grow_events(h->chunk_ev, nchunks + 1));
     // the copy stream must not overwrite rows before earlier work on the compute stream is done with the slab
     CK(cudaEventRecord(h->chunk_ev[nchunks], h->stream));
     CK(cudaStreamWaitEvent(h->copy_stream, h->chunk_ev[nchunks], 0));
@@ -1208,7 +633,7 @@ static int ingest_ex_locked(agr_handle* h, const agr_record* recs, uint32_t n, a
         TRY(launch_k1_locked(h, first + off, cn, out ? h->d_verdicts + off : nullptr, ids ? h->d_ids + (size_t)off * 16 : nullptr));
         if (out || ids) {
             // the chunk's read-backs (8 + 16 B per record) leave on their own stream as soon as its K1 is done
-            while (h->out_ev.size() <= c) { cudaEvent_t e; CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming)); h->out_ev.push_back(e); }
+            TRY(grow_events(h->out_ev, c + 1));
             CK(cudaEventRecord(h->out_ev[c], h->stream));
             CK(cudaStreamWaitEvent(h->d2h_stream, h->out_ev[c], 0));
             if (out) CK(cudaMemcpyAsync((out_pinned ? out : h->h_verdicts) + off, h->d_verdicts + off, (size_t)cn * sizeof(agr_verdict), cudaMemcpyDeviceToHost, h->d2h_stream));
@@ -1222,55 +647,11 @@ static int ingest_ex_locked(agr_handle* h, const agr_record* recs, uint32_t n, a
     return 0;
 }
 
-// ------------------------------------------------------------------------------------------ tickets (submit / collect)
-uint32_t agr_ring_capacity(void) { return SVC_SLOTS; }
-#define TICKET_OUTCOME (1ULL << 63)                               // a ticket = ring slot number | kind
-static int submit_one(agr_handle* h, uint32_t kind, const void* item, size_t bytes, agr_ticket* ticket) {
-    if (!h || !item || !ticket) return fail(AGR_EINVAL, "NULL argument");
-    svc_host* s = h->svc;
-    if (!s) return fail(AGR_EINVAL, "engine was not created with AGR_CFG_COMBINE");
-    uint64_t a = 0;
-    if (!svc_submit_one(s, kind, item, bytes, &a)) return AGR_EAGAIN;   // collect outstanding tickets (agr_poll) and come again
-    *ticket = a | (kind == SVC_OP_OUTCOME ? TICKET_OUTCOME : 0ULL);
-    return 0;
-}
-int agr_submit_ingest(agr_handle* h, const agr_record* rec, agr_ticket* ticket) { return submit_one(h, SVC_OP_RECORD, rec, sizeof(agr_record), ticket); }
-int agr_submit_complete(agr_handle* h, const agr_outcome* outcome, agr_ticket* ticket) { return submit_one(h, SVC_OP_OUTCOME, outcome, sizeof(agr_outcome), ticket); }
-static int collect(agr_handle* h, agr_ticket ticket, const svc_answer& r, agr_result* out) {
-    svc_host* s = h->svc;
-    const bool rec = !(ticket & TICKET_OUTCOME);
-    const uint64_t t = ticket & ~TICKET_OUTCOME;
-    if (out) {
-        memset(out, 0, sizeof *out);
-        out->is_outcome = rec ? 0u : 1u;
-        if (rec) {
-            if ((r.w0 & 0xffu) == 0u) out->result = (int32_t)r.w1;
-            else { memcpy(&out->verdict, &r.w0, 4); memcpy((uint8_t*)&out->verdict + 4, &r.w1, 4); out->rid = svc_row(s, r); svc_request_id(h, t, out->rid, out->request_id); }
-        } else out->result = (int32_t)r.w0;
-    }
-    svc_release(s, t);
-    return 0;
-}
-int agr_poll(agr_handle* h, agr_ticket ticket, agr_result* out) {
-    if (!h || !h->svc) return fail(AGR_EINVAL, "engine was not created with AGR_CFG_COMBINE");
-    svc_answer r;
-    if (!svc_try(h->svc, ticket & ~TICKET_OUTCOME, &r)) return AGR_EAGAIN;
-    return collect(h, ticket, r, out);
-}
-int agr_wait(agr_handle* h, agr_ticket ticket, agr_result* out) {
-    if (!h || !h->svc) return fail(AGR_EINVAL, "engine was not created with AGR_CFG_COMBINE");
-    svc_answer r;
-    svc_wait(h->svc, ticket & ~TICKET_OUTCOME, &r);
-    return collect(h, ticket, r, out);
-}
-
 // ------------------------------------------------------------------------------------------ K2
 static int complete_locked(agr_handle* h, const agr_outcome* outs, uint32_t n, int32_t* results, const agr_k2_bytes* bytes = nullptr,
                            bool bytes_dropped = false);
 static int complete_ex_locked(agr_handle* h, const agr_outcome* outs, uint32_t n, const uint8_t* bytes, const uint64_t* offsets,
                               const uint32_t* hdr_lens, int32_t* results);
-static int svc_complete_ex(agr_handle* h, const agr_outcome* outs, uint32_t n, const uint8_t* bytes, const uint64_t* offsets,
-                           const uint32_t* hdr_lens, int32_t* results);
 
 int agr_complete(agr_handle* h, const agr_outcome* outs, uint32_t n, int32_t* results) {
     if (!h || (n && !outs)) return fail(AGR_EINVAL, "NULL argument");
@@ -1309,9 +690,7 @@ static int complete_locked(agr_handle* h, const agr_outcome* outs, uint32_t n, i
     TRY(op_time_end(h, 0));
     CK(cudaMemcpyAsync(h->h_k2flag, h->k2.overflow, 4, cudaMemcpyDeviceToHost, h->stream));
     if (results) {
-        CK(cudaMemcpyAsync(h->h_results, h->k2.results, (size_t)n * 4, cudaMemcpyDeviceToHost, h->stream));
-        CK(cudaStreamSynchronize(h->stream));
-        memcpy(results, h->h_results, (size_t)n * 4);
+        TRY(d2h_staged(h, results, h->k2.results, (size_t)n * 4, h->h_results));
     } else {
         CK(cudaStreamSynchronize(h->stream));
     }
@@ -1325,10 +704,12 @@ static int complete_locked(agr_handle* h, const agr_outcome* outs, uint32_t n, i
     return 0;
 }
 
+}  // extern "C"
+namespace agr_impl __attribute__((visibility("hidden"))) {
 // ------------------------------------------------------------------------------------------ K2 with bytes (agr_complete_ex)
 // Places need bytes (a multiple of 16) in the response byte slab as one piece; len is the unrounded size the append-only check
 // uses.  With the ring a piece never wraps: the rest of the lap is skipped, and agr_reclaim moves resp_tail.
-static int resp_reserve_locked(agr_handle* h, uint64_t need, uint64_t len, unsigned long long* off) {
+int resp_reserve_locked(agr_handle* h, uint64_t need, uint64_t len, unsigned long long* off) {
     if (!is_ring(h)) {
         if (h->resp_used + len > h->resp_cap) return fail(AGR_ENOSPC, "response slab full");
         *off = h->resp_used;
@@ -1348,8 +729,8 @@ static int resp_reserve_locked(agr_handle* h, uint64_t need, uint64_t len, unsig
 
 // Checks what agr_complete_ex got; *total = the size of the batch's region (every segment rounded up to 16 B), *max_len = the
 // longest segment.
-static int check_segments(const agr_outcome* outs, uint32_t n, const uint64_t* offsets, const uint32_t* hdr_lens, uint64_t* total,
-                          uint64_t* max_len) {
+int check_segments(const agr_outcome* outs, uint32_t n, const uint64_t* offsets, const uint32_t* hdr_lens, uint64_t* total,
+                   uint64_t* max_len) {
     uint64_t t = 0, m = 0;
     for (uint32_t i = 0; i < n; ++i) {
         if (offsets[i + 1] < offsets[i]) return fail(AGR_EINVAL, "offsets must not decrease");
@@ -1366,6 +747,8 @@ static int check_segments(const agr_outcome* outs, uint32_t n, const uint64_t* o
     *total = t; *max_len = m;
     return 0;
 }
+}  // namespace agr_impl
+extern "C" {
 
 static int complete_ex_locked(agr_handle* h, const agr_outcome* outs, uint32_t n, const uint8_t* bytes, const uint64_t* offsets,
                               const uint32_t* hdr_lens, int32_t* results) {
@@ -1408,61 +791,6 @@ static int complete_ex_locked(agr_handle* h, const agr_outcome* outs, uint32_t n
     return complete_locked(h, outs, n, results, &b, false);
 }
 
-// agr_complete_ex through the single-request ring: every outcome goes as SVC_OP_OUTCOME_BYTES with its segment inline
-static int svc_complete_ex(agr_handle* h, const agr_outcome* outs, uint32_t n, const uint8_t* bytes, const uint64_t* offsets,
-                           const uint32_t* hdr_lens, int32_t* results) {
-    uint64_t total = 0, max_len = 0;
-    TRY(check_segments(outs, n, offsets, hdr_lens, &total, &max_len));
-    if (total && !bytes) return fail(AGR_EINVAL, "NULL bytes");
-    svc_host* s = h->svc;
-    uint64_t pos[SVC_MAX_CALL];
-    for (uint32_t i = 0; i < n; ++i) {
-        const uint32_t len = (uint32_t)(offsets[i + 1] - offsets[i]);
-        const uint32_t hl = (hdr_lens && outs[i].kind == AGR_OUT_RESPONSE) ? hdr_lens[i] : 0u;
-        while (!svc_submit_outcome_bytes(s, &outs[i], hl, len ? bytes + offsets[i] : nullptr, len, nullptr, 0u, &pos[i])) {}
-    }
-    int rc = 0;
-    for (uint32_t i = 0; i < n; ++i) {
-        svc_answer r; svc_wait(s, pos[i], &r);
-        int32_t res = (int32_t)r.w0;
-        if (res == AGR_ENOSPC) { res = 0; if (rc == 0) rc = AGR_ENOSPC; }
-        else if (res < 0 && res != AGR_ENOTFOUND) rc = res;
-        if (results) results[i] = res;
-        svc_release(s, pos[i]);
-    }
-    if (rc == AGR_ENOSPC)
-        return fail(rc, "response byte slab full: the outcomes were applied, their response / error bytes were not stored "
-                        "(raise agr_config.resp_bytes, or agr_reclaim with AGR_CFG_RING)");
-    if (rc < 0) return fail(rc, "single-request front end: CUDA error");
-    return 0;
-}
-
-// one outcome with its bytes in one ticket, hdr_len + body_len <= max_len (agr_submit_complete_ex: one slot;
-// agr_submit_complete_large: a span of slots above AGR_OUT_INLINE_BYTES)
-static int submit_outcome_bytes(agr_handle* h, const agr_outcome* outcome, const uint8_t* headers, uint32_t hdr_len, const uint8_t* body,
-                                uint32_t body_len, agr_ticket* ticket, uint32_t max_len, const char* too_long) {
-    if (!h || !outcome || !ticket || (hdr_len && !headers) || (body_len && !body)) return fail(AGR_EINVAL, "NULL argument");
-    if (!h->svc) return fail(AGR_EINVAL, "engine was not created with AGR_CFG_COMBINE");
-    if ((uint64_t)hdr_len + body_len > max_len) return fail(AGR_EINVAL, too_long);
-    if (outcome->kind != AGR_OUT_RESPONSE && outcome->kind != AGR_OUT_ERROR && hdr_len + body_len)
-        return fail(AGR_EINVAL, "only AGR_OUT_RESPONSE and AGR_OUT_ERROR outcomes carry bytes");
-    uint64_t a = 0;
-    if (!svc_submit_outcome_span(h->svc, outcome, outcome->kind == AGR_OUT_RESPONSE ? hdr_len : 0u, headers, hdr_len, body, body_len, &a))
-        return AGR_EAGAIN;                                       // collect outstanding tickets (agr_poll) and come again
-    *ticket = a | TICKET_OUTCOME;
-    return 0;
-}
-int agr_submit_complete_ex(agr_handle* h, const agr_outcome* outcome, const uint8_t* headers, uint32_t hdr_len,
-                           const uint8_t* body, uint32_t body_len, agr_ticket* ticket) {
-    return submit_outcome_bytes(h, outcome, headers, hdr_len, body, body_len, ticket, AGR_OUT_INLINE_BYTES,
-                                "headers + body exceed AGR_OUT_INLINE_BYTES: use agr_submit_complete_large or agr_complete_ex(n = 1)");
-}
-int agr_submit_complete_large(agr_handle* h, const agr_outcome* outcome, const uint8_t* headers, uint32_t hdr_len,
-                              const uint8_t* body, uint32_t body_len, agr_ticket* ticket) {
-    return submit_outcome_bytes(h, outcome, headers, hdr_len, body, body_len, ticket, AGR_OUT_TICKET_MAX_BYTES,
-                                "headers + body exceed AGR_OUT_TICKET_MAX_BYTES: use agr_complete_ex(n = 1)");
-}
-
 // ------------------------------------------------------------------------------------------ K3
 // (each buffer of a group is checked against its own capacity: after a failed regrow of one of them the others keep theirs)
 static int ensure_out(agr_handle* h, uint32_t cap) {
@@ -1487,8 +815,7 @@ static int gather_rows_locked(agr_handle* h, const uint32_t* d_rids, uint32_t n,
                          h->stream);
     h->k3_launches += 1;
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(h->h_gather.p, g, bytes, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
+    TRY(d2h_staged(h, nullptr, g, bytes, h->h_gather.p));
     if (disp) memcpy(disp, h->h_gather.p, disp_bytes);
     if (recs) memcpy(recs, h->h_gather.p + disp_bytes, rec_bytes);
     if (ids) memcpy(ids, h->h_gather.p + disp_bytes + rec_bytes, id_bytes);
@@ -1701,9 +1028,7 @@ static int gather_var_locked(agr_handle* h, uint32_t total, uint8_t* blob, uint6
     agr_launch_var_copy(h->d, h->d_out_rid.p, total, h->d_goffs.p, h->d_gather.p, h->stream);
     h->k3_launches += 2;
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(h->h_gather.p, h->d_gather.p, (size_t)offs[total], cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    memcpy(blob, h->h_gather.p, (size_t)offs[total]);
+    TRY(d2h_staged(h, blob, h->d_gather.p, (size_t)offs[total], h->h_gather.p));
     return 0;
 }
 
@@ -1892,629 +1217,6 @@ int agr_get_record_json(agr_handle* h, const char* agent_id, const uint8_t reque
     return rc;
 }
 
-// ------------------------------------------------------------------------------------------ durability
-static int dump_dev(agr_handle* h, FILE* f, void* dsrc, size_t bytes) {
-    const size_t chunk = h->bounce_bytes;
-    for (size_t o = 0; o < bytes; o += chunk) {
-        const size_t m = std::min(chunk, bytes - o);
-        CK(cudaMemcpyAsync(h->bounce[0], (const uint8_t*)dsrc + o, m, cudaMemcpyDeviceToHost, h->stream));
-        CK(cudaStreamSynchronize(h->stream));
-        if (fwrite(h->bounce[0], 1, m, f) != m) return fail(AGR_EINVAL, "snapshot: short write");
-    }
-    return 0;
-}
-static int load_dev(agr_handle* h, FILE* f, void* ddst, size_t bytes) {
-    const size_t chunk = h->bounce_bytes;
-    for (size_t o = 0; o < bytes; o += chunk) {
-        const size_t m = std::min(chunk, bytes - o);
-        if (fread(h->bounce[0], 1, m, f) != m) return fail(AGR_EINVAL, "restore: short read");
-        CK(cudaMemcpyAsync((uint8_t*)ddst + o, h->bounce[0], m, cudaMemcpyHostToDevice, h->stream));
-        CK(cudaStreamSynchronize(h->stream));
-    }
-    return 0;
-}
-// the physical rows a snapshot holds
-static size_t snap_rows(const snap_header& hd) {
-    return (hd.flags & AGR_CFG_RING) ? (size_t)std::min<uint64_t>(hd.rows_used, hd.slab_rows) : (size_t)hd.rows_used;
-}
-// One section of the file: its live device array, its size, and what later calls do to it.  kind SNAP_APPEND: only ever
-// appended to inside the window of a snapshot (the slab rows, the record bytes, the response bytes); SNAP_WORDS: per-row words
-// rewritten in place; SNAP_LOG: a log, rewritten in place (k_drop_logs) and compacted by agr_reclaim.  The online snapshot
-// copies the last two kinds into its shadow at the cut and streams the first from where it lies.
-enum { SNAP_APPEND = 0, SNAP_WORDS = 1, SNAP_LOG = 2 };
-struct snap_section { void* p; size_t bytes; int kind; };
-#define SNAP_NSEC 17
-// The sections that follow the header and the agent table, in file order.  Every size comes from the header alone: the one
-// description of the layout that agr_snapshot and agr_restore share (tests/test_snapshot_layout_gpu.py reads a file against it).
-static void snap_table(agr_handle* h, const snap_header& hd, snap_section out[SNAP_NSEC]) {
-    const bool ring = (hd.flags & AGR_CFG_RING) != 0, varlen = (hd.flags & AGR_CFG_VARLEN) != 0;
-    const size_t R = snap_rows(hd);
-    const snap_section sections[SNAP_NSEC] = {
-        {h->d.slab, varlen ? (size_t)(ring ? std::min<uint64_t>(hd.vused, hd.vcap) : hd.vused) : R * AGR_REC, SNAP_APPEND},
-        {h->d.state, R * 4, SNAP_WORDS},
-        {h->d.route, R * 4, SNAP_WORDS},
-        {h->d.aux, R * 4, SNAP_WORDS},
-        {h->d.cksum, R * 8, SNAP_WORDS},
-        {h->d.voff, varlen ? R * 8 : 0, SNAP_WORDS},
-        {h->d.vlen, varlen ? R * 4 : 0, SNAP_WORDS},
-        {h->d.completed_log, (size_t)hd.log_len[0] * 4, SNAP_LOG},
-        {h->d.failed_log, (size_t)hd.log_len[1] * 4, SNAP_LOG},
-        {h->d_resp, (size_t)(ring ? std::min<uint64_t>(hd.resp_used, hd.resp_cap) : hd.resp_used), SNAP_APPEND},
-        {h->d_resp_off, R * 8, SNAP_WORDS},
-        {h->d_resp_len, R * 4, SNAP_WORDS},
-        {h->d_resp_hlen, R * 4, SNAP_WORDS},
-        {h->d_err_off, R * 8, SNAP_WORDS},
-        {h->d_err_len, R * 4, SNAP_WORDS},
-        {h->d.ptime, R * 8, SNAP_WORDS},
-        {h->d.mtime, R * 8, SNAP_WORDS},
-    };
-    for (int k = 0; k < SNAP_NSEC; ++k) out[k] = sections[k];
-}
-// Hands every section to io (dump_dev, load_dev or the online writer's dump_online) as (device array, bytes).  The source
-// table says where each section's bytes are: nullptr = the live arrays; the online writer passes the cut's shadow, which
-// holds the sections rewritten in place at h->shadow_off (the append-only ones still come from the live arrays).
-static int snap_sections(agr_handle* h, const snap_header& hd, FILE* f, int (*io)(agr_handle*, FILE*, void*, size_t),
-                         uint8_t* shadow = nullptr) {
-    snap_section sec[SNAP_NSEC];
-    snap_table(h, hd, sec);
-    for (int k = 0; k < SNAP_NSEC; ++k) TRY(io(h, f, shadow && sec[k].kind != SNAP_APPEND ? shadow + h->shadow_off[k] : sec[k].p, sec[k].bytes));
-    return 0;
-}
-
-// ---- AGR_CFG_DELTA_SNAPSHOT
-// A delta file (AGRDELT1): this header; the parent's absolute path; the agent table, as in a full file; the appended slab rows
-// (record bytes with AGR_CFG_VARLEN) [rows_lo, rows_hi), then the appended response bytes [resp_lo, resp_hi), both in physical
-// order, in one run or two where the ring wraps; the ascending list of dirty word blocks (u32), then each listed block's slice
-// of every SNAP_WORDS section of snap_table, in table order; then per log (completed, failed) the same for its dirty log
-// blocks.  Only the last block of a section may be short.  The digests are the compare cut's keyed sums over the word
-// sections [0, R) and the log prefixes of the parent's cut and of this one.
-#define SNAP_BLOCK_ROWS 256u
-#define SNAP_LOG_BLOCK 1024u
-struct delta_header {
-    char magic[8];                 // "AGRDELT1"
-    snap_header cut;               // the state this file brings a restore to
-    uint64_t file_bytes;           // a restore refuses a shorter file
-    unsigned long long parent_digest[2], digest[2];
-    uint32_t block_rows, log_block;
-    uint64_t rows_lo, rows_hi, resp_lo, resp_hi;
-    uint64_t n_blocks[3];          // listed blocks per table of snap_block_tables
-    uint32_t parent_path_len, pad;
-};
-static_assert(sizeof(delta_header) == 264 && sizeof(snap_header) == 144, "delta_header is a file layout");
-
-// Everything the compare cut, the gather and the scatter use; allocated at agr_create (or by the restore of a delta chain)
-static int snap_delta_alloc(agr_handle* h) {
-    if (h->d_snap_stage) return 0;
-    const size_t nwb = (h->cfg.slab_rows + SNAP_BLOCK_ROWS - 1) / SNAP_BLOCK_ROWS, nlb = (h->d.log_cap + SNAP_LOG_BLOCK - 1) / SNAP_LOG_BLOCK;
-    h->snap_bit_off[1] = (nwb + 31) / 32; h->snap_bit_off[2] = h->snap_bit_off[1] + (nlb + 31) / 32;
-    h->snap_bit_words = h->snap_bit_off[2] + (nlb + 31) / 32;
-    TRY(dev_alloc(h, &h->d_snap_bits, h->snap_bit_words, false));
-    TRY(dev_alloc(h, &h->d_snap_digest, (size_t)2, false));
-    TRY(host_alloc(h, &h->h_snap_bits, 32 + h->snap_bit_words * 4));
-    TRY(dev_alloc(h, &h->d_snap_list, std::max<size_t>(std::max(nwb, nlb), 1), false));
-    h->snap_stage_bytes = std::max<size_t>(h->bounce_bytes, (size_t)1 << 20);   // >= one block of every section
-    TRY(dev_alloc(h, &h->d_snap_stage, h->snap_stage_bytes, false));
-    return 0;
-}
-static size_t snap_full_bytes(agr_handle* h, const snap_header& hd) {
-    snap_section sec[SNAP_NSEC];
-    snap_table(h, hd, sec);
-    size_t n = sizeof(snap_header) + (size_t)hd.n_agents * (AGR_AGENT_ID_BYTES + 1);
-    for (int k = 0; k < SNAP_NSEC; ++k) n += sec[k].bytes;
-    return n;
-}
-// The cut's sections: the SNAP_WORDS ones that hold bytes, then the two logs (whose lengths the kernel reads on the device
-// unless lens_from_host).  A word block is 256 rows: 16 * width pieces of 16 B; a log block 1024 entries: 256 pieces.
-static void snap_cut_params(agr_handle* h, const snap_header& hd, bool lens_from_host, agr_snap_cmp& c) {
-    snap_section sec[SNAP_NSEC];
-    snap_table(h, hd, sec);
-    const size_t R = snap_rows(hd);
-    c = agr_snap_cmp{};
-    c.shadow = h->d_shadow; c.bits = h->d_snap_bits; c.digest = h->d_snap_digest; c.key = h->d.id_secret;
-    c.lens_from_host = lens_from_host ? 1u : 0u;
-    int logs[2], nlog = 0;
-    for (int k = 0; k < SNAP_NSEC; ++k) {
-        if (sec[k].kind == SNAP_LOG) logs[nlog++] = k;
-        if (sec[k].kind != SNAP_WORDS || sec[k].bytes == 0) continue;
-        const uint32_t n = c.nrow++;
-        c.src[n] = (const uint8_t*)sec[k].p; c.dst_off[n] = h->shadow_off[k]; c.bytes[n] = sec[k].bytes;
-        c.pshift[n] = (uint32_t)__builtin_ctzll(16 * (sec[k].bytes / R)); c.bit_off[n] = 0; c.sec_id[n] = (uint32_t)k;
-    }
-    for (int j = 0; j < 2; ++j) {
-        const uint32_t n = c.nrow + j;
-        c.src[n] = (const uint8_t*)sec[logs[j]].p; c.dst_off[n] = h->shadow_off[logs[j]]; c.bytes[n] = sec[logs[j]].bytes;
-        c.pshift[n] = 8; c.bit_off[n] = (uint32_t)h->snap_bit_off[1 + j]; c.sec_id[n] = (uint32_t)logs[j];
-    }
-}
-// the cut (caller holds HLock): one kernel copies the per-row words of rows [0, R) and the two log prefixes into the shadow;
-// with compare, it also marks the blocks that differ from the previous cut and sums the digest of this one
-static int snap_cut_locked(agr_handle* h, const snap_header& hd, bool compare) {
-    agr_snap_cmp c;
-    snap_cut_params(h, hd, false, c);
-    if (compare) {
-        CK(cudaMemsetAsync(h->d_snap_bits, 0, h->snap_bit_words * 4, h->stream));
-        CK(cudaMemsetAsync(h->d_snap_digest, 0, 16, h->stream));
-    }
-    TRY(op_time_begin(h, 3));
-    if (compare) agr_launch_snap_cmp(h->d, c, true, h->sm_count, h->stream);
-    else agr_launch_snap_cut(h->d, c, h->sm_count, h->stream);
-    CK(cudaGetLastError());
-    TRY(op_time_end(h, 3));
-    CK(cudaEventRecord(h->snap_ev[0], h->stream));
-    return 0;
-}
-// (restore) the digest of the live arrays as hd describes them.  seed: through the compare cut, which also leaves them in the
-// shadow, so that the next snapshot of an AGR_CFG_DELTA_SNAPSHOT engine compares against the restored state
-static int snap_digest_locked(agr_handle* h, const snap_header& hd, bool seed, unsigned long long out[2]) {
-    agr_snap_cmp c;
-    snap_cut_params(h, hd, !seed, c);
-    if (seed) CK(cudaMemsetAsync(h->d_snap_bits, 0, h->snap_bit_words * 4, h->stream));
-    CK(cudaMemsetAsync(h->d_snap_digest, 0, 16, h->stream));
-    agr_launch_snap_cmp(h->d, c, seed, h->sm_count, h->stream);
-    CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(h->h_snap_bits, h->d_snap_digest, 16, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    memcpy(out, h->h_snap_bits, 16);
-    return 0;
-}
-// The block tables of a delta, in file order: [0] the word sections of hd (256 rows per block), [1] and [2] the completed and
-// failed logs (1024 entries per block), in the shadow (the writer) or the live arrays (restore).  Table t's bits start at
-// snap_bit_off[t].
-static void snap_block_tables(agr_handle* h, const snap_header& hd, bool shadow, agr_snap_blocks g[3]) {
-    snap_section sec[SNAP_NSEC];
-    snap_table(h, hd, sec);
-    for (int t = 0; t < 3; ++t) g[t] = agr_snap_blocks{};
-    g[0].block_rows = SNAP_BLOCK_ROWS; g[0].rows = snap_rows(hd);
-    for (int k = 0, j = 0; k < SNAP_NSEC; ++k) {
-        uint8_t* a = shadow ? h->d_shadow + h->shadow_off[k] : (uint8_t*)sec[k].p;
-        if (sec[k].kind == SNAP_LOG) {
-            agr_snap_blocks& l = g[1 + j];
-            l.arr[0] = a; l.nsec = 1; l.width[0] = 4; l.block_rows = SNAP_LOG_BLOCK; l.rows = hd.log_len[j++]; l.rec_bytes = 4ull * SNAP_LOG_BLOCK;
-        } else if (sec[k].kind == SNAP_WORDS && sec[k].bytes) {
-            agr_snap_blocks& w = g[0];
-            w.arr[w.nsec] = a; w.width[w.nsec] = (uint32_t)(sec[k].bytes / w.rows);
-            w.rec_bytes += (unsigned long long)w.width[w.nsec] * SNAP_BLOCK_ROWS;
-            w.nsec++;
-        }
-    }
-}
-// bytes of the slices of n listed blocks (only the table's last block may be short)
-static uint64_t snap_blocks_bytes(const agr_snap_blocks& g, const uint32_t* list, size_t n) {
-    if (!n) return 0;
-    const uint64_t last = list[n - 1], r0 = last * g.block_rows;
-    return (n - 1) * g.rec_bytes + std::min<uint64_t>(g.block_rows, g.rows - r0) * (g.rec_bytes / g.block_rows);
-}
-// The appended pieces of a delta, in file order: the slab rows (record bytes with AGR_CFG_VARLEN) [rows_lo, rows_hi), then the
-// response bytes [resp_lo, resp_hi), each in one physical run or two where its ring wraps, as (live device array, bytes)
-struct snap_piece { uint8_t* p; uint64_t bytes; };
-static int snap_delta_pieces(agr_handle* h, const delta_header& dh, snap_piece out[4]) {
-    const snap_header& hd = dh.cut;
-    const bool var = (hd.flags & AGR_CFG_VARLEN) != 0, ring = (hd.flags & AGR_CFG_RING) != 0;
-    const struct { uint64_t lo, hi, cap; uint8_t* base; uint64_t unit; } spans[2] = {
-        {dh.rows_lo, dh.rows_hi, var ? hd.vcap : hd.slab_rows, h->d.slab, var ? 1ull : (uint64_t)AGR_REC}, {dh.resp_lo, dh.resp_hi, hd.resp_cap, h->d_resp, 1}};
-    int n = 0;
-    for (const auto& s : spans) {
-        if (s.hi <= s.lo) continue;
-        const uint64_t p = ring ? s.lo % s.cap : s.lo, n0 = ring ? std::min(s.hi - s.lo, s.cap - p) : s.hi - s.lo;
-        out[n++] = {s.base + p * s.unit, n0 * s.unit};
-        if (s.hi - s.lo > n0) out[n++] = {s.base, (s.hi - s.lo - n0) * s.unit};
-    }
-    return n;
-}
-// the absolute name a chain keeps of a file: realpath of its directory, then its name ("" if the directory does not resolve)
-static std::string snap_abs_path(const std::string& p) {
-    const size_t cut = p.rfind('/');
-    const std::string dir = cut == std::string::npos ? "." : (cut == 0 ? "/" : p.substr(0, cut));
-    char buf[PATH_MAX];
-    if (!realpath(dir.c_str(), buf)) return "";
-    std::string out(buf);
-    if (out.back() != '/') out += '/';
-    return out + (cut == std::string::npos ? p : p.substr(cut + 1));
-}
-
-// ---- AGR_CFG_ONLINE_SNAPSHOT
-// The shadow holds every section rewritten in place at full capacity (slab_rows rows, log_entries entries), each at a 256 B
-// boundary behind a 256 B area with the two log lengths the cut read.  Everything is allocated here: nothing is allocated or
-// freed while a snapshot runs (cudaFree would wait for the resident service kernel).
-static int snap_online_create(agr_handle* h) {
-    snap_header cap{};
-    cap.flags = h->cfg.flags & (AGR_CFG_VARLEN | AGR_CFG_RING);
-    cap.rows_used = cap.slab_rows = h->cfg.slab_rows;
-    cap.log_len[0] = cap.log_len[1] = h->d.log_cap;
-    snap_section sec[SNAP_NSEC];
-    snap_table(h, cap, sec);
-    size_t at = 256;
-    for (int k = 0; k < SNAP_NSEC; ++k) {
-        if (sec[k].kind == SNAP_APPEND || sec[k].bytes == 0) continue;
-        h->shadow_off[k] = at;
-        at += (sec[k].bytes + 255) & ~(size_t)255;
-    }
-    TRY(dev_alloc(h, &h->d_shadow, at, false));
-    h->snap_buf_bytes = h->bounce_bytes;
-    for (int b = 0; b < 2; ++b) TRY(host_alloc(h, &h->snap_buf[b], h->snap_buf_bytes));
-    for (auto& e : h->snap_ev) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    // non-blocking: a stream that synchronised with the legacy default stream would also wait behind the resident kernel
-    CK(cudaStreamCreateWithFlags(&h->snap_stream, cudaStreamNonBlocking));
-    if (h->cfg.flags & AGR_CFG_DELTA_SNAPSHOT) TRY(snap_delta_alloc(h));
-    return 0;
-}
-// the writer stream starts behind the cut; reads what the cut left: the log lengths it read (into hd), and with compare the
-// digest and the dirty bits (into h_snap_bits + 16 and + 32)
-static int snap_read_cut(agr_handle* h, snap_header& hd, bool compare) {
-    if (cudaStreamWaitEvent(h->snap_stream, h->snap_ev[0], 0) != cudaSuccess ||
-        cudaMemcpyAsync(h->snap_buf[0], h->d_shadow, 16, cudaMemcpyDeviceToHost, h->snap_stream) != cudaSuccess ||
-        (compare && (cudaMemcpyAsync(h->h_snap_bits + 16, h->d_snap_digest, 16, cudaMemcpyDeviceToHost, h->snap_stream) != cudaSuccess ||
-                     cudaMemcpyAsync(h->h_snap_bits + 32, h->d_snap_bits, h->snap_bit_words * 4, cudaMemcpyDeviceToHost, h->snap_stream) != cudaSuccess)) ||
-        cudaStreamSynchronize(h->snap_stream) != cudaSuccess) return fail(AGR_ECUDA, "snapshot: cut");
-    memcpy(hd.log_len, h->snap_buf[0], 16);
-    return 0;
-}
-// writes the chunk waiting in the buffer the next chunk does not use, once its copy has landed
-static int snap_drain(agr_handle* h, FILE* f) {
-    if (!h->snap_pend) return 0;
-    const int b = h->snap_cur ^ 1;
-    const size_t m = h->snap_pend;
-    h->snap_pend = 0;
-    CK(cudaEventSynchronize(h->snap_ev[1 + b]));
-    if (fwrite(h->snap_buf[b], 1, m, f) != m) return fail(AGR_EINVAL, "snapshot: short write");
-    return 0;
-}
-// the online writer's io: chunk k's copy on the writer stream overlaps the fwrite of chunk k - 1 (two pinned buffers)
-static int dump_online(agr_handle* h, FILE* f, void* dsrc, size_t bytes) {
-    for (size_t o = 0; o < bytes;) {
-        const size_t m = std::min(h->snap_buf_bytes, bytes - o);
-        const int b = h->snap_cur;
-        CK(cudaMemcpyAsync(h->snap_buf[b], (const uint8_t*)dsrc + o, m, cudaMemcpyDeviceToHost, h->snap_stream));
-        CK(cudaEventRecord(h->snap_ev[1 + b], h->snap_stream));
-        TRY(snap_drain(h, f));
-        h->snap_cur ^= 1; h->snap_pend = m;
-        o += m;
-    }
-    return 0;
-}
-static void snap_fill_header(agr_handle* h, snap_header& hd) {
-    memcpy(hd.magic, "AGRSNAP3", 8);
-    hd.flags = h->cfg.flags & (AGR_CFG_PERSISTENCE | AGR_CFG_MINT_IDS | AGR_CFG_VARLEN | AGR_CFG_RING);
-    hd.n_agents = (uint32_t)h->agent_names.size(); hd.shard = h->d.shard_id; hd.gen = h->d.id_gen;
-    hd.rows_used = h->rows_used; hd.vused = h->vused; hd.id_secret = h->d.id_secret; hd.scan_lo = h->scan_lo;
-    hd.resp_used = h->resp_used; hd.expired_total = h->expired_total; hd.tail = h->tail; hd.released_total = h->released_total; hd.slab_rows = h->cfg.slab_rows; hd.vtail = h->vtail; hd.vcap = h->vcap; hd.resp_tail = h->resp_tail; hd.resp_cap = h->resp_cap;
-}
-// the agent table as a file holds it: per agent its NUL-padded name (AGR_AGENT_ID_BYTES), then its status byte
-static std::vector<char> snap_agents(agr_handle* h) {
-    std::vector<char> agents(h->agent_names.size() * (AGR_AGENT_ID_BYTES + 1), 0);
-    for (size_t a = 0; a < h->agent_names.size(); ++a) {
-        char* e = agents.data() + a * (AGR_AGENT_ID_BYTES + 1);
-        strncpy(e, h->agent_names[a].c_str(), AGR_AGENT_ID_BYTES - 1);
-        e[AGR_AGENT_ID_BYTES] = (char)h->agent_status[a];
-    }
-    return agents;
-}
-// A full file (AGRSNAP3): the header, the agent table, then the sections through io (dump_dev, or dump_online with the cut's
-// shadow as in snap_sections) and the drain of the last chunk (nothing is pending after dump_dev)
-static int snap_write_full(agr_handle* h, FILE* f, const snap_header& hd, const std::vector<char>& agents,
-                           int (*io)(agr_handle*, FILE*, void*, size_t), uint8_t* shadow = nullptr) {
-    if (fwrite(&hd, sizeof hd, 1, f) != 1 || fwrite(agents.data(), 1, agents.size(), f) != agents.size())
-        return fail(AGR_EINVAL, "snapshot: short write");
-    TRY(snap_sections(h, hd, f, io, shadow));
-    return snap_drain(h, f);
-}
-// closes a file a snapshot wrote; a failed close (the last buffered bytes did not reach the file) fails a snapshot that had not
-// failed already
-static int snap_close(FILE* f, int r) {
-    if (fclose(f) != 0 && r == 0) return fail(AGR_EINVAL, "snapshot: close failed");
-    return r;
-}
-// the writer: the list, then the listed blocks of g, packed on the writer stream into the staging buffer (stream order keeps
-// a chunk's copies ahead of the next chunk's gather) and streamed through the pinned buffers
-static int dump_blocks(agr_handle* h, FILE* f, agr_snap_blocks g, const std::vector<uint32_t>& list) {
-    TRY(snap_drain(h, f));
-    if (list.empty()) return 0;
-    if (fwrite(list.data(), 4, list.size(), f) != list.size()) return fail(AGR_EINVAL, "snapshot: short write");
-    CK(cudaMemcpyAsync(h->d_snap_list, list.data(), list.size() * 4, cudaMemcpyHostToDevice, h->snap_stream));
-    const size_t per = h->snap_stage_bytes / g.rec_bytes;
-    g.stage = h->d_snap_stage;
-    for (size_t j = 0; j < list.size(); j += per) {
-        const size_t n = std::min(per, list.size() - j);
-        g.list = h->d_snap_list + j;
-        agr_launch_snap_blocks(g, (uint32_t)n, true, h->snap_stream);
-        CK(cudaGetLastError());
-        TRY(dump_online(h, f, h->d_snap_stage, snap_blocks_bytes(g, list.data() + j, n)));
-    }
-    return 0;
-}
-// AGR_CFG_DELTA_SNAPSHOT: writes a delta on the chain's last file, or a full file when there is no chain, path is one of its
-// files, or the deltas would outgrow a full file (hd, the digest and the dirty bits are what the compare cut left)
-static int snap_write_chain(agr_handle* h, FILE* f, const char* path, const snap_header& hd, const std::vector<char>& agents, uint64_t bound) {
-    unsigned long long digest[2];
-    memcpy(digest, h->h_snap_bits + 16, 16);
-    const uint32_t* bits = reinterpret_cast<const uint32_t*>(h->h_snap_bits + 32);
-    const std::string at = snap_abs_path(path);
-    if (at.empty()) return fail(AGR_EINVAL, std::string("snapshot: cannot resolve the directory of ") + path);
-    snap_chain& ch = h->chain;
-    const size_t full = snap_full_bytes(h, hd);
-    bool delta = !ch.paths.empty() && std::find(ch.paths.begin(), ch.paths.end(), at) == ch.paths.end();
-    delta_header dh{};
-    std::vector<uint32_t> list[3];
-    agr_snap_blocks g[3];
-    snap_piece pc[4];
-    int npc = 0;
-    snap_block_tables(h, hd, true, g);
-    if (delta) {
-        const snap_header& b = ch.base;
-        const bool var = (hd.flags & AGR_CFG_VARLEN) != 0;
-        memcpy(dh.magic, "AGRDELT1", 8);
-        dh.cut = hd;
-        memcpy(dh.parent_digest, ch.digest, 16); memcpy(dh.digest, digest, 16);
-        dh.block_rows = SNAP_BLOCK_ROWS; dh.log_block = SNAP_LOG_BLOCK;
-        // appended since the parent's cut: from the first row (byte) it did not hold yet, clipped to this cut's window
-        dh.rows_hi = var ? hd.vused : hd.rows_used;
-        dh.rows_lo = std::min(dh.rows_hi, std::max(var ? b.vused : ch.base_bound, var ? hd.vtail : hd.tail));
-        dh.resp_hi = hd.resp_used;
-        dh.resp_lo = std::min(dh.resp_hi, std::max(b.resp_used, hd.resp_tail));
-        dh.parent_path_len = (uint32_t)ch.paths.back().size();
-        dh.file_bytes = sizeof dh + dh.parent_path_len + agents.size();
-        npc = snap_delta_pieces(h, dh, pc);
-        for (int j = 0; j < npc; ++j) dh.file_bytes += pc[j].bytes;
-        // dirty blocks, and every block that reaches past what the parent's cut held (the shadow has nothing of it there)
-        agr_snap_blocks pg[3];
-        snap_block_tables(h, b, true, pg);
-        for (int t = 0; t < 3; ++t) {
-            const uint32_t* tb = bits + h->snap_bit_off[t];
-            const uint64_t first_new = pg[t].rows / pg[t].block_rows;
-            for (uint64_t k = 0; k * g[t].block_rows < g[t].rows; ++k)
-                if (k >= first_new || ((tb[k >> 5] >> (k & 31)) & 1u)) list[t].push_back((uint32_t)k);
-            dh.n_blocks[t] = list[t].size();
-            dh.file_bytes += 4 * list[t].size() + snap_blocks_bytes(g[t], list[t].data(), list[t].size());
-        }
-        delta = ch.delta_bytes + dh.file_bytes <= full;              // else a full file: a restore reads at most ~2 full files
-    }
-    if (!delta) {
-        TRY(snap_write_full(h, f, hd, agents, dump_online, h->d_shadow));
-        ch = snap_chain{};
-        ch.full_bytes = full;
-    } else {
-        const std::string& parent = ch.paths.back();
-        if (fwrite(&dh, sizeof dh, 1, f) != 1 || fwrite(parent.data(), 1, parent.size(), f) != parent.size() ||
-            fwrite(agents.data(), 1, agents.size(), f) != agents.size()) return fail(AGR_EINVAL, "snapshot: short write");
-        for (int j = 0; j < npc; ++j) TRY(dump_online(h, f, pc[j].p, pc[j].bytes));
-        for (int t = 0; t < 3; ++t) TRY(dump_blocks(h, f, g[t], list[t]));
-        TRY(snap_drain(h, f));
-        ch.delta_bytes += dh.file_bytes;
-    }
-    ch.paths.push_back(at);
-    ch.base = hd; ch.base_bound = bound;
-    memcpy(ch.digest, digest, 16);
-    return 0;
-}
-
-// The handle is held only while the cut is enqueued; the file is written afterwards while every other call goes on.
-static int snapshot_online(agr_handle* h, const char* path) {
-    std::lock_guard<std::mutex> one(h->snap_mu);
-    CK(cudaSetDevice(h->device));
-    FILE* f = fopen(path, "wb");
-    if (!f) return fail(AGR_EINVAL, std::string("snapshot: cannot open ") + path);
-    const bool chain = (h->cfg.flags & AGR_CFG_DELTA_SNAPSHOT) != 0;
-    snap_header hd{};
-    std::vector<char> agents;                                  // the agent table as it was at the cut
-    uint64_t bound = 0;                                        // rows below were ingested at the cut
-    {
-        HLock lk(h);
-        snap_fill_header(h, hd);
-        agents = snap_agents(h);
-        bound = ingested_bound(h);
-        const int rc = snap_cut_locked(h, hd, chain);
-        if (rc < 0) { fclose(f); h->chain = snap_chain{}; return rc; }
-        if (is_ring(h)) { h->pinned = true; h->pin_tail = h->tail; h->pin_vtail = h->vtail; h->pin_resp_tail = h->resp_tail; }
-    }
-    int rc = snap_read_cut(h, hd, chain);
-    if (rc == 0) rc = chain ? snap_write_chain(h, f, path, hd, agents, bound) : snap_write_full(h, f, hd, agents, dump_online, h->d_shadow);
-    if (cudaStreamSynchronize(h->snap_stream) != cudaSuccess && rc == 0) rc = fail(AGR_ECUDA, "snapshot: writer stream");
-    h->snap_pend = 0; h->snap_cur = 0;
-    { std::lock_guard<std::mutex> g(h->mu); h->pinned = false; }
-    rc = snap_close(f, rc);
-    if (rc != 0) h->chain = snap_chain{};                      // a file that failed is no base: the next one is full
-    return rc;
-}
-
-int agr_snapshot(agr_handle* h, const char* path) {
-    if (!h || !path) return fail(AGR_EINVAL, "NULL argument");
-    if (h->cfg.flags & AGR_CFG_ONLINE_SNAPSHOT) return snapshot_online(h, path);
-    HLock lk(h);
-    CK(cudaSetDevice(h->device));
-    CK(cudaStreamSynchronize(h->stream));
-    FILE* f = fopen(path, "wb");
-    if (!f) return fail(AGR_EINVAL, std::string("snapshot: cannot open ") + path);
-    snap_header hd{};
-    snap_fill_header(h, hd);
-    unsigned long long lens[2] = {0, 0};
-    int rc = read_log_lens(h, lens);
-    hd.log_len[0] = lens[0]; hd.log_len[1] = lens[1];
-    if (rc == 0) rc = snap_write_full(h, f, hd, snap_agents(h), dump_dev);
-    return snap_close(f, rc);
-}
-
-// ---- restore: a full file, then the deltas of its chain, oldest first
-// The agent table of a file: entry a is slot a.  An agent the engine already has (registered before the parent's cut) keeps its
-// name and slot, and only its status changes; a new one is registered in table order, so that the slots match.
-static int restore_agents_locked(agr_handle* h, FILE* f, uint32_t n) {
-    for (uint32_t a = 0; a < n; ++a) {
-        char name[AGR_AGENT_ID_BYTES]; uint8_t st;
-        if (fread(name, 1, AGR_AGENT_ID_BYTES, f) != AGR_AGENT_ID_BYTES || fread(&st, 1, 1, f) != 1) return fail(AGR_EINVAL, "restore: short read");
-        name[AGR_AGENT_ID_BYTES - 1] = 0;
-        const bool removed = (st == AG_STATUS_REMOVED), known = a < h->agent_names.size();
-        if (known && h->agent_names[a] != name) return fail(AGR_EINVAL, "restore: the agent table of a delta does not extend its parent's");
-        if (!known || !removed) {
-            const int s = set_agent_state_locked(h, name, removed ? (uint8_t)AGR_AGENT_STOPPED : st, true);
-            if (s < 0) return s;
-            if ((uint32_t)s != a) return fail(AGR_EINVAL, "restore: an agent appears twice in the agent table");
-        }
-        if (removed) { h->agent_status[a] = AG_STATUS_REMOVED; TRY(push_agent_status(h, a, AG_STATUS_REMOVED)); }
-    }
-    return 0;
-}
-// the scatter: n listed blocks of g, read from the file chunk by chunk into the staging buffer and placed into the live arrays
-static int load_blocks(agr_handle* h, FILE* f, agr_snap_blocks g, uint64_t n) {
-    const uint64_t nb = (g.rows + g.block_rows - 1) / g.block_rows;
-    if (n > nb) return fail(AGR_EINVAL, "restore: corrupt delta (more blocks listed than its sections have)");
-    std::vector<uint32_t> list(n);
-    if (n && fread(list.data(), 4, n, f) != n) return fail(AGR_EINVAL, "restore: short read");
-    for (size_t j = 0; j < n; ++j)
-        if (list[j] >= nb || (j && list[j] <= list[j - 1])) return fail(AGR_EINVAL, "restore: corrupt delta (block list)");
-    if (!n) return 0;
-    CK(cudaMemcpyAsync(h->d_snap_list, list.data(), n * 4, cudaMemcpyHostToDevice, h->stream));
-    const size_t per = h->snap_stage_bytes / g.rec_bytes;
-    g.stage = h->d_snap_stage;
-    for (size_t j = 0; j < n; j += per) {
-        const size_t m = std::min<size_t>(per, n - j);
-        TRY(load_dev(h, f, h->d_snap_stage, snap_blocks_bytes(g, list.data() + j, m)));   // (stream-ordered after the last scatter)
-        g.list = h->d_snap_list + j;
-        agr_launch_snap_blocks(g, (uint32_t)m, false, h->stream);
-        CK(cudaGetLastError());
-    }
-    CK(cudaStreamSynchronize(h->stream));
-    return 0;
-}
-// applies one delta (f is past its header and parent path) to the live arrays; the header fields are set by the caller
-static int restore_delta_locked(agr_handle* h, FILE* f, const delta_header& dh) {
-    TRY(restore_agents_locked(h, f, dh.cut.n_agents));
-    snap_piece pc[4];
-    for (int n = snap_delta_pieces(h, dh, pc), j = 0; j < n; ++j) TRY(load_dev(h, f, pc[j].p, pc[j].bytes));
-    agr_snap_blocks g[3];
-    snap_block_tables(h, dh.cut, false, g);
-    for (int t = 0; t < 3; ++t) TRY(load_blocks(h, f, g[t], dh.n_blocks[t]));
-    if ((uint64_t)ftello(f) != dh.file_bytes) return fail(AGR_EINVAL, "restore: corrupt delta (its sections do not add up to its size)");
-    return 0;
-}
-// Follows the parent paths from path back to a full file: files[0] is that file, files[k] (k >= 1) the delta dh[k - 1].
-static int restore_chain(const char* path, std::vector<std::string>& files, std::vector<delta_header>& dh) {
-    std::string p = path;
-    for (;;) {
-        const std::string of = files.empty() ? "" : ", the parent of " + files.front();
-        if (files.size() > 65536) return fail(AGR_EINVAL, "restore: the chain of parents does not end in a full file");
-        FILE* f = fopen(p.c_str(), "rb");
-        if (!f) return fail(AGR_EINVAL, "restore: cannot open " + p + of);
-        char magic[8] = {0};
-        const bool got = fread(magic, 1, 8, f) == 8;
-        if (got && memcmp(magic, "AGRSNAP3", 8) == 0) { fclose(f); files.insert(files.begin(), p); return 0; }
-        if (!got || memcmp(magic, "AGRDELT1", 8) != 0) { fclose(f); return fail(AGR_EINVAL, files.empty() ? "restore: not a snapshot" : "restore: " + p + of + ", is not a snapshot"); }
-        delta_header d{};
-        struct stat st{};
-        rewind(f);
-        const bool ok = fread(&d, sizeof d, 1, f) == 1 && fstat(fileno(f), &st) == 0;
-        std::string parent(ok && d.parent_path_len <= PATH_MAX ? d.parent_path_len : 0, '\0');
-        const bool named = ok && d.parent_path_len && d.parent_path_len <= PATH_MAX && fread(&parent[0], 1, parent.size(), f) == parent.size();
-        fclose(f);
-        if (!ok || (uint64_t)st.st_size < d.file_bytes) return fail(AGR_EINVAL, "restore: " + p + of + " is shorter than its header says (truncated)");
-        const bool var = (d.cut.flags & AGR_CFG_VARLEN) != 0;
-        if (!named || d.block_rows != SNAP_BLOCK_ROWS || d.log_block != SNAP_LOG_BLOCK || d.rows_lo > d.rows_hi ||
-            d.rows_hi != (var ? d.cut.vused : d.cut.rows_used) || d.resp_lo > d.resp_hi || d.resp_hi != d.cut.resp_used ||
-            d.rows_hi - d.rows_lo > (var ? d.cut.vcap : d.cut.slab_rows) || d.resp_hi - d.resp_lo > d.cut.resp_cap)
-            return fail(AGR_EINVAL, "restore: " + p + of + " is not a valid delta");
-        files.insert(files.begin(), p);
-        dh.insert(dh.begin(), d);
-        p = parent;
-    }
-}
-// The state of the whole chain into h: the full file (f, past its header), each delta after a check that the state so far
-// is its parent's cut (digest), then the header fields, the log lengths, the dedupe index and the chain an
-// AGR_CFG_DELTA_SNAPSHOT engine continues, once.
-static int restore_locked(agr_handle* h, FILE* f, const snap_header& full, const std::vector<std::string>& files, const std::vector<delta_header>& dh) {
-    HLock lk(h);
-    CK(cudaSetDevice(h->device));
-    TRY(restore_agents_locked(h, f, full.n_agents));
-    TRY(snap_sections(h, full, f, load_dev));
-    const bool chain = (h->cfg.flags & AGR_CFG_DELTA_SNAPSHOT) != 0;
-    if (!dh.empty()) TRY(snap_delta_alloc(h));
-    const snap_header* at = &full;
-    unsigned long long dg[2] = {0, 0};
-    for (size_t k = 0; k < dh.size(); ++k) {
-        TRY(snap_digest_locked(h, *at, false, dg));
-        if (memcmp(dg, dh[k].parent_digest, 16) != 0)
-            return fail(AGR_EINVAL, "restore: " + files[k] + " is not the snapshot " + files[k + 1] + " was written on (digest differs): was it replaced?");
-        FILE* g = fopen(files[k + 1].c_str(), "rb");
-        if (!g) return fail(AGR_EINVAL, "restore: cannot open " + files[k + 1]);
-        int rc = fseeko(g, (off_t)(sizeof(delta_header) + dh[k].parent_path_len), SEEK_SET) == 0 ? restore_delta_locked(h, g, dh[k])
-                                                                                                : fail(AGR_EINVAL, "restore: short read");
-        fclose(g);
-        TRY(rc);
-        at = &dh[k].cut;
-    }
-    const snap_header& hd = *at;
-    const size_t R = snap_rows(hd);
-    h->resp_used = hd.resp_used; h->resp_tail = hd.resp_tail; h->expired_total = hd.expired_total;
-    unsigned long long lens[2] = {hd.log_len[0], hd.log_len[1]};
-    if (cudaMemcpy(h->d.log_len, lens, sizeof lens, cudaMemcpyHostToDevice) != cudaSuccess) return fail(AGR_ECUDA, "restore: log_len");
-    h->rows_used = hd.rows_used; h->vused = hd.vused; h->vtail = hd.vtail; h->scan_lo = hd.scan_lo;
-    h->d.shard_id = hd.shard; h->d.id_gen = hd.gen; h->tail = hd.tail; h->released_total = hd.released_total; sync_window(h);
-    h->d.idx_base = h->tail;
-    cudaMemsetAsync(h->d.cmin, 0, (size_t)(h->cfg.slab_rows / AGR_CHUNK_ROWS + 2) * 8, h->stream);       // time bounds unknown: the first sweep recomputes them
-    if (!(hd.flags & AGR_CFG_MINT_IDS) && R) {        // hash-id mode: rebuild the dedupe index from the restored rows
-        agr_launch_reindex(h->d, (uint32_t)R, h->stream);
-        h->k1_launches += 1;
-        if (cudaStreamSynchronize(h->stream) != cudaSuccess) return fail(AGR_ECUDA, "restore: reindex");
-    }
-    if (chain || !dh.empty()) {
-        TRY(snap_digest_locked(h, hd, chain, dg));    // an AGR_CFG_DELTA_SNAPSHOT engine: also seeds the shadow
-        if (!dh.empty() && memcmp(dg, dh.back().digest, 16) != 0)
-            return fail(AGR_EINVAL, "restore: the state after " + files.back() + " differs from the one it was written from (digest)");
-    }
-    if (chain) {
-        snap_chain& ch = h->chain;
-        ch = snap_chain{};
-        ch.paths = files;
-        ch.paths.back() = snap_abs_path(files.back());   // (the parents' paths are absolute already)
-        ch.full_bytes = snap_full_bytes(h, full);
-        for (const auto& d : dh) ch.delta_bytes += d.file_bytes;
-        ch.base = hd; ch.base_bound = hd.rows_used;
-        memcpy(ch.digest, dg, 16);
-        if (ch.paths.back().empty()) ch = snap_chain{};
-    }
-    return 0;
-}
-
-int agr_restore(const agr_config* cfg, const char* path, agr_handle** out) {
-    if (!cfg || !path || !out) return fail(AGR_EINVAL, "NULL argument");
-    *out = nullptr;
-    std::vector<std::string> files;
-    std::vector<delta_header> dh;
-    TRY(restore_chain(path, files, dh));
-    FILE* f = fopen(files[0].c_str(), "rb");
-    if (!f) return fail(AGR_EINVAL, "restore: cannot open " + files[0]);
-    snap_header hd{};
-    if (fread(&hd, sizeof hd, 1, f) != 1 || memcmp(hd.magic, "AGRSNAP3", 8) != 0) { fclose(f); return fail(AGR_EINVAL, "restore: not a snapshot"); }
-    agr_config c = *cfg;
-    if (c.flags == 0) c.flags = AGR_CFG_PERSISTENCE;
-    const uint32_t mode_bits = AGR_CFG_MINT_IDS | AGR_CFG_VARLEN | AGR_CFG_RING;
-    if ((c.flags & mode_bits) != (hd.flags & mode_bits)) { fclose(f); return fail(AGR_EINVAL, "restore: id mode / record form differ from the snapshot"); }
-    if (c.id_secret == 0) c.id_secret = hd.id_secret;
-    if (c.id_secret != hd.id_secret) { fclose(f); return fail(AGR_EINVAL, "restore: id_secret differs from the snapshot"); }
-    for (size_t k = 0; k < dh.size(); ++k)
-        if ((dh[k].cut.flags & mode_bits) != (hd.flags & mode_bits) || dh[k].cut.id_secret != hd.id_secret || dh[k].cut.slab_rows != hd.slab_rows) {
-            fclose(f);
-            return fail(AGR_EINVAL, "restore: " + files[k + 1] + " and its full file " + files[0] + " come from different engines");
-        }
-    agr_handle* h = nullptr;
-    int rc = agr_create(&c, &h);
-    if (rc < 0) { fclose(f); return rc; }
-    auto bail = [&](int r) { std::string keep = g_err; fclose(f); agr_destroy(h); g_err = keep; return r; };
-    auto fits = [&](const snap_header& s) -> int {
-        const bool snap_ring = (s.flags & AGR_CFG_RING) != 0;
-        if (!snap_ring && s.resp_used > h->resp_cap) return fail(AGR_ENOSPC, "restore: stored responses larger than resp_bytes");
-        if (snap_ring && s.resp_cap != h->resp_cap) return fail(AGR_EINVAL, "restore: a ring snapshot needs the same resp_bytes");
-        if (snap_ring && (s.flags & AGR_CFG_VARLEN) && s.vcap != h->vcap) return fail(AGR_EINVAL, "restore: a ring snapshot needs the same vslab_bytes");
-        if (snap_ring && s.slab_rows != h->cfg.slab_rows) return fail(AGR_EINVAL, "restore: a ring snapshot needs the same slab_rows (rows live at logical mod slab_rows)");
-        if ((!snap_ring && s.rows_used > h->cfg.slab_rows) || s.log_len[0] > h->d.log_cap || s.log_len[1] > h->d.log_cap || ((s.flags & AGR_CFG_VARLEN) && !snap_ring && s.vused > h->vcap))
-            return fail(AGR_ENOSPC, "restore: snapshot larger than the configured capacities");
-        return 0;
-    };
-    if ((rc = fits(hd)) < 0) return bail(rc);
-    for (const auto& d : dh) if ((rc = fits(d.cut)) < 0) return bail(rc);
-    if ((rc = restore_locked(h, f, hd, files, dh)) < 0) return bail(rc);
-    fclose(f);
-    *out = h;
-    return 0;
-}
-
 int agr_expire(agr_handle* h, uint64_t now, uint64_t ttl, uint64_t* expired) {
     if (!h) return fail(AGR_EINVAL, "NULL argument");
     HLock lk(h);
@@ -2697,375 +1399,6 @@ int agr_stats_get(agr_handle* h, agr_stats* out) {
     return 0;
 }
 
-// ------------------------------------------------------------------------------------------ K4 exchange
-static int nccl_load() {
-    if (g_nccl.lib) return 0;
-    void* lib = dlopen("libnccl.so.2", RTLD_NOW | RTLD_GLOBAL);
-    if (!lib) return fail(AGR_ECOMM, std::string("dlopen libnccl.so.2: ") + dlerror());
-#define SYM(field, name) *(void**)(&g_nccl.field) = dlsym(lib, name); if (!g_nccl.field) return fail(AGR_ECOMM, "libnccl.so.2 lacks " name)
-    SYM(GetUniqueId, "ncclGetUniqueId"); SYM(CommInitRank, "ncclCommInitRank"); SYM(CommDestroy, "ncclCommDestroy");
-    SYM(Send, "ncclSend"); SYM(Recv, "ncclRecv"); SYM(GroupStart, "ncclGroupStart"); SYM(GroupEnd, "ncclGroupEnd");
-    SYM(GetErrorString, "ncclGetErrorString");
-#undef SYM
-    g_nccl.lib = lib;
-    return 0;
-}
-#define NK(call) do { ncclResult_t r_ = (call); if (r_ != ncclSuccess) return fail(AGR_ECOMM, std::string(#call) + ": " + g_nccl.GetErrorString(r_)); } while (0)
-
-int agr_comm_unique_id(uint8_t out[128]) {
-    if (!out) return fail(AGR_EINVAL, "NULL argument");
-    TRY(nccl_load());
-    ncclUniqueId id;
-    NK(g_nccl.GetUniqueId(&id));
-    memcpy(out, id.internal, 128);
-    return 0;
-}
-
-static int exchange_setup(agr_handle* h, int rank, int world);
-int agr_comm_init(agr_handle* h, const uint8_t id[128], int rank, int world) {
-    if (!h || !id) return fail(AGR_EINVAL, "NULL argument");
-    if (world < 1 || world > 32 || rank < 0 || rank >= world) return fail(AGR_EINVAL, "bad rank / world (1..32 shards)");
-    TRY(nccl_load());
-    HLock lk(h);
-    CK(cudaSetDevice(h->device));
-    ncclUniqueId uid; memcpy(uid.internal, id, 128);
-    NK(g_nccl.CommInitRank(&h->comm, world, uid, rank));
-    return exchange_setup(h, rank, world);
-}
-
-// Everything agr_comm_init does besides the communicator: this shard's rank (minted ids carry it) and the exchange's scratch
-static int exchange_setup(agr_handle* h, int rank, int world) {
-    h->rank = rank; h->world = world;
-    h->d.shard_id = (uint32_t)rank;
-    if (h->d_k4cnt) return 0;                      // scratch of an earlier call (agr_debug_world may run more than once)
-    const size_t mb = h->cfg.max_batch;
-    TRY(dev_alloc(h, &h->d_stage, mb * sizeof(agr_outcome), false));   // outcomes before binning (records are binned in their slab rows)
-    TRY(dev_alloc(h, &h->d_send, mb * AGR_REC, false));
-    TRY(dev_alloc(h, &h->d_owner, mb, false));
-    h->d.xowner = h->d_owner;                      // K1 tells the rows K4 shipped away by it (AGR_CFGI_HOLES)
-    TRY(dev_alloc(h, &h->d_perm, mb, false));
-    h->k4_nwarps = (uint32_t)std::min<size_t>((size_t)h->sm_count * 32, std::max<size_t>(1, (mb + 1023) / 1024));
-    TRY(dev_alloc(h, &h->d_k4matrix, (size_t)h->k4_nwarps * 32, false));
-    TRY(dev_alloc(h, &h->d_k4cnt, (size_t)4 * 40, true));
-    TRY(dev_alloc(h, &h->d_xverd, 2 * mb, false));
-    TRY(dev_alloc(h, &h->d_vback, mb, false));
-    TRY(dev_alloc(h, &h->d_vout, mb, false));
-    // K2 over local + received outcomes: scratch for 2 * max_batch ops
-    TRY(dev_alloc(h, &h->d_outs, 2 * mb, false));
-    TRY(k2_scratch_alloc(h, 2 * mb));
-    CK(cudaStreamSynchronize(h->stream));
-    return 0;
-}
-
-// The first half of the exchanges, in three stages: find every item's owner (K4 count + scan: exchange_count), swap the per-peer
-// counts with one grouped send/recv (exchange_swap_counts), and lay out the owner-major send offsets and the source-major receive
-// offsets (exchange_layout).  `d_items` are the items on the device: the staging buffer (outcomes), or the slab rows the batch was
-// DMA'd into (records, in-place mode).
-static uint32_t* k4_gtotal(agr_handle* h) { return h->d_k4cnt; }
-static uint32_t* k4_goff(agr_handle* h) { return h->d_k4cnt + 40; }
-static uint32_t* k4_rcnt(agr_handle* h) { return h->d_k4cnt + 80; }
-static int exchange_count(agr_handle* h, uint8_t* d_items, uint32_t item_bytes, uint32_t agent_off, uint32_t n, bool inplace, exchange_plan& x) {
-    if (n > h->cfg.max_batch) return fail(AGR_EINVAL, "n exceeds max_batch");
-    x.G = (uint32_t)h->world; x.me = (uint32_t)h->rank;
-    agr_k4_params& p = x.p;
-    p.items = d_items; p.inplace = inplace ? 1u : 0u;
-    p.item_bytes = item_bytes; p.agent_off = agent_off; p.n = n; p.G = x.G; p.me = x.me;
-    // every warp takes a run of per_warp items (a multiple of 32); at most k4_nwarps warps (32 per SM)
-    uint32_t per = (n + h->k4_nwarps - 1) / std::max<uint32_t>(1, h->k4_nwarps);
-    per = std::max<uint32_t>(32, (per + 31) & ~31u);
-    p.per_warp = per; p.nwarps = std::max<uint32_t>(1, (n + per - 1) / per);
-    p.matrix = h->d_k4matrix; p.gtotal = k4_gtotal(h); p.goff = k4_goff(h); p.owner = h->d_owner; p.perm = h->d_perm;
-    agr_launch_k4_count(p, h->stream);
-    h->k4_launches += 2;
-    CK(cudaGetLastError());
-    return 0;
-}
-static int exchange_swap_counts(agr_handle* h, const exchange_plan& x) {
-    NK(g_nccl.GroupStart());
-    for (uint32_t q = 0; q < x.G; ++q) {
-        NK(g_nccl.Send(k4_gtotal(h) + q, 1, ncclUint32, (int)q, h->comm, h->stream));
-        NK(g_nccl.Recv(k4_rcnt(h) + q, 1, ncclUint32, (int)q, h->comm, h->stream));
-    }
-    NK(g_nccl.GroupEnd());
-    return 0;
-}
-static int exchange_layout(agr_handle* h, exchange_plan& x) {
-    const bool inplace = x.p.inplace != 0u;
-    const uint32_t n = x.p.n;
-    cudaStream_t st = h->stream;
-    // the one host round trip of the exchange: ncclSend / ncclRecv take their element counts from the host, and the rows for
-    // the records that arrive have to be reserved
-    uint32_t* hc = h->h_small;                       // [0..31] send counts, [32..63] receive counts
-    CK(cudaMemcpyAsync(hc, k4_gtotal(h), x.G * 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(hc + 32, k4_rcnt(h), x.G * 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    x.soff[0] = 0; x.roff[0] = 0;
-    for (uint32_t q = 0; q < x.G; ++q) {
-        x.scnt[q] = hc[q]; x.rcnt[q] = (q == x.me) ? 0 : hc[32 + q];
-        // in-place mode: the send buffer holds the peers' segments only
-        x.soff[q + 1] = x.soff[q] + ((inplace && q == x.me) ? 0u : x.scnt[q]); x.roff[q + 1] = x.roff[q] + x.rcnt[q];
-    }
-    x.n_local = x.scnt[x.me]; x.n_recv = x.roff[x.G];
-    x.recv_res_base = inplace ? n : x.n_local;
-    if ((inplace ? n : x.n_local) + x.n_recv > 2 * h->cfg.max_batch) return fail(AGR_ENOSPC, "received more items than 2 * max_batch");
-    return 0;
-}
-static int exchange_begin(agr_handle* h, uint8_t* d_items, uint32_t item_bytes, uint32_t agent_off, uint32_t n, bool inplace, exchange_plan& x) {
-    if (!h->comm) return fail(AGR_ECOMM, "agr_comm_init has not been called on this handle");
-    TRY(exchange_count(h, d_items, item_bytes, agent_off, n, inplace, x));
-    TRY(exchange_swap_counts(h, x));
-    return exchange_layout(h, x);
-}
-// the all-to-all itself: peer segments of `send` to their owners, landing at recv_base in source-rank order
-static int exchange_payload(agr_handle* h, const exchange_plan& x, const uint8_t* send, uint8_t* recv_base, size_t item_bytes) {
-    NK(g_nccl.GroupStart());
-    for (uint32_t q = 0; q < x.G; ++q) {
-        if (q == x.me) continue;
-        if (x.scnt[q]) NK(g_nccl.Send(send + (size_t)x.soff[q] * item_bytes, (size_t)x.scnt[q] * item_bytes, ncclUint8, (int)q, h->comm, h->stream));
-        if (x.rcnt[q]) NK(g_nccl.Recv(recv_base + (size_t)x.roff[q] * item_bytes, (size_t)x.rcnt[q] * item_bytes, ncclUint8, (int)q, h->comm, h->stream));
-    }
-    NK(g_nccl.GroupEnd());
-    return 0;
-}
-// results of the received items back to where they came from (owner-major at the reporter), then the caller's order
-static int exchange_unpermute(agr_handle* h, const exchange_plan& x, const uint8_t* res_all, const uint8_t* back, uint8_t* out_dev, uint32_t res_bytes);
-static int exchange_results(agr_handle* h, const exchange_plan& x, const uint8_t* res_all /*own items first, then received*/, uint8_t* back,
-                            uint8_t* out_dev, uint32_t res_bytes) {
-    NK(g_nccl.GroupStart());
-    for (uint32_t q = 0; q < x.G; ++q) {
-        if (q == x.me) continue;
-        if (x.rcnt[q]) NK(g_nccl.Send(res_all + (size_t)(x.recv_res_base + x.roff[q]) * res_bytes, (size_t)x.rcnt[q] * res_bytes, ncclUint8, (int)q, h->comm, h->stream));
-        if (x.scnt[q]) NK(g_nccl.Recv(back + (size_t)x.soff[q] * res_bytes, (size_t)x.scnt[q] * res_bytes, ncclUint8, (int)q, h->comm, h->stream));
-    }
-    NK(g_nccl.GroupEnd());
-    return exchange_unpermute(h, x, res_all, back, out_dev, res_bytes);
-}
-static int exchange_unpermute(agr_handle* h, const exchange_plan& x, const uint8_t* res_all, const uint8_t* back, uint8_t* out_dev, uint32_t res_bytes) {
-    if (x.p.n) {
-        agr_launch_k4_unpermute(x.p, res_all, back, out_dev, res_bytes, h->stream);
-        h->k4_launches += 1;
-        CK(cudaGetLastError());
-    }
-    return 0;
-}
-static void exchange_fill_info(const exchange_plan& x, uint32_t n, uint64_t first, uint64_t recv_first, agr_exchange_info* info) {
-    if (!info) return;
-    memset(info, 0, sizeof *info);
-    info->world = x.G; info->rank = x.me; info->n_local = x.n_local; info->n_sent = n - x.n_local; info->n_received = x.n_recv;
-    info->first_rid = first; info->recv_first_rid = recv_first;
-    for (uint32_t q = 0; q < x.G; ++q) { info->sent_to[q] = (q == x.me) ? 0 : x.scnt[q]; info->received_from[q] = x.rcnt[q]; }
-}
-
-// The exchange over a batch that already lies in slab rows [first, first + n) (DMA'd there by agr_ingest_sharded, or filled on
-// the device).  Records of this shard's agents never move: K4 only copies the records owned by a PEER into the send buffer and
-// K1 skips their rows; received records land in rows reserved behind the batch, straight from the all-to-all.
-// Its stages: K4 count + scan over the rows, then (after the counts are known) sharded_rows_local, the all-to-all of the records,
-// K1 over the received rows, the all-to-all of their verdicts, and sharded_rows_finish.  agr_debug_exchange_begin / _end run the
-// same stages with the test in place of the two all-to-alls.
-static uint8_t* batch_rows(agr_handle* h, uint64_t first) { return h->d.slab + phys_row(h, first) * AGR_REC; }
-// rows for the records that arrive, the peers' records packed for shipping, K1 over the batch's own rows (the rows of the records
-// K4 packed are holes: K1 skips them by K4's owner array, AGR_CFGI_HOLES) — runs while the all-to-all moves the peers' records
-static int sharded_rows_local(agr_handle* h, uint64_t first, exchange_plan& x, uint64_t* first2) {
-    const uint32_t n = x.p.n;
-    *first2 = h->rows_used;
-    if (x.n_recv) TRY(reserve_rows_locked(h, x.n_recv, first2));
-    const uint32_t n_remote = n - x.n_local;
-    x.p.local_dst = nullptr; x.p.send_dst = h->d_send;
-    if (n_remote) { agr_launch_k4_scatter(x.p, h->stream); h->k4_launches += 1; CK(cudaGetLastError()); }
-    if (n) {
-        const uint32_t keep = h->d.cfg_flags;
-        if (n_remote) h->d.cfg_flags |= AGR_CFGI_HOLES;
-        const int rc = launch_k1_locked(h, first, n, h->d_xverd);
-        h->d.cfg_flags = keep;
-        TRY(rc);
-    }
-    return 0;
-}
-// the verdicts in the caller's order (d_vout, after exchange_unpermute) to the host
-static int sharded_rows_finish(agr_handle* h, const exchange_plan& x, uint64_t first, uint64_t first2, agr_verdict* out, agr_exchange_info* info) {
-    const uint32_t n = x.p.n;
-    if (n && out) CK(cudaMemcpyAsync(h->h_verdicts, h->d_vout, (size_t)n * sizeof(agr_verdict), cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    if (n && out) memcpy(out, h->h_verdicts, (size_t)n * sizeof(agr_verdict));
-    exchange_fill_info(x, n, first, first2, info);
-    return 0;
-}
-static int sharded_rows_locked(agr_handle* h, uint64_t first, uint32_t n, agr_verdict* out, agr_exchange_info* info) {
-    exchange_plan x;
-    TRY(exchange_begin(h, batch_rows(h, first), AGR_REC, AGR_OFF_AGENT_ID, n, true, x));
-    uint64_t first2 = 0;
-    TRY(sharded_rows_local(h, first, x, &first2));
-    // the all-to-all: every peer segment to its owner, landing directly in the owner's slab rows
-    TRY(exchange_payload(h, x, h->d_send, batch_rows(h, first2), AGR_REC));
-    // K1 at the owner over the received rows (own host's records first, then peers by rank: the merge order)
-    if (x.n_recv) TRY(launch_k1_locked(h, first2, x.n_recv, h->d_xverd + n));
-    // verdicts back to where the records came from, restored to the caller's order
-    TRY(exchange_results(h, x, (const uint8_t*)h->d_xverd, (uint8_t*)h->d_vback, (uint8_t*)h->d_vout, sizeof(agr_verdict)));
-    return sharded_rows_finish(h, x, first, first2, out, info);
-}
-
-int agr_ingest_sharded(agr_handle* h, const agr_record* recs, uint32_t n, agr_verdict* out, agr_exchange_info* info) {
-    if (!h || (n && !recs)) return fail(AGR_EINVAL, "NULL argument");
-    HLock lk(h);
-    CK(cudaSetDevice(h->device));
-    if (!h->comm) return fail(AGR_ECOMM, "agr_comm_init has not been called on this handle");
-    if (n > h->cfg.max_batch) return fail(AGR_EINVAL, "n exceeds max_batch");
-    uint64_t first = h->rows_used;
-    if (n) {
-        TRY(reserve_rows_locked(h, n, &first));
-        // the batch goes STRAIGHT into its slab rows, on the copy stream
-        while (h->chunk_ev.size() < 2) { cudaEvent_t e; CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming)); h->chunk_ev.push_back(e); }
-        CK(cudaEventRecord(h->chunk_ev[0], h->stream));
-        CK(cudaStreamWaitEvent(h->copy_stream, h->chunk_ev[0], 0));
-        int bk = 0;
-        TRY(upload_rows(h, batch_rows(h, first), (const uint8_t*)recs, (size_t)n * AGR_REC, is_pinned(recs), bk));
-        CK(cudaEventRecord(h->chunk_ev[1], h->copy_stream));
-        CK(cudaStreamWaitEvent(h->stream, h->chunk_ev[1], 0));
-    }
-    return sharded_rows_locked(h, first, n, out, info);
-}
-// The same over rows the caller reserved (agr_reserve_rows) and filled on the device: the exchange with the batch resident in HBM.
-int agr_ingest_sharded_rows(agr_handle* h, uint64_t first_rid, uint32_t n, agr_verdict* out, agr_exchange_info* info) {
-    if (!h) return fail(AGR_EINVAL, "NULL handle");
-    HLock lk(h);
-    CK(cudaSetDevice(h->device));
-    if (!h->comm) return fail(AGR_ECOMM, "agr_comm_init has not been called on this handle");
-    if (first_rid + n > h->rows_used) return fail(AGR_EINVAL, "rows not reserved");
-    if (n > h->cfg.max_batch) return fail(AGR_EINVAL, "n exceeds max_batch");
-    if (!h->resv.empty()) resv_remove(h, first_rid, first_rid + n);
-    return sharded_rows_locked(h, first_rid, n, out, info);
-}
-
-int agr_complete_sharded(agr_handle* h, const agr_outcome* outs, uint32_t n, int32_t* results, agr_exchange_info* info) {
-    if (!h || (n && !outs)) return fail(AGR_EINVAL, "NULL argument");
-    HLock lk(h);
-    CK(cudaSetDevice(h->device));
-    exchange_plan x;
-    if (!h->comm) return fail(AGR_ECOMM, "agr_comm_init has not been called on this handle");
-    if (n > h->cfg.max_batch) return fail(AGR_EINVAL, "n exceeds max_batch");
-    if (n) CK(cudaMemcpyAsync(h->d_stage, outs, (size_t)n * sizeof(agr_outcome), cudaMemcpyHostToDevice, h->stream));
-    TRY(exchange_begin(h, h->d_stage, sizeof(agr_outcome), 16, n, false, x));
-    const uint32_t total = x.n_local + x.n_recv;
-    // pack: own outcomes straight into the K2 input array, peer segments into the send buffer
-    x.p.local_dst = (uint8_t*)h->d_outs; x.p.send_dst = h->d_send;
-    if (n) { agr_launch_k4_scatter(x.p, h->stream); h->k4_launches += 1; CK(cudaGetLastError()); }
-    TRY(exchange_payload(h, x, h->d_send, (uint8_t*)(h->d_outs + x.n_local), sizeof(agr_outcome)));
-    // K2 at the owner over local + received outcomes (own host first, then peers by rank)
-    if (total) {
-        sync_window(h);
-        agr_launch_k2(h->d, h->d_outs, h->k2, total, h->stream);
-        h->k2_launches += 3;
-        CK(cudaGetLastError());
-    }
-    TRY(exchange_results(h, x, (const uint8_t*)h->k2.results, (uint8_t*)h->d_vback, (uint8_t*)h->d_vout, 4));
-    if (n && results) CK(cudaMemcpyAsync(h->h_results, h->d_vout, (size_t)n * 4, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    if (n && results) memcpy(results, h->h_results, (size_t)n * 4);
-    exchange_fill_info(x, n, 0, 0, info);
-    return 0;
-}
-
-// ------------------------------------------------------------------ test-only stages of the exchange (no communicator)
-int agr_debug_world(agr_handle* h, int rank, int world) {
-    if (!h) return fail(AGR_EINVAL, "NULL argument");
-    if (world < 1 || world > 32 || rank < 0 || rank >= world) return fail(AGR_EINVAL, "bad rank / world (1..32 shards)");
-    HLock lk(h);
-    CK(cudaSetDevice(h->device));
-    if (h->comm) return fail(AGR_EINVAL, "the handle has a communicator (agr_comm_init)");
-    if (h->xdbg_open) return fail(AGR_EINVAL, "an agr_debug_exchange_begin is waiting for its agr_debug_exchange_end");
-    return exchange_setup(h, rank, world);
-}
-
-namespace {
-struct dbg_dev_buf {                     // device scratch of one agr_debug_k4 call
-    void* p = nullptr;
-    ~dbg_dev_buf() { if (p) cudaFree(p); }
-};
-}
-int agr_debug_k4(agr_handle* h, const void* items, uint32_t n, uint32_t item_bytes, uint32_t agent_off, int inplace,
-                 const void* local_res, const void* remote_res, uint32_t res_bytes, uint8_t* owner, uint32_t* perm, uint32_t* gtotal,
-                 uint32_t* goff, void* send_out, void* local_out, void* items_out, void* res_out) {
-    if (!h || (n && (!items || !local_res || !remote_res || !owner || !perm || !send_out || !local_out || !items_out || !res_out)) || !gtotal || !goff)
-        return fail(AGR_EINVAL, "NULL argument");
-    if (item_bytes < 48 || item_bytes > AGR_REC || item_bytes % 16 || agent_off % 16 || agent_off + 32 > item_bytes)
-        return fail(AGR_EINVAL, "items are 48..512 B, a multiple of 16, with the 32 B agent id 16 B aligned inside");
-    if (res_bytes != 4 && res_bytes != 8) return fail(AGR_EINVAL, "results are 4 or 8 B");
-    HLock lk(h);
-    CK(cudaSetDevice(h->device));
-    if (!h->d_k4cnt) return fail(AGR_ECOMM, "neither agr_comm_init nor agr_debug_world has been called on this handle");
-    if (n > h->cfg.max_batch) return fail(AGR_EINVAL, "n exceeds max_batch");
-    const size_t ib = (size_t)std::max<uint32_t>(n, 1) * item_bytes, rb = (size_t)std::max<uint32_t>(n, 1) * res_bytes;
-    dbg_dev_buf d_items, d_local, d_lres, d_rres, d_out;
-    CK(cudaMalloc(&d_items.p, ib)); CK(cudaMalloc(&d_local.p, ib));
-    CK(cudaMalloc(&d_lres.p, rb)); CK(cudaMalloc(&d_rres.p, rb)); CK(cudaMalloc(&d_out.p, rb));
-    cudaStream_t st = h->stream;
-    CK(cudaMemsetAsync(d_local.p, 0, ib, st));
-    CK(cudaMemsetAsync(h->d_send, 0, ib, st));
-    CK(cudaMemsetAsync(d_out.p, 0, rb, st));
-    if (n) {
-        CK(cudaMemcpyAsync(d_items.p, items, (size_t)n * item_bytes, cudaMemcpyHostToDevice, st));
-        CK(cudaMemcpyAsync(d_lres.p, local_res, (size_t)n * res_bytes, cudaMemcpyHostToDevice, st));
-        CK(cudaMemcpyAsync(d_rres.p, remote_res, (size_t)n * res_bytes, cudaMemcpyHostToDevice, st));
-    }
-    exchange_plan x;
-    TRY(exchange_count(h, (uint8_t*)d_items.p, item_bytes, agent_off, n, inplace != 0, x));
-    CK(cudaMemsetAsync(k4_rcnt(h), 0, 32 * sizeof(uint32_t), st));        // nothing received
-    TRY(exchange_layout(h, x));
-    x.p.local_dst = (uint8_t*)d_local.p; x.p.send_dst = h->d_send;
-    agr_launch_k4_scatter(x.p, st); h->k4_launches += 1;
-    CK(cudaGetLastError());
-    TRY(exchange_unpermute(h, x, (const uint8_t*)d_lres.p, (const uint8_t*)d_rres.p, (uint8_t*)d_out.p, res_bytes));
-    CK(cudaMemcpyAsync(gtotal, k4_gtotal(h), x.G * 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(goff, k4_goff(h), (x.G + 1) * 4, cudaMemcpyDeviceToHost, st));
-    if (n) {
-        CK(cudaMemcpyAsync(owner, h->d_owner, n, cudaMemcpyDeviceToHost, st));
-        CK(cudaMemcpyAsync(perm, h->d_perm, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
-        CK(cudaMemcpyAsync(send_out, h->d_send, (size_t)n * item_bytes, cudaMemcpyDeviceToHost, st));
-        CK(cudaMemcpyAsync(local_out, d_local.p, (size_t)n * item_bytes, cudaMemcpyDeviceToHost, st));
-        CK(cudaMemcpyAsync(items_out, d_items.p, (size_t)n * item_bytes, cudaMemcpyDeviceToHost, st));
-        CK(cudaMemcpyAsync(res_out, d_out.p, (size_t)n * res_bytes, cudaMemcpyDeviceToHost, st));
-    }
-    CK(cudaStreamSynchronize(st));
-    return 0;
-}
-
-int agr_debug_exchange_begin(agr_handle* h, uint64_t first_rid, uint32_t n, agr_record* send_out, agr_exchange_info* info) {
-    if (!h || (n && !send_out)) return fail(AGR_EINVAL, "NULL argument");
-    HLock lk(h);
-    CK(cudaSetDevice(h->device));
-    if (!h->d_k4cnt || h->comm) return fail(AGR_EINVAL, "agr_debug_world has not been called on this handle");
-    if (h->xdbg_open) return fail(AGR_EINVAL, "an agr_debug_exchange_begin is waiting for its agr_debug_exchange_end");
-    if (first_rid + n > h->rows_used) return fail(AGR_EINVAL, "rows not reserved");
-    if (!h->resv.empty()) resv_remove(h, first_rid, first_rid + n);
-    exchange_plan& x = h->xdbg;
-    x = exchange_plan{};
-    TRY(exchange_count(h, batch_rows(h, first_rid), AGR_REC, AGR_OFF_AGENT_ID, n, true, x));
-    CK(cudaMemsetAsync(k4_rcnt(h), 0, 32 * sizeof(uint32_t), h->stream));   // the peers' records arrive through agr_ingest_rows instead
-    TRY(exchange_layout(h, x));
-    uint64_t first2 = 0;
-    TRY(sharded_rows_local(h, first_rid, x, &first2));
-    const uint32_t n_sent = n - x.n_local;
-    if (n_sent) CK(cudaMemcpyAsync(send_out, h->d_send, (size_t)n_sent * AGR_REC, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    exchange_fill_info(x, n, first_rid, first2, info);
-    h->xdbg_first = first_rid; h->xdbg_n = n; h->xdbg_open = true;
-    return 0;
-}
-
-int agr_debug_exchange_end(agr_handle* h, const agr_verdict* back, agr_verdict* out) {
-    if (!h) return fail(AGR_EINVAL, "NULL argument");
-    HLock lk(h);
-    CK(cudaSetDevice(h->device));
-    if (!h->xdbg_open) return fail(AGR_EINVAL, "no agr_debug_exchange_begin to end");
-    const exchange_plan& x = h->xdbg;
-    const uint32_t n = h->xdbg_n, n_sent = n - x.n_local;
-    if ((n_sent && !back) || (n && !out)) return fail(AGR_EINVAL, "NULL argument");
-    h->xdbg_open = false;
-    if (n_sent) CK(cudaMemcpyAsync(h->d_vback, back, (size_t)n_sent * sizeof(agr_verdict), cudaMemcpyHostToDevice, h->stream));
-    TRY(exchange_unpermute(h, x, (const uint8_t*)h->d_xverd, (const uint8_t*)h->d_vback, (uint8_t*)h->d_vout, sizeof(agr_verdict)));
-    return sharded_rows_finish(h, x, h->xdbg_first, h->rows_used, out, nullptr);
-}
-
 int agr_debug_read(agr_handle* h, int which, uint64_t first_rid, uint32_t n, void* out) {
     if (!h || (n && !out)) return fail(AGR_EINVAL, "NULL argument");
     HLock lk(h);
@@ -3130,7 +1463,7 @@ int agr_debug_skip_arrivals(agr_handle* h, uint64_t n) {
     h->scan_lo = h->tail; h->sweep_clean = h->rows_used; h->reclaim_bound = h->tail;
     h->d.idx_base = h->tail;
     sync_window(h);                                          // agr_dev's window, and rows_out for the single-request callers
-    CK(cudaMemsetAsync(h->d.cmin, 0, (size_t)(h->cfg.slab_rows / AGR_CHUNK_ROWS + 2) * 8, h->stream));
+    TRY(chunk_bounds_unknown(h));
     CK(cudaStreamSynchronize(h->stream));
     return 0;
 }

@@ -1,7 +1,7 @@
 // agr_ring.hpp — the CALLERS' side of the single-request ring (AGR_CFG_COMBINE; layout and protocol: agr_svc.h).
 //
 // Everything a calling thread does to hand one operation over and to collect its answer, as templates over the host-side ring
-// object H (agr_engine.cu's svc_host; the stand-ins of tests/ring_sim.cpp, tests/ring_sim_bytes.cpp and tests/ring_sim_span.cpp).
+// object H (agr_engine.h's svc_host; the stand-ins of tests/ring_sim.cpp, tests/ring_sim_bytes.cpp and tests/ring_sim_span.cpp).
 // H provides:
 //   svc_res* res; uint8_t* payload; std::atomic<uint32_t>* ready;          pinned, device-mapped in the engine
 //   std::atomic<uint64_t> head, scanned; std::atomic<uint32_t> waiters; uint32_t spin_cpus;

@@ -1,5 +1,5 @@
 // agr_svc.h — the single-request front end (AGR_CFG_COMBINE): shared layout of the pinned op ring between the calling
-// threads, the dispatcher thread (agr_engine.cu) and the service kernel (agr_svc.cu).
+// threads, the dispatcher thread (agr_front.cu) and the service kernel (agr_svc.cu).
 //
 // The reference serves one goroutine per HTTP request (net/http accept loop -> proxyToAgentHandler, server.go:493-573), so
 // the call pattern at the boundary is "many OS threads, ONE request per call": agr_ingest_ex(n = 1) then agr_complete(n = 1).

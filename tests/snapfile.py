@@ -1,4 +1,4 @@
-"""Plain reader of the two snapshot file formats of csrc/agr_engine.cu: a full file (AGRSNAP3) and a delta (AGRDELT1), and
+"""Plain reader of the two snapshot file formats of csrc/agr_snapshot.cu: a full file (AGRSNAP3) and a delta (AGRDELT1), and
 what a delta should hold given the full files of its parent's cut and of its own.  Needs no GPU."""
 import numpy as np
 
@@ -7,13 +7,13 @@ from agentainer_lab_b200 import constants as K
 R, V = K.AGR_CFG_RING, K.AGR_CFG_VARLEN
 BLOCK_ROWS, LOG_BLOCK = 256, 1024
 
-# mirrors struct snap_header in csrc/agr_engine.cu
+# mirrors struct snap_header in csrc/agr_engine.h
 HEADER = np.dtype([("magic", "S8"), ("flags", "<u4"), ("n_agents", "<u4"), ("shard", "<u4"), ("gen", "<u4"),
                    ("rows_used", "<u8"), ("vused", "<u8"), ("log_len", "<u8", (2,)), ("id_secret", "<u8"), ("scan_lo", "<u8"),
                    ("resp_used", "<u8"), ("expired_total", "<u8"), ("tail", "<u8"), ("released_total", "<u8"), ("slab_rows", "<u8"),
                    ("vtail", "<u8"), ("vcap", "<u8"), ("resp_tail", "<u8"), ("resp_cap", "<u8")])
 WORDS = ("state", "route", "aux", "cksum", "voff", "vlen", "resp_off", "resp_len", "resp_hlen", "err_off", "err_len", "ptime", "mtime")
-# mirrors struct delta_header in csrc/agr_engine.cu
+# mirrors struct delta_header in csrc/agr_snapshot.cu
 DELTA = np.dtype([("magic", "S8"), ("cut", HEADER), ("file_bytes", "<u8"), ("parent_digest", "<u8", (2,)), ("digest", "<u8", (2,)),
                   ("block_rows", "<u4"), ("log_block", "<u4"), ("rows_lo", "<u8"), ("rows_hi", "<u8"), ("resp_lo", "<u8"),
                   ("resp_hi", "<u8"), ("n_blocks", "<u8"), ("n_log_blocks", "<u8", (2,)), ("parent_path_len", "<u4"), ("pad", "<u4")])
