@@ -2,8 +2,6 @@
 parity with the (size-agnostic) Python oracle, stored bytes round trip, checksum, tile-ownership edge cases."""
 import dataclasses
 
-import os
-
 import numpy as np
 import pytest
 
@@ -15,14 +13,14 @@ from scenario import run_oracle, run_engine, assert_same, random_scenario, Req, 
 pytestmark = pytest.mark.gpu
 GOLD, _ = load_golden()
 VAR = K.AGR_CFG_PERSISTENCE | K.AGR_CFG_VARLEN
+FORMS = {"staged": 0, "lsu": 0x20}      # k1_variant: K1v through per-warp TMA stages / its LSU form (bit 0x20)
 
 
-def engine(flags=VAR, **kw):
+def engine(flags=VAR, form="staged", **kw):
     kw.setdefault("slab_rows", 1 << 15)
     kw.setdefault("max_agents", 256)
     kw.setdefault("vslab_bytes", 256 << 20)
-    kw.setdefault("k1_variant", int(os.environ.get("AGR_TEST_K1_VARIANT", "0"), 0))   # e.g. 0x20: the LSU form of K1v
-    return A.Engine(flags=flags, **kw)
+    return A.Engine(flags=flags, k1_variant=FORMS[form], **kw)
 
 
 def with_bodies(events, seed):
@@ -40,9 +38,10 @@ def with_bodies(events, seed):
 
 @pytest.mark.parametrize("kat", sorted(SCENARIOS))
 @pytest.mark.parametrize("flags", [VAR, VAR | K.AGR_CFG_MINT_IDS])
-def test_kats_variable_length(kat, flags):
+@pytest.mark.parametrize("form", FORMS)
+def test_kats_variable_length(form, kat, flags):
     ev = with_bodies(SCENARIOS[kat], 1)
-    with engine(flags) as eng:
+    with engine(flags, form) as eng:
         got = run_engine(eng, ev)
     exp = GOLD[kat]
     assert got.verdicts == exp["verdicts"] and got.ticks == exp["ticks"] and got.records == exp["records"]
@@ -51,16 +50,23 @@ def test_kats_variable_length(kat, flags):
 
 
 @pytest.mark.parametrize("seed", range(6))
-def test_random_streams_variable_length(seed):
+@pytest.mark.parametrize("form", FORMS)
+def test_random_streams_variable_length(form, seed):
     ev = with_bodies(random_scenario(300 + seed, n_events=500, n_agents=2 + seed % 5, p_replay=0.15), seed)
     ref = run_oracle(ev)
-    with engine(VAR | (K.AGR_CFG_MINT_IDS if seed % 2 else 0)) as eng:
+    with engine(VAR | (K.AGR_CFG_MINT_IDS if seed % 2 else 0), form) as eng:
         assert_same(ref, run_engine(eng, ev, rng=np.random.default_rng(seed)))
 
 
 def test_stored_bytes_checksum_and_tile_edges():
     """Record sizes chosen to hit the byte-tile machinery: records that end exactly on an 8 KiB tile boundary, the
-    longest legal record (8192 B), runs of minimum-size records (96 B header + 16 B), tiles in which no record starts."""
+    longest legal record (8192 B), runs of minimum-size records (96 B header + 16 B), tiles in which no record starts.
+    Both forms of K1v, one after the other."""
+    for form in FORMS:
+        stored_bytes_checksum_and_tile_edges(form)
+
+
+def stored_bytes_checksum_and_tile_edges(form):
     sizes = [8192 - 96 - 48] * 3 + [16] * 200 + [4000, 8192 - 96 - 48, 16, 8192 - 96 - 48, 8192 - 96 - 48] + [100, 3000, 5, 0, 777] * 40
     rng = np.random.default_rng(3)
     reqs = []
@@ -71,7 +77,7 @@ def test_stored_bytes_checksum_and_tile_edges():
     blob, offs = make_var_batch(reqs)
     lens = np.diff(offs)
     assert lens.max() <= K.AGR_VAR_MAX_RECORD and (lens % 16 == 0).all()
-    with engine(slab_rows=1 << 12) as eng:
+    with engine(form=form, slab_rows=1 << 12) as eng:
         eng.set_agent_state("agent-1", "stopped"); eng.set_agent_state("agent-2", "running")
         # two batches: the second starts at an arbitrary (16 B aligned) slab offset
         cut = 150
