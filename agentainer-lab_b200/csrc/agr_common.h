@@ -68,7 +68,6 @@ AGR_HD uint32_t rt_flags(uint32_t r) { return r >> RT_FLAG_SHIFT; }
 #define AUX_ERR_SHIFT 16
 
 #define AGR_RID_NONE 0xffffffffu
-#define AGR_CFGI_SPLIT_INDEX 0x10000u   // internal cfg_flags bit: K1 runs as stream kernel + k1_index kernel
 #define AGR_CFGI_HOLES 0x20000u         // internal cfg_flags bit (set per launch by the exchange path): rows of the batch that K4
                                         // shipped to their owner shard (agr_dev::xowner) are skipped
 

@@ -1,4 +1,4 @@
-// agr_device.cuh — device helpers shared by the K1 variants and K2/K3: cache-hinted loads, the 128-bit CAS, the
+// agr_device.cuh — device helpers shared by the K1 kernels and K2/K3: cache-hinted loads, the 128-bit CAS, the
 // agent-table and dedupe-index probes, and the per-record decision of proxyToAgentHandler + StoreRequest.
 #pragma once
 #include "agr_kernels.cuh"
@@ -157,9 +157,8 @@ __device__ __forceinline__ void k1_begin(const agr_dev& d, const ag_probe& ap, c
     const bool found = c.slot != RT_SLOT_NONE && c.astatus != AG_STATUS_REMOVED;
     c.want_store = found && (d.cfg_flags & AGR_CFG_PERSISTENCE) && !c.replay && !c.hole;  // server.go:508
     c.bad = c.want_store && ((unsigned long long)(h4.w & 0xffffu) + (h4.w >> 16) + body_len > payload_cap);
-    // split mode: the insert is done by k1_index after the stream kernel; the row is provisionally "stored"
     // mint mode: the id is a function of the row, nothing to insert; the caller's request_id is ignored
-    c.deferred = c.want_store && !c.bad && ((d.cfg_flags & AGR_CFG_MINT_IDS) || ((c.id_lo | c.id_hi) != 0ULL && (d.cfg_flags & AGR_CFGI_SPLIT_INDEX)));
+    c.deferred = c.want_store && !c.bad && (d.cfg_flags & AGR_CFG_MINT_IDS);
     c.cas_issued = c.want_store && !c.bad && (c.id_lo | c.id_hi) != 0ULL && !c.deferred && !(d.cfg_flags & AGR_CFG_DIAG_NO_INDEX);
     c.old = 0;
     c.tidx = 0;

@@ -167,7 +167,8 @@ static int create_impl(const agr_config* cfg_in, agr_handle* h) {
         if (c.max_batch == 0) return fail(AGR_EINVAL, "AGR_CFG_RING: slab_rows too small");
     }
     if (c.log_entries == 0) c.log_entries = c.slab_rows * 3;   // a replayed request pushes twice (Q7), plus once per earlier retry
-    if ((c.k1_variant & 0xfu) == 0) c.k1_variant |= 4u;      // default K1 shape: TMA, 14 warps x 1 stage, fused index
+    if (c.k1_variant & ~(0x20u | 0xff0000u))
+        return fail(AGR_EINVAL, "k1_variant: only bit 0x20 (K1v form) and bits 16..23 (timing stride) are defined; the A/B alternates of the fixed-stride K1 were retired");
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return fail(AGR_ENODEV, "no CUDA device visible (this library has no CPU fallback)"); }
     int dev = c.device;
@@ -243,10 +244,9 @@ static int create_impl(const agr_config* cfg_in, agr_handle* h) {
     }
     h->cfg.id_secret = d.id_secret;
     d.shard_id = 0; d.id_gen = 1; d.tail = 0; d.head_l = 0; d.ring_rows = 0; d.tail_phys = 0; d.idx_base = 0;
-    if (!varlen && (c.k1_variant & 0xfu) != AGR_K1_LSU && agr_k1_tma_make_map(d.slab, c.slab_rows, h->tmap) != 0)
+    if (!varlen && agr_k1_tma_make_map(d.slab, c.slab_rows, h->tmap) != 0)
         return fail(AGR_ECUDA, "cuTensorMapEncodeTiled failed for the slab");
     d.cfg_flags = c.flags & 0xffffu;
-    if (c.k1_variant & 0x10u) d.cfg_flags |= AGR_CFGI_SPLIT_INDEX;
     // staging
     h->bounce_bytes = std::min<size_t>((size_t)c.max_batch * AGR_REC, (size_t)32 << 20);
     for (int k = 0; k < 2; ++k) {
@@ -511,8 +511,7 @@ int launch_k1_locked(agr_handle* h, uint64_t first, uint32_t n, agr_verdict* d_o
     // is a stream operation of its own between two kernels, and two of them per step cost a back-to-back loop a few microseconds
     const uint32_t tstride = std::max<uint32_t>(1u, (h->cfg.k1_variant >> 16) & 0xffu);
     if ((h->cfg.flags & AGR_CFG_TIMING) && (h->timing_calls++ % tstride) == 0) TRY(claim_k1_events(h, &e0, &e1));
-    h->k1_launches += agr_launch_k1(h->d, (uint32_t)phys_row(h, first), first, n, h->cfg.k1_variant,
-                                    (h->cfg.k1_variant & 0xfu) != AGR_K1_LSU ? h->tmap : nullptr, h->sm_count, h->stream, e0, e1, d_out, d_ids);
+    h->k1_launches += agr_launch_k1(h->d, (uint32_t)phys_row(h, first), first, n, h->tmap, h->sm_count, h->stream, e0, e1, d_out, d_ids);
     CK(cudaGetLastError());
     return 0;
 }

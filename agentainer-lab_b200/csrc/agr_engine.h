@@ -144,7 +144,7 @@ struct agr_handle {
     uint64_t k1_launches = 0, k2_launches = 0, k3_launches = 0, k4_launches = 0;
     uint64_t replay_scans = 0, replay_dispatched = 0;
     std::vector<void*> dev_allocs, host_allocs;
-    alignas(64) unsigned char tmap[128];       // CUtensorMap of the slab for the TMA K1 variants
+    alignas(64) unsigned char tmap[128];       // CUtensorMap of the slab for the fixed-stride TMA K1
     // stored responses: byte slab + per-row (offset, length), written off the hot path
     uint8_t* d_resp = nullptr; uint64_t resp_used = 0, resp_cap = 0;   // bytes appended so far (ring: logical, pads included) / capacity
     uint64_t resp_tail = 0;                    // ring: logical offset of the oldest byte a live row still refers to

@@ -5,8 +5,8 @@
 // position c ^ (r & 7) of its 128 B line, so when lane r walks ITS OWN record chunk by chunk, the eight lanes of a
 // quarter-warp hit eight different 16 B bank groups — thread-per-record parsing without bank conflicts and without
 // a single LSU global load for the record stream (the SM's LSU only sees the index / state traffic).
-// Every warp runs its own mbarrier pipeline (STAGES tiles deep) over tiles handed out by a global counter;
-// CTAs are persistent (one per SM), so the grid is exactly the SM count.
+// Every warp runs its own one-stage mbarrier pipeline over a static schedule of tiles; CTAs are persistent (one per SM,
+// 14 warps each), so the grid is exactly the SM count.
 #include <cuda.h>
 
 #include "agr_device.cuh"
@@ -35,10 +35,6 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
         "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
         ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1) : "memory");
 }
-// L2 prefetch of a box: starts the DRAM fetch without occupying shared memory (latency hiding beyond the smem ring)
-__device__ __forceinline__ void tma_prefetch_2d(const CUtensorMap* map, int32_t c0, int32_t c1) {
-    asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];" ::"l"(map), "r"(c0), "r"(c1) : "memory");
-}
 __device__ __forceinline__ uint4 lds128(uint32_t addr) {
     uint4 v;
     asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
@@ -48,18 +44,18 @@ __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefe
 
 // MINT: the engine mints ids (AGR_CFG_MINT_IDS), so k1_begin decides every replay's dedupe hit; the hash-id instantiation carries
 // none of that code (the index CAS loop is latency-bound, and the larger loop body cost it ~1.6 us a C2 step on H100).
-template <int WARPS, int STAGES, bool MINT>
+template <int WARPS, bool MINT>
 __global__ void __launch_bounds__(WARPS * 32, 1)
 k1_ingest_tma(const __grid_constant__ CUtensorMap tmap, const agr_dev d, const uint32_t first_rid, const unsigned long long first_log,
-              const uint32_t n, const uint32_t pf_dist) {
+              const uint32_t n) {
     extern __shared__ uint8_t smem_raw[];
-    __shared__ uint64_t bars[WARPS * STAGES];
+    __shared__ uint64_t bars[WARPS];
     __shared__ uint32_t s_ctr[K1_NLC];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     // 128 B swizzle needs 1024 B aligned tiles
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     if (threadIdx.x < K1_NLC) s_ctr[threadIdx.x] = 0;
-    if (threadIdx.x < WARPS * STAGES) mbar_init(smem_u32(&bars[threadIdx.x]), 1);
+    if (threadIdx.x < WARPS) mbar_init(smem_u32(&bars[threadIdx.x]), 1);
     if (threadIdx.x == 0) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap) : "memory");
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     __syncthreads();
@@ -73,49 +69,26 @@ k1_ingest_tma(const __grid_constant__ CUtensorMap tmap, const agr_dev d, const u
 #pragma unroll
     for (int c = 0; c <= K1_NLC; ++c) lc[c] = 0;
     const uint32_t tiles = (n + TILE_RECS - 1) / TILE_RECS;
-    const uint32_t my_smem = smem_base + (uint32_t)warp * STAGES * TILE_BYTES;
-    const uint32_t my_bar = smem_u32(&bars[warp * STAGES]);
+    const uint32_t my_smem = smem_base + (uint32_t)warp * TILE_BYTES;
+    const uint32_t bar = smem_u32(&bars[warp]);
 
-    uint32_t tile_of[STAGES];
-    // prologue: claim and issue STAGES tiles
+    // static schedule: tile = warp's global index + k * total warps (no atomics on the refill path)
+    uint32_t tile = blockIdx.x * WARPS + warp;
+    // prologue: issue the first tile
+    if (lane == 0 && tile < tiles) {
+        mbar_expect_tx(bar, TILE_BYTES);
 #pragma unroll
-    for (int s = 0; s < STAGES; ++s) {
-        // static schedule: tile = warp's global index + k * total warps (no atomics on the refill path)
-        const uint32_t t = (blockIdx.x * WARPS + warp) + (uint32_t)s * (gridDim.x * WARPS);
-        tile_of[s] = t;
-        if (lane == 0 && t < tiles) {
-            const uint32_t bar = my_bar + s * 8, dst = my_smem + s * TILE_BYTES;
-            mbar_expect_tx(bar, TILE_BYTES);
-#pragma unroll
-            for (int cb = 0; cb < 4; ++cb) tma_load_2d(dst + cb * 4096, &tmap, bar, cb * 128, (int32_t)(first_rid + t * TILE_RECS));
-        }
-    }
-    const uint32_t tstride = gridDim.x * WARPS;
-    // L2 prefetch window: the pf_dist tiles this warp will load after the ones already in flight
-    if (lane < 4) {
-        for (uint32_t k = 0; k < pf_dist; ++k) {
-            const uint32_t t = (blockIdx.x * WARPS + warp) + (STAGES + k) * tstride;
-            if (t < tiles) tma_prefetch_2d(&tmap, lane * 128, (int32_t)(first_rid + t * TILE_RECS));
-        }
+        for (int cb = 0; cb < 4; ++cb) tma_load_2d(my_smem + cb * 4096, &tmap, bar, cb * 128, (int32_t)(first_rid + tile * TILE_RECS));
     }
     // per-lane swizzled chunk offsets inside a [32][128 B] box: row * 128 + ((c ^ (row & 7)) << 4)
     const uint32_t rowoff = (uint32_t)lane * 128u;
     const uint32_t sw = ((uint32_t)lane & 7u) << 4;
+    const uint32_t base = my_smem + rowoff;
     uint32_t phase = 0;
     // software pipeline across tiles: the index CAS of tile t is issued in the middle of tile t and consumed in the
     // middle of tile t+1 (k1_finish), so its whole round trip hides behind a tile of checksum work
     k1_ctx pcx; uint4 ph1 = make_uint4(0, 0, 0, 0); uint32_t ph5y = 0, prid = 0, ptile = 0; bool pvalid = false;
-    for (uint32_t it = 0;; ++it) {
-        const int s = (STAGES == 1) ? 0 : (int)(it % STAGES);
-        uint32_t tile;
-        if (STAGES == 1) tile = tile_of[0];
-        else {
-            tile = tile_of[0];
-#pragma unroll
-            for (int q = 1; q < STAGES; ++q) if (s == q) tile = tile_of[q];
-        }
-        if (tile >= tiles) break;
-        const uint32_t bar = my_bar + s * 8, base = my_smem + s * TILE_BYTES + rowoff;
+    for (uint32_t it = 0; tile < tiles; ++it) {
         mbar_wait(bar, phase);
         const uint32_t i = tile * TILE_RECS + lane;
         const bool valid = i < n;
@@ -127,7 +100,7 @@ k1_ingest_tma(const __grid_constant__ CUtensorMap tmap, const agr_dev d, const u
         const ag_probe ap = k1_agent_issue(d, h2, h3);
         if (valid && !(h4.z & AGR_F_REPLAY) && !(d.cfg_flags & AGR_CFG_MINT_IDS))
             prefetch_l2(&d.table[agr_hash_id(pack64(h0.x, h0.y), pack64(h0.z, h0.w)) & d.table_mask]);
-        const uint32_t next_tile = tile + (uint32_t)STAGES * (gridDim.x * WARPS);
+        const uint32_t next_tile = tile + gridDim.x * WARPS;
         // position-weighted checksum over the 32 chunks of the record (weights k+1 over the 128 words).  Only shared
         // memory is touched between the wait and the refill, so the stage is held for the checksum alone.
         uint32_t c0 = 0, c1 = 0;
@@ -141,18 +114,11 @@ k1_ingest_tma(const __grid_constant__ CUtensorMap tmap, const agr_dev d, const u
         }
         __syncwarp();      // every lane has consumed the stage: refill it right away
         if (lane == 0 && next_tile < tiles) {
-            const uint32_t dst = my_smem + s * TILE_BYTES;
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic reads before async refill
             mbar_expect_tx(bar, TILE_BYTES);
 #pragma unroll
-            for (int cb = 0; cb < 4; ++cb) tma_load_2d(dst + cb * 4096, &tmap, bar, cb * 128, (int32_t)(first_rid + next_tile * TILE_RECS));
+            for (int cb = 0; cb < 4; ++cb) tma_load_2d(my_smem + cb * 4096, &tmap, bar, cb * 128, (int32_t)(first_rid + next_tile * TILE_RECS));
         }
-        if (pf_dist && lane < 4) {
-            const uint32_t t = next_tile + pf_dist * tstride;
-            if (t < tiles) tma_prefetch_2d(&tmap, lane * 128, (int32_t)(first_rid + t * TILE_RECS));
-        }
-#pragma unroll
-        for (int q = 0; q < STAGES; ++q) if (s == q) tile_of[q] = next_tile;
         if (valid) {
             d.cksum[rid] = agr_cksum_pack(c0, c1);
             // a ring sweeps every step: the row's last-SET time (= created_at, requests.go:106) goes into the word the sweep streams,
@@ -179,7 +145,8 @@ k1_ingest_tma(const __grid_constant__ CUtensorMap tmap, const agr_dev d, const u
         // (just consumed), so the CAS writes straight into the loop-carried registers.
         if (valid) k1_begin(d, ap, h0, h1, h2, h3, h4, h5.x, AGR_REC - AGR_OFF_PAYLOAD, MINT, first_log, first_log + i, i, pcx);
         ph1 = h1; ph5y = h5.y; prid = rid; pvalid = valid; ptile = tile;
-        if (s == STAGES - 1) phase ^= 1u;
+        phase ^= 1u;
+        tile = next_tile;
     }
     // The next K1 on the stream may start once every CTA of this one has streamed its tiles: its launch is processed during this
     // launch's drain, and its CTAs take each SM the moment this launch's CTA leaves it.  (Measured on H100: ~0.5 us a step
@@ -224,13 +191,14 @@ int agr_k1_tma_make_map(void* slab, unsigned long long rows, void* out_map /*128
     return r == CUDA_SUCCESS ? 0 : -2;
 }
 
-template <int WARPS, int STAGES, bool MINT>
-static cudaError_t launch_tma_k(const void* map, const agr_dev& d, uint32_t first_rid, unsigned long long first_log, uint32_t n,
-                              uint32_t pf_dist, int sm_count, cudaStream_t st) {
-    const size_t smem = (size_t)WARPS * STAGES * TILE_BYTES + 1024;
+template <bool MINT>
+static cudaError_t launch_tma(const void* map, const agr_dev& d, uint32_t first_rid, unsigned long long first_log, uint32_t n,
+                             int sm_count, cudaStream_t st) {
+    constexpr int WARPS = 14;
+    const size_t smem = (size_t)WARPS * TILE_BYTES + 1024;
     static bool attr_done = false;
     if (!attr_done) {
-        cudaError_t e = cudaFuncSetAttribute(k1_ingest_tma<WARPS, STAGES, MINT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        cudaError_t e = cudaFuncSetAttribute(k1_ingest_tma<WARPS, MINT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
         attr_done = true;
     }
@@ -246,22 +214,12 @@ static cudaError_t launch_tma_k(const void* map, const agr_dev& d, uint32_t firs
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(blocks); cfg.blockDim = dim3(WARPS * 32); cfg.dynamicSmemBytes = smem; cfg.stream = st;
     cfg.attrs = attr; cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, k1_ingest_tma<WARPS, STAGES, MINT>, *(const CUtensorMap*)map, d, first_rid, first_log, n, pf_dist);
-}
-template <int WARPS, int STAGES>
-static cudaError_t launch_tma(const void* map, const agr_dev& d, uint32_t first_rid, unsigned long long first_log, uint32_t n,
-                              uint32_t pf_dist, int sm_count, cudaStream_t st) {
-    return (d.cfg_flags & AGR_CFG_MINT_IDS) ? launch_tma_k<WARPS, STAGES, true>(map, d, first_rid, first_log, n, pf_dist, sm_count, st)
-                                            : launch_tma_k<WARPS, STAGES, false>(map, d, first_rid, first_log, n, pf_dist, sm_count, st);
+    return cudaLaunchKernelEx(&cfg, k1_ingest_tma<WARPS, MINT>, *(const CUtensorMap*)map, d, first_rid, first_log, n);
 }
 
-// variant 1 (default TMA): 7 warps x 2 stages; 2: 6 x 2; 3: 4 x 3; 4: 14 x 1 (all: one persistent CTA per SM)
-cudaError_t agr_launch_k1_tma(uint32_t variant, const void* map, const agr_dev& d, uint32_t first_rid, unsigned long long first_log,
-                              uint32_t n, uint32_t pf_dist, int sm_count, cudaStream_t st) {
-    switch (variant) {
-        case 2: return launch_tma<6, 2>(map, d, first_rid, first_log, n, pf_dist, sm_count, st);
-        case 3: return launch_tma<4, 3>(map, d, first_rid, first_log, n, pf_dist, sm_count, st);
-        case 4: return launch_tma<14, 1>(map, d, first_rid, first_log, n, pf_dist, sm_count, st);
-        default: return launch_tma<7, 2>(map, d, first_rid, first_log, n, pf_dist, sm_count, st);
-    }
+// one persistent CTA of 14 warps per SM, each warp with one 16 KiB stage
+cudaError_t agr_launch_k1_tma(const void* map, const agr_dev& d, uint32_t first_rid, unsigned long long first_log, uint32_t n,
+                              int sm_count, cudaStream_t st) {
+    return (d.cfg_flags & AGR_CFG_MINT_IDS) ? launch_tma<true>(map, d, first_rid, first_log, n, sm_count, st)
+                                            : launch_tma<false>(map, d, first_rid, first_log, n, sm_count, st);
 }

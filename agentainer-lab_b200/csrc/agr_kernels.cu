@@ -1,7 +1,7 @@
 // agr_kernels.cu — sm_90a kernels of the request path.
 //
-//   K1  k1_ingest_v0 (LSU variant; the default TMA kernel is in agr_k1_tma.cu, the variable-length one in
-//       agr_k1_var.cu), k1_index (split mode), k1_post          (requests.go:64-117, server.go:493-557)
+//   K1  k1_post, k1_index (the TMA kernel is in agr_k1_tma.cu, the variable-length one in agr_k1_var.cu)
+//                                                                 (requests.go:64-117, server.go:493-557)
 //   K2  k2_link / k2_apply / k2_append; with bytes (agr_complete_ex) k2_apply_bytes and k2_copy_bytes
 //                                                                 (requests.go:120-194,228-275, server.go:583-615)
 //   K3  k3_pass<count|scatter> / k3_scan_groups / k3_scan_total / k3_gather, k_resolve, k_verify, k_drop_*
@@ -10,76 +10,6 @@
 // All arithmetic is integer / byte work bounded by HBM bandwidth; there is no tensor-core work on this path.
 #include "agr_device.cuh"
 
-
-// v0: each warp owns 32 consecutive records.  Pass 1: lane i loads the 96 B header of record i (six 16 B loads,
-// every fetched sector fully used) and runs the decision chain thread-per-record, so 32 index inserts are in
-// flight per warp.  Pass 2: the warp streams the 416 B payloads coalesced (lane l = 16 B chunk l) for the record
-// checksum, REDUX-reducing per record.  Every byte of the record is read exactly once.
-template <int WARPS>
-__global__ void __launch_bounds__(WARPS * 32) k1_ingest_v0(const agr_dev d, const uint32_t first_rid, const uint32_t n) {
-    __shared__ uint32_t s_ctr[K1_NLC];
-    if (threadIdx.x < K1_NLC) s_ctr[threadIdx.x] = 0;
-    __syncthreads();
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    uint32_t lc[K1_NLC + 1];
-#pragma unroll
-    for (int c = 0; c <= K1_NLC; ++c) lc[c] = 0;
-    const uint32_t tiles = (n + 31u) >> 5;
-    for (uint32_t tile = blockIdx.x * WARPS + warp; tile < tiles; tile += gridDim.x * WARPS) {
-        const uint32_t i = tile * 32u + lane;
-        const bool valid = i < n;
-        const uint32_t rid = first_rid + i;
-        const uint8_t* tile_base = d.slab + (size_t)(first_rid + tile * 32u) * AGR_REC;
-        uint4 h0, h1, h2, h3, h4, h5;
-        h0 = h1 = h2 = h3 = h4 = h5 = make_uint4(0, 0, 0, 0);
-        if (valid) {
-            const uint8_t* rec = tile_base + (size_t)lane * AGR_REC;
-            h0 = ldg_nc_v4(rec);      h1 = ldg_nc_v4(rec + 16); h2 = ldg_nc_v4(rec + 32);
-            h3 = ldg_nc_v4(rec + 48); h4 = ldg_nc_v4(rec + 64); h5 = ldg_nc_v4(rec + 80);
-        }
-        // ---- long-latency chain first: agent probe -> classification -> first index CAS in flight
-        const ag_probe ap = k1_agent_issue(d, h2, h3);
-        k1_ctx cx;
-        if (valid) k1_begin(d, ap, h0, h1, h2, h3, h4, h5.x, AGR_REC - AGR_OFF_PAYLOAD, false, 0ULL, 0ULL, i, cx);
-        // ---- pass 2 (pure streaming, independent of the decision chain): payload checksum
-        uint32_t c0 = 0, c1 = 0;
-        {
-            const uint32_t hw[24] = {h0.x, h0.y, h0.z, h0.w, h1.x, h1.y, h1.z, h1.w, h2.x, h2.y, h2.z, h2.w,
-                                     h3.x, h3.y, h3.z, h3.w, h4.x, h4.y, h4.z, h4.w, h5.x, h5.y, h5.z, h5.w};
-#pragma unroll
-            for (int k = 0; k < 24; ++k) { c0 += hw[k]; c1 += (uint32_t)(k + 1) * hw[k]; }
-        }
-        const uint32_t in_tile = min(32u, n - tile * 32u);
-        const uint32_t wbase = 4u * lane + 1u;
-#pragma unroll 1
-        for (uint32_t r0 = 0; r0 < in_tile; r0 += 8) {
-            uint4 v[8];
-#pragma unroll
-            for (int u = 0; u < 8; ++u) {
-                v[u] = make_uint4(0, 0, 0, 0);
-                if (lane >= 6 && r0 + u < in_tile) v[u] = ldg_nc_v4(tile_base + (size_t)(r0 + u) * AGR_REC + lane * 16);
-            }
-#pragma unroll
-            for (int u = 0; u < 8; ++u) {
-                uint32_t p0 = v[u].x + v[u].y + v[u].z + v[u].w;
-                uint32_t p1 = wbase * v[u].x + (wbase + 1) * v[u].y + (wbase + 2) * v[u].z + (wbase + 3) * v[u].w;
-                p0 = __reduce_add_sync(FULL, p0);
-                p1 = __reduce_add_sync(FULL, p1);
-                if ((uint32_t)lane == r0 + u) { c0 += p0; c1 += p1; }
-            }
-        }
-        k1_note_time(d, first_rid + tile * 32u, min(32u, n - tile * 32u), valid ? pack64(h4.x, h4.y) : ~0ULL);
-        // ---- pass 1: decision chain, one record per lane
-        if (valid) {
-            k1_result r = k1_finish(d, rid, h1, h5, cx, lc);
-            d.state[rid] = r.state;
-            d.route[rid] = r.route;
-            d.cksum[rid] = agr_cksum_pack(c0, c1);
-            if (d.cfg_flags & AGR_CFG_RING) d.mtime[rid] = pack64(h4.x, h4.y);          // (see agr_k1_tma.cu)
-        }
-    }
-    k1_flush_counters(d, lc, s_ctr);
-}
 
 // Post pass over the batch's route words (4 B / record; the records themselves are re-read only for the rare rows
 // that need it).  Runs after ALL inserts of the batch:
@@ -131,9 +61,8 @@ __global__ void __launch_bounds__(256) k1_post(const agr_dev d, const uint32_t f
     if (threadIdx.x == 0) { int tot[3] = {s_delta[0], s_delta[1], s_delta[2]}; k1_post_apply(d, tot); }
 }
 
-// K1b (split mode): the dedupe-index insert of every provisionally stored row, one thread per record at full
-// occupancy — the random-access round trips are hidden by ~2 K resident threads per SM instead of by the streaming
-// warps' software pipeline.  A row whose id is already present becomes a provisional duplicate (k1_post decides).
+// The dedupe-index insert of every stored row, one thread per row at full occupancy (agr_launch_reindex: rebuilds the index
+// after a restore).  A row whose id is already present becomes a provisional duplicate (k1_post decides).
 __global__ void __launch_bounds__(256) k1_index(const agr_dev d, const uint32_t first_rid, const uint32_t n) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     const int lane = threadIdx.x & 31;
@@ -461,51 +390,30 @@ static uint32_t k1_post_blocks(uint32_t n, int sm_count) {
     return b < cap ? b : cap;
 }
 
-cudaError_t agr_launch_k1_tma(uint32_t variant, const void* map, const agr_dev& d, uint32_t first_rid, unsigned long long first_log,
-                              uint32_t n, uint32_t pf_dist, int sm_count, cudaStream_t st);
+cudaError_t agr_launch_k1_tma(const void* map, const agr_dev& d, uint32_t first_rid, unsigned long long first_log, uint32_t n,
+                              int sm_count, cudaStream_t st);
 
 void agr_launch_k1_post(const agr_dev& d, uint32_t first_rid, uint32_t n, int sm_count, cudaStream_t st, void* verdicts, void* ids,
                         const uint32_t* marks) {
     if (n) k1_post<<<k1_post_blocks(n, sm_count), 256, 0, st>>>(d, first_rid, n, (uint2*)verdicts, (uint4*)ids, marks);
 }
 
-int agr_launch_k1(const agr_dev& d, uint32_t first_rid, unsigned long long first_log, uint32_t n, uint32_t variant, const void* tmap,
+int agr_launch_k1(const agr_dev& d, uint32_t first_rid, unsigned long long first_log, uint32_t n, const void* tmap,
                   int sm_count, cudaStream_t st, cudaEvent_t ev0, cudaEvent_t ev1, void* verdicts, void* ids) {
     if (n == 0) return 0;
     if (ev0) cudaEventRecord(ev0, st);
-    if ((variant & 0xfu) != AGR_K1_LSU && tmap != nullptr) {
-        // minted ids never race for an id (dupfix stays 0) and the TMA kernel decides every replay's dedupe hit itself: without
-        // verdicts or ids to write there is nothing left for k1_post, and the kernel neither marks rows nor needs the pass
-        const bool post = !(d.cfg_flags & AGR_CFG_MINT_IDS) || (d.cfg_flags & AGR_CFGI_SPLIT_INDEX) || verdicts != nullptr || ids != nullptr;
-        agr_dev dk = d;
-        if (!post) dk.marks = nullptr;
-        agr_launch_k1_tma(variant & 0xfu, tmap, dk, first_rid, first_log, n, (variant >> 8) & 0xffu, sm_count, st);
-        if (ev1) cudaEventRecord(ev1, st);
-        if (!post) return 1;
-        int launched = 2;
-        if ((d.cfg_flags & AGR_CFGI_SPLIT_INDEX) && !(d.cfg_flags & AGR_CFG_MINT_IDS)) {
-            k1_index<<<(n + 255u) / 256u, 256, 0, st>>>(d, first_rid, n);
-            launched = 3;
-        }
-        // minted ids never race for an id (dupfix stays 0): without verdicts or ids to write, k1_post visits the marked rows only
-        const bool sparse = d.marks && (d.cfg_flags & AGR_CFG_MINT_IDS) && verdicts == nullptr && ids == nullptr;
-        k1_post<<<k1_post_blocks(sparse ? (n + 31u) / 32u : n, sm_count), 256, 0, st>>>(d, first_rid, n, (uint2*)verdicts, (uint4*)ids, d.marks);
-        return launched;
-    }
-    constexpr int WARPS = 8;
-    const uint32_t tiles = (n + 31u) / 32u;
-    uint32_t blocks = (tiles + WARPS - 1) / WARPS;
-    const uint32_t maxb = (uint32_t)sm_count * 8u;
-    if (blocks > maxb) blocks = maxb;
-    k1_ingest_v0<WARPS><<<blocks, WARPS * 32, 0, st>>>(d, first_rid, n);
+    // minted ids never race for an id (dupfix stays 0) and the TMA kernel decides every replay's dedupe hit itself: without
+    // verdicts or ids to write there is nothing left for k1_post, and the kernel neither marks rows nor needs the pass
+    const bool post = !(d.cfg_flags & AGR_CFG_MINT_IDS) || verdicts != nullptr || ids != nullptr;
+    agr_dev dk = d;
+    if (!post) dk.marks = nullptr;
+    agr_launch_k1_tma(tmap, dk, first_rid, first_log, n, sm_count, st);
     if (ev1) cudaEventRecord(ev1, st);
-    int launched = 2;
-    if ((d.cfg_flags & AGR_CFGI_SPLIT_INDEX) && !(d.cfg_flags & AGR_CFG_MINT_IDS)) {
-        k1_index<<<(n + 255u) / 256u, 256, 0, st>>>(d, first_rid, n);
-        launched = 3;
-    }
-    k1_post<<<k1_post_blocks(n, sm_count), 256, 0, st>>>(d, first_rid, n, (uint2*)verdicts, (uint4*)ids, nullptr);
-    return launched;
+    if (!post) return 1;
+    // minted ids never race for an id (dupfix stays 0): without verdicts or ids to write, k1_post visits the marked rows only
+    const bool sparse = d.marks && (d.cfg_flags & AGR_CFG_MINT_IDS) && verdicts == nullptr && ids == nullptr;
+    k1_post<<<k1_post_blocks(sparse ? (n + 31u) / 32u : n, sm_count), 256, 0, st>>>(d, first_rid, n, (uint2*)verdicts, (uint4*)ids, d.marks);
+    return 2;
 }
 
 // ------------------------------------------------------------------------------------------------ K2

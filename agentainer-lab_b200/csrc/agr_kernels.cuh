@@ -126,11 +126,6 @@ struct agr_k3_params {
     uint32_t* min_inq;         // TICK: lowest item (offset from lo) still in a pending list: low-water mark for the next scan
 };
 
-// K1 variants (agr_config.k1_variant low nibble): 0 = default (= 4); 1..4 = TMA kernel shapes (agr_k1_tma.cu:
-// 1 = 7 warps x 2 stages, 2 = 6 x 2, 3 = 4 x 3, 4 = 14 x 1), tmap = the slab's CUtensorMap (128 B);
-// 5 = LSU kernel (k1_ingest_v0, no TMA).  Bit 0x10 = split mode: stream kernel + k1_index kernel.
-#define AGR_K1_LSU 5u
-// The optional events bracket the main (dominant) kernel.
 // K1 for variable-length records (agr_k1_var.cu) and the matching gathers
 cudaError_t agr_launch_k1_var(const agr_dev& d, const uint8_t* blob, const uint32_t* off, uint32_t n, unsigned long long blob_bytes,
                               uint32_t* tile_first, uint32_t first_rid, unsigned long long blob_base, int sm_count, cudaStream_t st,
@@ -180,10 +175,10 @@ void agr_launch_k4_scatter(const agr_k4_params& p, cudaStream_t st);
 void agr_launch_k4_unpermute(const agr_k4_params& p, const void* local_res, const void* remote_res, void* out, uint32_t res_bytes,
                              cudaStream_t st);
 
-// first_log: arrival number of the batch's first row (= first_rid unless the slab is a ring).  With engine-minted ids the TMA
-// kernels decide every replay's dedupe hit themselves, and k1_post is launched only to write verdicts or ids.
-// Returns the number of kernels launched.
-int agr_launch_k1(const agr_dev& d, uint32_t first_rid, unsigned long long first_log, uint32_t n, uint32_t variant, const void* tmap,
+// first_log: arrival number of the batch's first row (= first_rid unless the slab is a ring); tmap: the slab's CUtensorMap (128 B,
+// agr_k1_tma_make_map).  With engine-minted ids the TMA kernel decides every replay's dedupe hit itself, and k1_post is launched
+// only to write verdicts or ids.  The optional events bracket the TMA kernel.  Returns the number of kernels launched (1 or 2).
+int agr_launch_k1(const agr_dev& d, uint32_t first_rid, unsigned long long first_log, uint32_t n, const void* tmap,
                    int sm_count, cudaStream_t st, cudaEvent_t ev0 = nullptr, cudaEvent_t ev1 = nullptr,
                    void* verdicts = nullptr /* device agr_verdict[n], written by k1_post */,
                    void* ids = nullptr /* device u8[n][16]: Request.ID per record, written by k1_post */);

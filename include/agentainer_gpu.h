@@ -133,10 +133,9 @@ typedef struct agr_config {
     uint64_t id_secret;      /* AGR_CFG_MINT_IDS: key of the id permutation; 0 = drawn from the OS CSPRNG at agr_create */
     uint64_t vslab_bytes;    /* AGR_CFG_VARLEN: capacity of the byte slab; 0 = 1024 * slab_rows */
     uint64_t resp_bytes;     /* capacity of the stored-response byte slab; 0 = 64 * slab_rows */
-    uint32_t k1_variant;     /* 0 = default K1 kernel (TMA, 14 warps x 1 stage, fused index); 1..4 TMA shapes, 5 = LSU kernel,
-                                | 0x10 = split stream / index kernels, | 0x20 = LSU form of the variable-length kernel —
-                                alternates kept for A/B measurement; bits 8..15 = L2 prefetch distance of the TMA kernel;
-                                bits 16..23 = k: AGR_CFG_TIMING times every k-th K1 launch (0, 1 = every launch) */
+    uint32_t k1_variant;     /* | 0x20 = LSU form of the variable-length kernel (AGR_CFG_VARLEN; default: TMA form);
+                                bits 16..23 = k: AGR_CFG_TIMING times every k-th K1 launch (0, 1 = every launch);
+                                every other bit must be 0 (AGR_EINVAL) */
     uint32_t reserved;
 } agr_config;
 

@@ -134,7 +134,7 @@ class RefIds:
         return verdicts, ids, first
 
 
-MODES = {"tma": dict(flags=MINT_RING), "lsu": dict(flags=MINT_RING, k1_variant=5),
+MODES = {"tma": dict(flags=MINT_RING),
          "varlen": dict(flags=MINT_RING | K.AGR_CFG_VARLEN, vslab_bytes=R * 1024),
          "combine": dict(flags=MINT_RING | K.AGR_CFG_COMBINE)}
 CASES = [(m, s) for m in MODES for s in STARTS if not (m == "combine" and s.endswith("pad"))]
@@ -167,7 +167,7 @@ def uuid_str(b):
     return str(uuid.UUID(bytes=bytes(b)))
 
 
-@pytest.mark.parametrize("mode", ["tma", "lsu", "varlen"])
+@pytest.mark.parametrize("mode", ["tma", "varlen"])
 @pytest.mark.parametrize("start", ["2^32-37", "2^40-37", "2^40-pad", "2^48-37", "bound"])
 def test_ids_and_resolution_far_along_the_counter(mode, start):
     """Every id the engine emits equals the reference's id of its arrival (ingest, dispatch, gathered records, agr_get_record,

@@ -57,7 +57,8 @@ def test_capacities_and_argument_checks():
 
 
 def test_bad_configs_are_rejected():
-    for kw in (dict(slab_rows=1 << 10, table_slots=1000), dict(slab_rows=1 << 10, table_slots=1024), dict(slab_rows=1 << 31)):
+    retired_k1 = [dict(slab_rows=1 << 10, k1_variant=v) for v in (1, 5, 0x10, 0x100)]     # K1 alternates that no longer exist
+    for kw in [dict(slab_rows=1 << 10, table_slots=1000), dict(slab_rows=1 << 10, table_slots=1024), dict(slab_rows=1 << 31)] + retired_k1:
         with pytest.raises(A.AgrError) as e:
             A.Engine(**kw)
         assert e.value.code == K.AGR_EINVAL

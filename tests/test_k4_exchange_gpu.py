@@ -171,19 +171,18 @@ def _owned_mask(b, G, r):
     return np.array([A.agent_shard(a.decode(), G) == r for a in b["agent_id"]], dtype=bool) if len(b) else np.zeros(0, bool)
 
 
-WORLD_CASES = [  # (G, minted ids, k1_variant, every agent registered on every shard)
-    (2, False, 0, False), (3, True, 0, False), (5, False, 2, False), (3, False, 5, False), (2, True, 5, False),
-    (5, True, 0x14, False), (3, False, 0x14, False), (2, True, 2, False),
-    (3, False, 0, True), (5, True, 0, True), (2, False, 5, True), (3, False, 0x14, True),
+WORLD_CASES = [  # (G, minted ids, every agent registered on every shard)
+    (2, False, False), (3, True, False), (5, False, False), (3, False, False), (2, True, False), (5, True, False),
+    (3, False, True), (5, True, True), (2, False, True),
 ]
 
 
-@pytest.mark.parametrize("G,mint,variant,everywhere", WORLD_CASES)
-def test_simulated_world_against_cref(G, mint, variant, everywhere):
+@pytest.mark.parametrize("G,mint,everywhere", WORLD_CASES)
+def test_simulated_world_against_cref(G, mint, everywhere):
     own = owned_agents(G, 6)
     status = lambda a: "running" if int(a[-1]) % 3 else "stopped"
     flags = K.AGR_CFG_PERSISTENCE | (K.AGR_CFG_MINT_IDS if mint else 0)
-    engs = [A.Engine(slab_rows=1 << 15, max_agents=256, max_batch=4096, flags=flags, k1_variant=variant) for _ in range(G)]
+    engs = [A.Engine(slab_rows=1 << 15, max_agents=256, max_batch=4096, flags=flags) for _ in range(G)]
     refs = [CRef() for _ in range(G)]
     try:
         for r, e in enumerate(engs):
@@ -306,15 +305,13 @@ def test_same_batch_replay_is_known_at_the_owner():
 
 
 # ------------------------------------------------------------------------------------------------ (c) the caller's bit 31
-@pytest.mark.parametrize("variant", [0, 5, 0x14])
-def test_caller_bit31_does_not_make_a_hole(variant):
+def test_caller_bit31_does_not_make_a_hole():
     """A record of this shard whose caller left flags bit 31 set, in an exchange batch that ships a record away, gets the
     verdict, stored state and bytes plain agr_ingest gives it."""
     G = 2
     own = owned_agents(G, 3)
     rng = np.random.default_rng(5)
-    with A.Engine(slab_rows=1 << 12, max_batch=1024, k1_variant=variant) as e, \
-            A.Engine(slab_rows=1 << 12, max_batch=1024, k1_variant=variant) as twin:
+    with A.Engine(slab_rows=1 << 12, max_batch=1024) as e, A.Engine(slab_rows=1 << 12, max_batch=1024) as twin:
         e.debug_world(0, G)
         for a in own[0] + own[1]:
             e.set_agent_state(a, "running"); twin.set_agent_state(a, "running")

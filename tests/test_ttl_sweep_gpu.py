@@ -314,15 +314,6 @@ def test_ttl_ring_caller_ids():
         rig.close()
 
 
-def test_ttl_ring_lsu_k1():
-    """Fixed-stride ring through the LSU K1 (k1_variant = 5): its own k1_note_time call site."""
-    rig = _rig(R_ODD, RING, k1_variant=5)
-    try:
-        drive_ring(rig, 18)
-    finally:
-        rig.close()
-
-
 def test_ttl_ring_tickets():
     """AGR_CFG_COMBINE: part of the records and outcomes go through the single-request ring (the service kernel's TTL
     bookkeeping), the rest through K1 / K2 batches."""
