@@ -694,12 +694,11 @@ static int complete_locked(agr_handle* h, const agr_outcome* outs, uint32_t n, i
         CK(cudaStreamSynchronize(h->stream));
     }
     // the state transitions were applied; list entries beyond the log capacity were dropped (agr_config.log_entries)
-    const char* log_full = "completed / failed log full: entries of this batch were dropped (raise agr_config.log_entries, or agr_reclaim)";
     if (bytes_dropped)
         return fail(AGR_ENOSPC, std::string("response byte slab full: the batch's outcomes were applied, none of its response / error bytes "
                                             "were stored (raise agr_config.resp_bytes, or agr_reclaim with AGR_CFG_RING)") +
-                                    (*h->h_k2flag ? std::string("; also ") + log_full : std::string()));
-    if (*h->h_k2flag) return fail(AGR_ENOSPC, log_full);
+                                    (*h->h_k2flag ? std::string("; also ") + K2_LOG_FULL : std::string()));
+    if (*h->h_k2flag) return fail(AGR_ENOSPC, K2_LOG_FULL);
     return 0;
 }
 

@@ -293,6 +293,9 @@ int launch_k1_locked(agr_handle* h, uint64_t first, uint32_t n, agr_verdict* d_o
 int resp_reserve_locked(agr_handle* h, uint64_t need, uint64_t len, unsigned long long* off);
 int check_segments(const agr_outcome* outs, uint32_t n, const uint64_t* offsets, const uint32_t* hdr_lens, uint64_t* total,
                    uint64_t* max_len);
+// agr_last_error of an agr_complete / agr_complete_ex whose pushes did not all fit the completed / failed log (batch and ring)
+constexpr const char* K2_LOG_FULL =
+    "completed / failed log full: entries of this batch were dropped (raise agr_config.log_entries, or agr_reclaim)";
 // agr_front.cu
 int svc_create(agr_handle* h);
 void svc_destroy(agr_handle* h);

@@ -291,14 +291,17 @@ int svc_complete(agr_handle* h, const agr_outcome* outs, uint32_t n, int32_t* re
     uint64_t pos[SVC_MAX_CALL];
     for (uint32_t i = 0; i < n; ++i) while (!svc_submit_one(s, SVC_OP_OUTCOME, &outs[i], sizeof(agr_outcome), &pos[i])) {}
     int rc = 0;
+    bool log_full = false;
     for (uint32_t i = 0; i < n; ++i) {
         svc_answer r; svc_wait(s, pos[i], &r);
         const int32_t res = (int32_t)r.w0;
         if (res < 0 && res != AGR_ENOTFOUND) rc = res;
+        log_full |= (r.w1 & SVC_OUT_LOG_FULL) != 0u;
         if (results) results[i] = res;
         svc_release(s, pos[i]);
     }
     if (rc < 0) return fail(rc, "single-request front end: CUDA error");
+    if (log_full) return fail(AGR_ENOSPC, K2_LOG_FULL);       // as the batch path: applied, the push dropped
     return 0;
 }
 
@@ -316,18 +319,22 @@ int svc_complete_ex(agr_handle* h, const agr_outcome* outs, uint32_t n, const ui
         while (!svc_submit_outcome_bytes(s, &outs[i], hl, len ? bytes + offsets[i] : nullptr, len, nullptr, 0u, &pos[i])) {}
     }
     int rc = 0;
+    bool log_full = false;
     for (uint32_t i = 0; i < n; ++i) {
         svc_answer r; svc_wait(s, pos[i], &r);
         int32_t res = (int32_t)r.w0;
         if (res == AGR_ENOSPC) { res = 0; if (rc == 0) rc = AGR_ENOSPC; }
         else if (res < 0 && res != AGR_ENOTFOUND) rc = res;
+        log_full |= (r.w1 & SVC_OUT_LOG_FULL) != 0u;
         if (results) results[i] = res;
         svc_release(s, pos[i]);
     }
     if (rc == AGR_ENOSPC)
-        return fail(rc, "response byte slab full: the outcomes were applied, their response / error bytes were not stored "
-                        "(raise agr_config.resp_bytes, or agr_reclaim with AGR_CFG_RING)");
+        return fail(rc, std::string("response byte slab full: the outcomes were applied, their response / error bytes were not stored "
+                                    "(raise agr_config.resp_bytes, or agr_reclaim with AGR_CFG_RING)") +
+                            (log_full ? std::string("; also ") + K2_LOG_FULL : std::string()));
     if (rc < 0) return fail(rc, "single-request front end: CUDA error");
+    if (log_full) return fail(AGR_ENOSPC, K2_LOG_FULL);
     return 0;
 }
 
@@ -358,7 +365,7 @@ static int collect(agr_handle* h, agr_ticket ticket, const svc_answer& r, agr_re
         if (rec) {
             if ((r.w0 & 0xffu) == 0u) out->result = (int32_t)r.w1;
             else { memcpy(&out->verdict, &r.w0, 4); memcpy((uint8_t*)&out->verdict + 4, &r.w1, 4); out->rid = svc_row(s, r); svc_request_id(h, t, out->rid, out->request_id); }
-        } else out->result = (int32_t)r.w0;
+        } else out->result = (r.w1 & SVC_OUT_LOG_FULL) ? AGR_ENOSPC : (int32_t)r.w0;   // applied, its log push dropped
     }
     svc_release(s, t);
     return 0;

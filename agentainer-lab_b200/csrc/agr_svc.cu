@@ -320,10 +320,11 @@ k_svc(const agr_dev d0, const svc_dev v, const agr_k2_scratch k2, const unsigned
             uint32_t pc = 0, pf = 0, tc = 0, tf = 0;
 #pragma unroll
             for (int w = 0; w < (int)(SVC_WORKERS / 32u); ++w) { if ((uint32_t)w < wwarp) { pc += s_wc[w]; pf += s_wf[w]; } tc += s_wc[w]; tf += s_wf[w]; }
+            uint32_t log_full = 0u;                                               // this outcome's push was dropped: its caller is told
             if (eff) {
                 const uint32_t rid = k2.ops[wt].rid;
-                if (eff & 1u) { const unsigned long long p = s_logbase[0] + pc + __popc(bc & lt); if (p < d.log_cap) d.completed_log[p] = rid; }
-                if (eff & 2u) { const unsigned long long p = s_logbase[1] + pf + __popc(bf & lt); if (p < d.log_cap) d.failed_log[p] = rid; }
+                if (eff & 1u) { const unsigned long long p = s_logbase[0] + pc + __popc(bc & lt); if (p < d.log_cap) d.completed_log[p] = rid; else log_full = SVC_OUT_LOG_FULL; }
+                if (eff & 2u) { const unsigned long long p = s_logbase[1] + pf + __popc(bf & lt); if (p < d.log_cap) d.failed_log[p] = rid; else log_full = SVC_OUT_LOG_FULL; }
             }
             if (wt == 0 && (tc | tf)) {
                 unsigned long long nc = s_logbase[0] + tc, nf = s_logbase[1] + tf;
@@ -345,12 +346,12 @@ k_svc(const agr_dev d0, const svc_dev v, const agr_k2_scratch k2, const unsigned
                 }
             }
             // the outcomes' result codes (the records' verdicts went out as soon as they were final); an outcome whose bytes found
-            // no room was applied all the same and says so with AGR_ENOSPC
+            // no room was applied all the same and says so with AGR_ENOSPC, one whose log push was dropped with SVC_OUT_LOG_FULL
             if (wt < nout) {
                 const unsigned long long slot_abs = from + s_out_op[st][wt];
                 int32_t res = k2.results[wt];
                 if (res == 0 && nbyt && !bytes_in && s_out_stage[st][wt] != 0xffffu) res = AGR_ENOSPC;
-                st_res(v.res + (slot_abs & (SVC_SLOTS - 1u)), (uint32_t)res, 0u, 0u, svc_tag(slot_abs) << 16);
+                st_res(v.res + (slot_abs & (SVC_SLOTS - 1u)), (uint32_t)res, log_full, 0u, svc_tag(slot_abs) << 16);
             }
         }
         bar_sync(BAR_WORK, SVC_WORKERS);                                         // everything of the stage has been read

@@ -94,12 +94,14 @@ static_assert(sizeof(svc_desc) == 256, "svc_desc must be 256 B (sixteen 16 B lan
 // none of it, so no system-wide fence sits between "result" and "done"):
 //   record   w0, w1 = agr_verdict (w0's low byte = AGR_V_*, never 0);  w2 | (w3 & 0xffff) << 32 = logical row
 //            host-side failure (slab full / CUDA error, written by the dispatcher): w0 = 0, w1 = (uint32_t)error code
-//   outcome  w0 = (uint32_t)result (0 / AGR_ENOTFOUND / error code)
+//   outcome  w0 = (uint32_t)result (0 / AGR_ENOTFOUND / error code);  w1 = SVC_OUT_LOG_FULL when its completed / failed
+//            push landed past the log's capacity and was dropped (the transition was applied), else 0
 //   w3 >> 16 = tag of the slot's lap (svc_tag): the caller spins on it, and sets SVC_COLLECTED in it once it has read the
 //              answer — that line is in the collector's cache anyway, so freeing a slot costs no extra miss.
 // Request.ID is not shipped: with engine-minted ids it is a function of the row (agr_mint_id, computed by the caller's
 // thread), with caller-supplied ids the caller has it already.
 struct __attribute__((aligned(16))) svc_res { volatile uint32_t w[4]; };
+#define SVC_OUT_LOG_FULL 1u
 #if defined(__CUDACC__)
 __host__ __device__
 #endif

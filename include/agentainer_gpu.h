@@ -222,7 +222,10 @@ typedef struct agr_outcome {
 
 /* Applies outs[0..n) in array order.  results (nullable) receives per outcome 0 or AGR_ENOTFOUND (the
  * "failed to get request" error the callers only log, Q20).  An all-zero request_id is a no-op
- * (t.requestID == "", server.go:588,597). */
+ * (t.requestID == "", server.go:588,597).  Returns AGR_ENOSPC ("completed / failed log full" in agr_last_error) when a
+ * completed / failed push of the call did not fit agr_config.log_entries: every transition was applied and results filled,
+ * the pushes past the capacity were dropped (a call that ends exactly at the capacity returns 0).  The same holds whichever
+ * path the call takes (one locked batch, or the single-request ring with AGR_CFG_COMBINE). */
 int agr_complete(agr_handle* h, const agr_outcome* outs, uint32_t n, int32_t* results);
 
 /* agr_complete with the bytes StoreResponse / MarkRequestFailed keep (requests.go:134-175,244), in the same call.  Segment i =
@@ -263,7 +266,8 @@ typedef struct agr_result {
     agr_verdict verdict;       /* record: the proxy decision (zeroed for an outcome) */
     uint8_t  request_id[16];   /* record: Request.ID as the engine knows it */
     uint64_t rid;              /* record: its row */
-    int32_t  result;           /* 0, AGR_ENOTFOUND (outcome: "failed to get request"), AGR_ENOSPC (record: slab full), AGR_ECUDA */
+    int32_t  result;           /* 0, AGR_ENOTFOUND (outcome: "failed to get request"), AGR_ENOSPC (record: slab full; outcome:
+                                  applied, but its completed / failed push did not fit the log, or its bytes found no room), AGR_ECUDA */
     uint32_t is_outcome;
 } agr_result;                  /* 40 B */
 int agr_submit_ingest(agr_handle* h, const agr_record* rec, agr_ticket* ticket);
@@ -271,7 +275,7 @@ int agr_submit_complete(agr_handle* h, const agr_outcome* outcome, agr_ticket* t
 /* agr_submit_complete with the outcome's bytes in the ticket (agr_complete_ex(n = 1) semantics): headers then body for a
  * response, the error text in body for an error (hdr_len 0).  hdr_len + body_len <= AGR_OUT_INLINE_BYTES, else AGR_EINVAL:
  * the caller then uses agr_submit_complete_large, or agr_complete_ex(n = 1).  The ticket's result is AGR_ENOSPC when the transition was applied but the
- * bytes found no room in the response byte slab. */
+ * bytes found no room in the response byte slab, or its completed / failed push did not fit the log (as for agr_submit_complete). */
 int agr_submit_complete_ex(agr_handle* h, const agr_outcome* outcome, const uint8_t* headers, uint32_t hdr_len,
                            const uint8_t* body, uint32_t body_len, agr_ticket* ticket);
 /* agr_submit_complete_ex for hdr_len + body_len <= AGR_OUT_TICKET_MAX_BYTES: a segment longer than AGR_OUT_INLINE_BYTES takes
@@ -458,7 +462,8 @@ typedef struct agr_stats {
     uint64_t k5_launches;
     uint64_t rows_tail;     /* AGR_CFG_RING: first row id that has not been released (0 otherwise); rows_used - rows_tail <= rows_cap */
     uint64_t malformed;     /* records rejected with AGR_VF_BAD_LEN */
-    uint64_t log_overflow;  /* agr_complete batches whose completed / failed pushes did not fit the log (they returned AGR_ENOSPC) */
+    uint64_t log_overflow;  /* agr_complete batches whose completed / failed pushes did not fit the log (their calls returned AGR_ENOSPC);
+                               through the single-request ring (AGR_CFG_COMBINE) it counts batches of the service kernel */
     uint64_t svc_batches, svc_ops;   /* AGR_CFG_COMBINE: batches formed by the dispatcher / single-request operations served */
     uint32_t agents, device;
 } agr_stats;
