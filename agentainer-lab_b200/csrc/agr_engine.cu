@@ -489,7 +489,8 @@ static int claim_k1_events(agr_handle* h, cudaEvent_t* e0, cudaEvent_t* e1) {
     *e0 = h->tev[2 * k]; *e1 = h->tev[2 * k + 1];
     return 0;
 }
-// AGR_CFG_TIMING: events around the last launch group g (0 = K2, 1 = K3 select, 2 = K5 encode, 3 = snapshot cut) that agr_op_time reads
+// AGR_CFG_TIMING: events around the last launch group g (0 = K2, 1 = K3 select, 2 = K5 encode, 3 = snapshot cut, 4 = the
+// relocation of a restore) that agr_op_time reads
 int op_time_begin(agr_handle* h, int g) {
     if (!(h->cfg.flags & AGR_CFG_TIMING)) return 0;
     for (auto& e : h->op_ev) if (!e) CK(cudaEventCreate(&e));
@@ -1467,7 +1468,7 @@ int agr_debug_skip_arrivals(agr_handle* h, uint64_t n) {
 }
 
 int agr_op_time(agr_handle* h, int which, double* ms) {
-    if (!h || !ms || which < 0 || which > 3) return fail(AGR_EINVAL, "bad argument");
+    if (!h || !ms || which < 0 || which > 4) return fail(AGR_EINVAL, "bad argument");
     HLock lk(h);
     CK(cudaSetDevice(h->device));
     if (!h->op_timed[which]) return fail(AGR_ENOTFOUND, "no timed launch of that group yet (needs AGR_CFG_TIMING)");

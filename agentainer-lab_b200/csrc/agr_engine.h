@@ -181,8 +181,8 @@ struct agr_handle {
     exchange_plan xdbg{}; uint64_t xdbg_first = 0; uint32_t xdbg_n = 0; bool xdbg_open = false;   // agr_debug_exchange_begin -> _end
     // AGR_CFG_TIMING: CUDA-event pairs around the dominant K1 kernel, on the launching stream
     std::vector<cudaEvent_t> tev; uint64_t tev_next = 0, tev_read = 0, timing_calls = 0;
-    cudaEvent_t op_ev[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // [0,1] last K2 group, [2,3] last K3 select group, [4,5] last K5 encode, [6,7] last snapshot cut
-    bool op_timed[4] = {false, false, false, false};
+    cudaEvent_t op_ev[10] = {};                // [0,1] last K2 group, [2,3] last K3 select group, [4,5] last K5 encode, [6,7] last snapshot cut, [8,9] the relocation of the restore that made the engine
+    bool op_timed[5] = {false, false, false, false, false};
     // AGR_CFG_ONLINE_SNAPSHOT: the cut's device shadow of the sections rewritten in place (the two log lengths at offset 0, then
     // every such section at shadow_off), the writer's own stream, its two pinned buffers, and the pins (agr_snapshot)
     uint8_t* d_shadow = nullptr; size_t shadow_off[17] = {};

@@ -253,3 +253,29 @@ struct agr_snap_blocks {
     uint8_t* stage;
 };
 void agr_launch_snap_blocks(const agr_snap_blocks& g, uint32_t n, bool gather, cudaStream_t st);
+
+// Relocation of a restore into other capacities (agr_relayout.cu).  Row ids [s.tail, s.tail + n) of the source engine s move
+// to row id mod t.ring_rows of the target t with every per-row word; the record bytes (AGR_CFG_VARLEN) and the response / error
+// bytes of the live rows (state != 0) are packed in row-id order from byte 0 of t's byte rings, each response and error
+// segment on a 16 B boundary.  count: per-tile sums, then their exclusive scan and the two totals (record bytes, response
+// bytes) at totals; rows: the words, the 512 B rows and the segment lists; bytes: one byte ring from its segment list
+// (destination offsets non-decreasing); log: one completed / failed log's physical rows.
+struct agr_relayout_words {            // the per-row words of the stored responses, which agr_dev does not carry
+    unsigned long long* resp_off; uint32_t* resp_len; uint32_t* resp_hlen;
+    unsigned long long* err_off; uint32_t* err_len;
+};
+struct agr_relayout {
+    agr_dev s, t;
+    agr_relayout_words sw, tw;
+    unsigned long long n;
+    unsigned long long* tile_sum;      // [2 * agr_relayout_tiles(n)]
+    unsigned long long* totals;        // [2]
+    unsigned long long *vseg_dst, *vseg_src; uint32_t* vseg_len;   // [n]: row k's record
+    unsigned long long *rseg_dst, *rseg_src; uint32_t* rseg_len;   // [2n]: row k's response, then its error text
+};
+uint32_t agr_relayout_tiles(unsigned long long n);
+void agr_launch_relayout_count(const agr_relayout& p, cudaStream_t st);
+void agr_launch_relayout_rows(const agr_relayout& p, cudaStream_t st);
+void agr_launch_relayout_bytes(const uint8_t* src, uint8_t* dst, const unsigned long long* seg_dst, const unsigned long long* seg_src,
+                               const uint32_t* seg_len, unsigned long long nseg, unsigned long long total, cudaStream_t st);
+void agr_launch_relayout_log(const agr_dev& s, const agr_dev& t, const uint32_t* in, uint32_t* out, unsigned long long len, cudaStream_t st);

@@ -529,8 +529,10 @@ static int restore_chain(const char* path, std::vector<std::string>& files, std:
 }
 // The state of the whole chain into h: the full file (f, past its header), each delta after a check that the state so far
 // is its parent's cut (digest), then the header fields, the log lengths, the dedupe index and the chain an
-// AGR_CFG_DELTA_SNAPSHOT engine continues, once.
-static int restore_locked(agr_handle* h, FILE* f, const snap_header& full, const std::vector<std::string>& files, const std::vector<delta_header>& dh) {
+// AGR_CFG_DELTA_SNAPSHOT engine continues, once.  index = false leaves the dedupe index out (the source engine of a relocation,
+// whose rows only move).
+static int restore_locked(agr_handle* h, FILE* f, const snap_header& full, const std::vector<std::string>& files, const std::vector<delta_header>& dh,
+                          bool index = true) {
     HLock lk(h);
     CK(cudaSetDevice(h->device));
     TRY(restore_agents_locked(h, f, full.n_agents));
@@ -560,7 +562,7 @@ static int restore_locked(agr_handle* h, FILE* f, const snap_header& full, const
     h->d.shard_id = hd.shard; h->d.id_gen = hd.gen; h->tail = hd.tail; h->released_total = hd.released_total; sync_window(h);
     h->d.idx_base = h->tail;
     TRY(chunk_bounds_unknown(h));
-    if (!(hd.flags & AGR_CFG_MINT_IDS) && R) {        // hash-id mode: rebuild the dedupe index from the restored rows
+    if (index && !(hd.flags & AGR_CFG_MINT_IDS) && R) {   // hash-id mode: rebuild the dedupe index from the restored rows
         agr_launch_reindex(h->d, (uint32_t)R, h->stream);
         h->k1_launches += 1;
         if (cudaStreamSynchronize(h->stream) != cudaSuccess) return fail(AGR_ECUDA, "restore: reindex");
@@ -584,6 +586,121 @@ static int restore_locked(agr_handle* h, FILE* f, const snap_header& full, const
     return 0;
 }
 
+// ---- restore into other capacities (DESIGN.md section 5)
+// Whether the restored state of the last cut s has to move: a ring snapshot into other ring capacities, or an append-only
+// snapshot into a ring.  Every other restore loads the file in place.
+static bool restore_relocates(const agr_handle* h, const snap_header& s) {
+    if (!(s.flags & AGR_CFG_RING)) return is_ring(h);
+    return s.slab_rows != h->cfg.slab_rows || s.resp_cap != h->resp_cap || ((s.flags & AGR_CFG_VARLEN) && s.vcap != h->vcap);
+}
+static std::string relocation_enomem() {
+    return "restore: relocating into other capacities holds the snapshot's engine and the configured one on the device at once, "
+           "and both do not fit: " + g_err;
+}
+// Moves the state of the source engine s (the last cut hd, restored in s's own geometry) into h (a ring): the window's rows to
+// row id mod h's slab_rows, the live rows' record and response bytes packed from byte 0, the logs remapped.  The header fields
+// other than the byte rings' cursors stay as hd has them.
+static int relocate_locked(agr_handle* h, agr_handle* s, const snap_header& hd) {
+    HLock lk(h);
+    CK(cudaSetDevice(h->device));
+    CK(cudaStreamSynchronize(s->stream));
+    for (uint32_t a = 0; a < (uint32_t)s->agent_names.size(); ++a) {   // the agent table, slot for slot (as restore_agents_locked)
+        const bool removed = s->agent_status[a] == AG_STATUS_REMOVED;
+        const int slot = set_agent_state_locked(h, s->agent_names[a].c_str(), removed ? (uint8_t)AGR_AGENT_STOPPED : s->agent_status[a], true);
+        if (slot < 0) return slot;
+        if ((uint32_t)slot != a) return fail(AGR_EINVAL, "restore: an agent appears twice in the agent table");
+        if (removed) { h->agent_status[a] = AG_STATUS_REMOVED; TRY(push_agent_status(h, a, AG_STATUS_REMOVED)); }
+    }
+    const bool var = (hd.flags & AGR_CFG_VARLEN) != 0;
+    const uint64_t n = hd.rows_used - hd.tail;
+    h->rows_used = hd.rows_used; h->tail = hd.tail; h->released_total = hd.released_total; h->scan_lo = hd.scan_lo;
+    h->expired_total = hd.expired_total; h->d.shard_id = hd.shard; h->d.id_gen = hd.gen;
+    sync_window(h);                                            // h->d now has the target's window and ring geometry
+    agr_relayout p{};
+    p.s = s->d; p.t = h->d; p.n = n;
+    p.sw = agr_relayout_words{s->d_resp_off, s->d_resp_len, s->d_resp_hlen, s->d_err_off, s->d_err_len};
+    p.tw = agr_relayout_words{h->d_resp_off, h->d_resp_len, h->d_resp_hlen, h->d_err_off, h->d_err_len};
+    {   // scratch of the move: allocated with the source engine, freed with it
+        const size_t tiles = std::max<uint32_t>(agr_relayout_tiles(n), 1), rows = std::max<uint64_t>(n, 1);
+        const int rc = [&]() {
+            TRY(dev_alloc(s, &p.tile_sum, 2 * tiles, false));
+            TRY(dev_alloc(s, &p.totals, (size_t)2, false));
+            if (var) { TRY(dev_alloc(s, &p.vseg_dst, rows, false)); TRY(dev_alloc(s, &p.vseg_src, rows, false)); TRY(dev_alloc(s, &p.vseg_len, rows, false)); }
+            TRY(dev_alloc(s, &p.rseg_dst, 2 * rows, false)); TRY(dev_alloc(s, &p.rseg_src, 2 * rows, false)); TRY(dev_alloc(s, &p.rseg_len, 2 * rows, false));
+            return 0;
+        }();
+        if (rc == AGR_ENOMEM) return fail(rc, relocation_enomem());
+        TRY(rc);
+    }
+    TRY(op_time_begin(h, 4));
+    agr_launch_relayout_count(p, h->stream);
+    CK(cudaGetLastError());
+    unsigned long long tot[2];
+    TRY(d2h_staged(h, tot, p.totals, sizeof tot, h->h_small));
+    if (var && tot[0] > h->vcap)
+        return fail(AGR_ENOSPC, "restore: the live records take " + std::to_string(tot[0]) + " B, more than vslab_bytes (" +
+                                    std::to_string(h->vcap) + " B) by " + std::to_string(tot[0] - h->vcap) + " B");
+    if (tot[1] > h->resp_cap)
+        return fail(AGR_ENOSPC, "restore: the live response and error bytes take " + std::to_string(tot[1]) + " B, more than resp_bytes (" +
+                                    std::to_string(h->resp_cap) + " B) by " + std::to_string(tot[1] - h->resp_cap) + " B");
+    agr_launch_relayout_rows(p, h->stream);
+    if (var) agr_launch_relayout_bytes(s->d.slab, h->d.slab, p.vseg_dst, p.vseg_src, p.vseg_len, n, tot[0], h->stream);
+    agr_launch_relayout_bytes(s->d_resp, h->d_resp, p.rseg_dst, p.rseg_src, p.rseg_len, 2 * n, tot[1], h->stream);
+    agr_launch_relayout_log(s->d, h->d, s->d.completed_log, h->d.completed_log, hd.log_len[0], h->stream);
+    agr_launch_relayout_log(s->d, h->d, s->d.failed_log, h->d.failed_log, hd.log_len[1], h->stream);
+    CK(cudaGetLastError());
+    TRY(op_time_end(h, 4));
+    const unsigned long long lens[2] = {hd.log_len[0], hd.log_len[1]};
+    CK(cudaMemcpyAsync(h->d.log_len, lens, sizeof lens, cudaMemcpyHostToDevice, h->stream));
+    h->vused = var ? tot[0] : 0; h->vtail = 0;
+    h->resp_used = tot[1]; h->resp_tail = 0;
+    h->d.idx_base = h->tail;
+    TRY(chunk_bounds_unknown(h));
+    const uint64_t R = rows_span(h);
+    if (!(hd.flags & AGR_CFG_MINT_IDS) && R) {                 // hash-id mode: the dedupe index of the moved rows
+        agr_launch_reindex(h->d, (uint32_t)R, h->stream);
+        h->k1_launches += 1;
+    }
+    if (cudaStreamSynchronize(h->stream) != cudaSuccess) return fail(AGR_ECUDA, "restore: relocation");
+    return 0;
+}
+// The relocating restore into h: the file (f, past its header) and its deltas go into a source engine of the snapshot's own
+// geometry, which is then moved into h and freed.  The source engine is bare: no single-request front end, no snapshot shadows,
+// no dedupe index (created in minted-id form, so that it allocates none; nothing of the id mode is in the arrays it holds).
+static int restore_relocate(agr_handle* h, FILE* f, const snap_header& full, const std::vector<std::string>& files, const std::vector<delta_header>& dh) {
+    const snap_header& last = dh.empty() ? full : dh.back().cut;
+    const bool ring = (last.flags & AGR_CFG_RING) != 0;
+    const uint64_t window = last.rows_used - last.tail;
+    if (window > h->cfg.slab_rows)
+        return fail(AGR_ENOSPC, "restore: the live window of the snapshot holds " + std::to_string(window) + " rows, more than slab_rows (" +
+                                    std::to_string(h->cfg.slab_rows) + ") by " + std::to_string(window - h->cfg.slab_rows));
+    uint64_t logs = 1;
+    for (size_t k = 0; k <= dh.size(); ++k) {
+        const snap_header& s = k ? dh[k - 1].cut : full;
+        if (s.log_len[0] > h->d.log_cap || s.log_len[1] > h->d.log_cap) return fail(AGR_ENOSPC, "restore: snapshot larger than the configured capacities");
+        logs = std::max<uint64_t>(logs, std::max(s.log_len[0], s.log_len[1]));
+    }
+    agr_config sc{};
+    sc.flags = AGR_CFG_PERSISTENCE | AGR_CFG_MINT_IDS | (last.flags & (AGR_CFG_VARLEN | AGR_CFG_RING));
+    sc.device = h->device; sc.id_secret = last.id_secret; sc.max_agents = h->cfg.max_agents; sc.log_entries = logs;
+    sc.max_batch = 1u << 16;                                   // (sizes the staging buffers the load streams through)
+    if (ring) { sc.slab_rows = last.slab_rows; sc.vslab_bytes = last.vcap; sc.resp_bytes = last.resp_cap; }
+    else {                                                     // append-only: what the file holds (the last cut holds the most)
+        sc.slab_rows = std::max<uint64_t>(last.rows_used, 1);
+        sc.vslab_bytes = std::max<uint64_t>(last.vused, 16); sc.resp_bytes = std::max<uint64_t>(last.resp_used, 16);
+    }
+    agr_handle* s = nullptr;
+    int rc = agr_create(&sc, &s);
+    if (rc == AGR_ENOMEM) return fail(rc, relocation_enomem());
+    TRY(rc);
+    rc = restore_locked(s, f, full, files, dh, false);
+    if (rc == 0) rc = relocate_locked(h, s, last);
+    const std::string keep = g_err;
+    agr_destroy(s);
+    g_err = keep;
+    return rc;
+}
+
 int agr_restore(const agr_config* cfg, const char* path, agr_handle** out) {
     if (!cfg || !path || !out) return fail(AGR_EINVAL, "NULL argument");
     *out = nullptr;
@@ -597,7 +714,8 @@ int agr_restore(const agr_config* cfg, const char* path, agr_handle** out) {
     agr_config c = *cfg;
     if (c.flags == 0) c.flags = AGR_CFG_PERSISTENCE;
     const uint32_t mode_bits = AGR_CFG_MINT_IDS | AGR_CFG_VARLEN | AGR_CFG_RING;
-    if ((c.flags & mode_bits) != (hd.flags & mode_bits)) { fclose(f); return fail(AGR_EINVAL, "restore: id mode / record form differ from the snapshot"); }
+    const uint32_t form = (hd.flags & AGR_CFG_RING) ? mode_bits : mode_bits & ~AGR_CFG_RING;   // (append-only into a ring relocates)
+    if ((c.flags & form) != (hd.flags & form)) { fclose(f); return fail(AGR_EINVAL, "restore: id mode / record form differ from the snapshot"); }
     if (c.id_secret == 0) c.id_secret = hd.id_secret;
     if (c.id_secret != hd.id_secret) { fclose(f); return fail(AGR_EINVAL, "restore: id_secret differs from the snapshot"); }
     for (size_t k = 0; k < dh.size(); ++k)
@@ -609,6 +727,12 @@ int agr_restore(const agr_config* cfg, const char* path, agr_handle** out) {
     int rc = agr_create(&c, &h);
     if (rc < 0) { fclose(f); return rc; }
     auto bail = [&](int r) { std::string keep = g_err; fclose(f); agr_destroy(h); g_err = keep; return r; };
+    if (restore_relocates(h, dh.empty() ? hd : dh.back().cut)) {
+        if ((rc = restore_relocate(h, f, hd, files, dh)) < 0) return bail(rc);
+        fclose(f);
+        *out = h;
+        return 0;
+    }
     auto fits = [&](const snap_header& s) -> int {
         const bool snap_ring = (s.flags & AGR_CFG_RING) != 0;
         if (!snap_ring && s.resp_used > h->resp_cap) return fail(AGR_ENOSPC, "restore: stored responses larger than resp_bytes");

@@ -425,7 +425,19 @@ int agr_json_decode(const uint8_t* json, uint32_t len, uint8_t* record, uint32_t
  * agr_restore accepts either kind.  Given a delta it follows the parent paths back to the full file, loads it and applies the
  * deltas oldest first; a parent that is missing, replaced by another file or shorter than its header says fails with
  * AGR_EINVAL.  So the files of a chain must stay where they were written until a newer full file exists.  An engine restored
- * with the flag continues the chain: its next agr_snapshot is a delta on the file it was restored from. */
+ * with the flag continues the chain: its next agr_snapshot is a delta on the file it was restored from — except after a
+ * relocating restore (below), which starts a new chain: its next agr_snapshot is a full file, and deltas follow on that file.
+ * Other capacities: agr_restore RELOCATES the restored state instead of loading it in place when the snapshot (the full file,
+ * or the last cut of a chain) is a ring and cfg's slab_rows, resp_bytes or (AGR_CFG_VARLEN) vslab_bytes differ from its own,
+ * or when the snapshot is append-only and cfg has AGR_CFG_RING.  Every other restore loads in place as before.  The id mode,
+ * record form and id_secret must still match, and a ring snapshot does not go into an append-only engine (AGR_EINVAL).  The
+ * live window [rows_tail, rows_used) keeps its row ids (minted ids keep resolving, ids outside it keep missing) and moves to
+ * row id mod the new slab_rows; the record bytes and the response / error bytes of the rows that hold one are packed from
+ * the start of the new byte rings; the completed / failed logs follow their rows (layout: DESIGN.md section 5).
+ * AGR_ENOSPC, with agr_last_error naming what did not fit and by how much, when the window is longer than slab_rows or the
+ * live record / response bytes exceed vslab_bytes / resp_bytes.  While it runs, the snapshot's state is held on the device
+ * in an engine of its own geometry next to the new one (freed before agr_restore returns): peak HBM is both engines, and
+ * AGR_ENOMEM (naming the relocation) when both do not fit. */
 int agr_snapshot(agr_handle* h, const char* path);
 int agr_restore(const agr_config* cfg, const char* path, agr_handle** out);
 /* The 24 h TTL of the record keys (SET ... EX 24h at requests.go:106,175,270; every SET restarts it, Q11).  Times are the
@@ -495,7 +507,10 @@ int agr_kernel_time(agr_handle* h, double* sum_ms, uint64_t* launches);
 /* With AGR_CFG_TIMING: device time (CUDA events on the launching stream) of the most recent kernel group:
  * which = 0 the K2 kernels of the last agr_complete, 1 the K3 select kernels of the last scan / pending / list,
  * 2 the K5 kernels of the last JSON encode (measure + scan + emit, including the host's read of the total between them),
- * 3 the cut of the last agr_snapshot with AGR_CFG_ONLINE_SNAPSHOT (the compare cut with AGR_CFG_DELTA_SNAPSHOT). */
+ * 3 the cut of the last agr_snapshot with AGR_CFG_ONLINE_SNAPSHOT (the compare cut with AGR_CFG_DELTA_SNAPSHOT),
+ * 4 the relocation kernels of the agr_restore that created h (see agr_restore: other capacities), including the host's read
+ * of the packed totals between them.  AGR_ENOTFOUND when the group has not run (which = 3 before any cut, which = 4 when h
+ * was not made by a relocating restore). */
 int agr_op_time(agr_handle* h, int which, double* ms);
 void* agr_slab_ptr(agr_handle* h, uint64_t rid); /* device address of a slab row */
 
