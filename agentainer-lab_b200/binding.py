@@ -119,6 +119,8 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
         "agr_submit_complete_large": (i32, [vp, vp, vp, u32, vp, u32, C.POINTER(u64)]),
         "agr_submit_complete": (i32, [vp, vp, C.POINTER(u64)]),
         "agr_wait": (i32, [vp, u64, vp]),
+        "agr_submit_ingest": (i32, [vp, vp, C.POINTER(u64)]),
+        "agr_poll": (i32, [vp, u64, vp]),
         "agr_replay_scan": (i32, [vp, vp, vp, u32, C.POINTER(u32)]),
         "agr_pending": (i32, [vp, C.c_char_p, vp, u32, C.POINTER(u32)]),
         "agr_get_record": (i32, [vp, C.c_char_p, vp, vp]),
@@ -542,6 +544,29 @@ class Engine:
         return rc, res
 
     # ---- tickets (AGR_CFG_COMBINE)
+    def submit_ingest(self, rec: np.ndarray) -> int:
+        """agr_submit_ingest: one record into the request ring; collect its answer with poll()."""
+        assert rec.dtype == record_dtype
+        r = np.ascontiguousarray(rec.reshape(1))
+        t = C.c_uint64()
+        while True:
+            rc = self.lib.agr_submit_ingest(self.h, _ptr(r), C.byref(t))
+            if rc != K.AGR_EAGAIN:
+                _check(self.lib, rc)
+                return int(t.value)
+
+    def poll(self, ticket: int, block: bool = True) -> Optional[dict]:
+        """agr_poll (block: agr_wait) on a record's ticket: {verdict, request_id, rid, result}, or None while undecided."""
+        out = (C.c_uint8 * 40)()
+        fn = self.lib.agr_wait if block else self.lib.agr_poll
+        rc = fn(self.h, C.c_uint64(ticket), C.cast(out, C.c_void_p))
+        if rc == K.AGR_EAGAIN:
+            return None
+        _check(self.lib, rc)
+        b = bytes(out)
+        return dict(verdict=np.frombuffer(b[:8], dtype=verdict_dtype).copy(), request_id=b[8:24],
+                    rid=int.from_bytes(b[24:32], "little"), result=int.from_bytes(b[32:36], "little", signed=True))
+
     def submit_complete(self, outcome: np.ndarray) -> int:
         assert outcome.dtype == outcome_dtype
         o = np.ascontiguousarray(outcome.reshape(1))

@@ -309,7 +309,11 @@ __device__ __forceinline__ void k1_flush_counters(const agr_dev& d, uint32_t* lc
 // Returns the row's final route word; delta = {dedupe hits, stored, queued} corrections for the global counters.
 // `marked`: the caller knows from K1's row marks that this row is a tracked replay, so the row's own route word and its
 // replay_of are fetched together, and the target row's two words together: two dependent round trips instead of four.
-__device__ __forceinline__ uint32_t k1_post_one(const agr_dev& d, const uint32_t rid, const uint32_t dupfix, int* delta, const bool marked = false) {
+// first_log: arrival number of the batch's first row.  (a) and (b) of different rows run in no particular order, so with
+// dupfix != 0 a target of this batch may not have been promoted yet when (a) reads its state word.  The row the index names
+// for an id is the id's owner, and a caller-id owner of this batch always ends up stored, so (a) takes that from its arrival.
+__device__ __forceinline__ uint32_t k1_post_one(const agr_dev& d, const uint32_t rid, const uint32_t dupfix, int* delta, const bool marked = false,
+                                                const unsigned long long first_log = ~0ULL) {
     uint4 t = make_uint4(0, 0, 0, 0);
     if (marked) t = __ldcg(reinterpret_cast<const uint4*>(rec_ptr(d, rid) + AGR_OFF_REPLAY_OF));
     uint32_t r = d.route[rid];
@@ -320,7 +324,9 @@ __device__ __forceinline__ uint32_t k1_post_one(const agr_dev& d, const uint32_t
         vf &= ~AGR_VF_DUP_ID;
         uint32_t oroute = 0u, ostate = 0u;
         if (orid != AGR_RID_NONE) { oroute = __ldcg(&d.route[orid]); ostate = __ldcg(&d.state[orid]); }
-        if (orid != AGR_RID_NONE && row_logical(d, orid) < row_logical(d, rid) && rt_slot(oroute) == rt_slot(r) && (ostate & ST_STORED)) {
+        const unsigned long long olog = orid != AGR_RID_NONE ? row_logical(d, orid) : ~0ULL;
+        const bool owner_here = dupfix != 0u && !(d.cfg_flags & AGR_CFG_MINT_IDS) && olog >= first_log;   // promoted, or about to be
+        if (orid != AGR_RID_NONE && olog < row_logical(d, rid) && rt_slot(oroute) == rt_slot(r) && ((ostate & ST_STORED) || owner_here)) {
             vf |= AGR_VF_KNOWN;
             delta[0]++;
         }

@@ -27,6 +27,7 @@ __global__ void __launch_bounds__(256) k1_post(const agr_dev d, const uint32_t f
     if (dupfix == 0u && __ldcg(d.dupfix + 2) == 0u && verdicts == nullptr && ids == nullptr) return;
     const uint32_t stride = gridDim.x * blockDim.x;
     const int lane = threadIdx.x & 31;
+    const unsigned long long first_log = row_logical(d, first_rid);
     int delta[3] = {0, 0, 0};                                                     // dedupe hits, stored, queued
     if (marks && dupfix == 0u && (d.cfg_flags & AGR_CFG_MINT_IDS) && verdicts == nullptr && ids == nullptr) {
         // minted ids: K1 has decided every replay that names a row of an earlier batch, so the few rows left are far apart.  One
@@ -42,7 +43,7 @@ __global__ void __launch_bounds__(256) k1_post(const agr_dev d, const uint32_t f
             const bool marked = marks && ((__ldg(&marks[i >> 5]) >> (i & 31u)) & 1u);
             if (marks && !marked && dupfix == 0u && verdicts == nullptr && ids == nullptr) continue;
             const uint32_t rid = first_rid + i;
-            const uint32_t r = k1_post_one(d, rid, dupfix, delta, marked);
+            const uint32_t r = k1_post_one(d, rid, dupfix, delta, marked, first_log);
             if (verdicts) verdicts[i] = k1_verdict_word(r);
             if (ids) ids[i] = k1_request_id(d, rid);
         }

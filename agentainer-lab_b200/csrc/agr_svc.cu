@@ -224,7 +224,9 @@ k_svc(const agr_dev d0, const svc_dev v, const agr_k2_scratch k2, const unsigned
             const k1_result r = k1_finish(d, rid, h1, h5, cx, lc);
             d.state[rid] = r.state;
             d.route[rid] = r.route;
-            if ((r.state & ST_STORED) && (d.cfg_flags & AGR_CFG_RING)) {         // TTL bookkeeping (see k1_note_time)
+            // TTL bookkeeping of every record row, as the batch kernel keeps it (k1_note_time): a row k1_post_one promotes below
+            // is stored without having been stored here
+            if (d.cfg_flags & AGR_CFG_RING) {
                 unsigned long long t = pack64(h4.x, h4.y);
                 atomicMin(d.cmin + rid / AGR_CHUNK_ROWS, t == 0ULL ? 1ULL : t == ~0ULL ? ~0ULL - 1ULL : t);   // 0 unknown, ~0 empty
                 d.mtime[rid] = t;
@@ -237,7 +239,7 @@ k_svc(const agr_dev d0, const svc_dev v, const agr_k2_scratch k2, const unsigned
             int delta[3] = {0, 0, 0};
             if (wt < nrec) {
                 const uint32_t rid = D.first_p + wt;
-                const uint32_t r = k1_post_one(d, rid, dupfix, delta);
+                const uint32_t r = k1_post_one(d, rid, dupfix, delta, false, D.first_l);
                 const unsigned long long slot_abs = from + s_rec_op[st][wt], lrow = D.first_l + wt;
                 const uint2 vw = k1_verdict_word(r);
                 st_res(v.res + (slot_abs & (SVC_SLOTS - 1u)), vw.x, vw.y, (uint32_t)lrow, (uint32_t)((lrow >> 32) & 0xffffu) | (svc_tag(slot_abs) << 16));
