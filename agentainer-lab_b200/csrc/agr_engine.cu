@@ -197,6 +197,11 @@ static int create_impl(const agr_config* cfg_in, agr_handle* h) {
         TRY(dev_alloc(h, &h->d_voffsets, (size_t)c.max_batch + 1, false));
         TRY(host_alloc(h, &h->h_voffsets, (size_t)c.max_batch + 1));
         TRY(dev_alloc(h, &h->d_tile_first, (size_t)(((size_t)c.max_batch * AGR_VT_MAXREC) / AGR_VT_TILE + 8), false));
+        // runs of 512-byte slots: up to 2 x max_batch (the exchange decides own + received rows), offsets below 2^32
+        h->slot_off_max = (uint32_t)std::min<uint64_t>(2ull * c.max_batch, (0xffffffffull / AGR_REC) - 1);
+        TRY(dev_alloc(h, &h->d_slot_off, (size_t)h->slot_off_max + 1, false));
+        agr_launch_slot_offsets(h->d_slot_off, h->slot_off_max, h->stream);
+        CK(cudaGetLastError());
     } else {
         TRY(dev_alloc(h, &d.slab, (size_t)c.slab_rows * AGR_REC, false));
     }
@@ -426,13 +431,42 @@ uint64_t ingested_bound(const agr_handle* h) {
     return b;
 }
 void resv_remove(agr_handle* h, uint64_t first, uint64_t end) {
-    std::vector<std::pair<uint64_t, uint64_t>> keep;
+    std::vector<resv_run> keep;
     for (const auto& r : h->resv) {
-        if (r.second <= first || r.first >= end) { keep.push_back(r); continue; }
-        if (r.first < first) keep.emplace_back(r.first, first);
-        if (r.second > end) keep.emplace_back(end, r.second);
+        if (r.end <= first || r.first >= end) { keep.push_back(r); continue; }
+        if (r.first < first) keep.push_back(resv_run{r.first, first, r.vbase});
+        if (r.end > end) keep.push_back(resv_run{end, r.end, r.vbase + (end - r.first) * AGR_REC});
     }
     h->resv.swap(keep);
+}
+// b continues a: the rows follow on (logically and physically: K1 numbers a run's rows from its first physical row) and so do
+// the slots (variable-length engines; a slot run never wraps the byte ring)
+static bool runs_adjoin(const agr_handle* h, uint64_t a_first, uint64_t a_end, uint64_t a_vbase, uint64_t b_first, uint64_t b_vbase) {
+    if (a_end != b_first) return false;
+    if (!(h->cfg.flags & AGR_CFG_VARLEN)) return true;
+    return phys_row(h, a_first) + (a_end - a_first) == phys_row(h, b_first) && a_vbase + (a_end - a_first) * AGR_REC == b_vbase;
+}
+// Variable-length engines: rows [first, first + n) as the runs whose slots lie back to back, in row order.  Every row must be
+// reserved and not decided yet (the resv list keeps the slots of those rows only).  Fixed-stride engines: the range itself.
+int row_runs(agr_handle* h, uint64_t first, uint32_t n, std::vector<slot_run>& out) {
+    out.clear();
+    if (!(h->cfg.flags & AGR_CFG_VARLEN)) {
+        if (n) out.push_back(slot_run{first, n, 0});
+        return 0;
+    }
+    for (uint64_t at = first, end = first + n; at < end;) {
+        const resv_run* r = nullptr;
+        for (const auto& q : h->resv) if (q.first <= at && at < q.end) { r = &q; break; }
+        if (!r) return fail(AGR_EINVAL, "variable-length engine: row " + std::to_string(at) + " is not a reserved row that awaits its record "
+                                        "(agr_reserve_rows hands out rows with 512-byte slots; a decided row has none)");
+        const uint64_t k = std::min(end, r->end) - at;
+        const slot_run s{at, (uint32_t)k, r->vbase + (at - r->first) * AGR_REC};
+        slot_run* b = out.empty() ? nullptr : &out.back();
+        if (b && runs_adjoin(h, b->first, b->first + b->n, b->vbase, s.first, s.vbase)) b->n += s.n;
+        else out.push_back(s);
+        at += k;
+    }
+    return 0;
 }
 // The cursor rule of the three rings (slab rows, variable-length record bytes, response bytes), in logical units: a piece of
 // `need` units never wraps — if it does not fit before the end of the lap, the rest of the lap is skipped (*pad units) — and
@@ -469,6 +503,45 @@ int reserve_rows_locked(agr_handle* h, uint32_t n, uint64_t* first) {
     *first = h->rows_used;
     h->rows_used += n;
     sync_window(h);
+    return 0;
+}
+
+// The byte ring of a variable-length engine takes `bytes` as one piece (a blob of agr_ingest_var, or the slots of one row
+// reservation): vbytes_fit checks (*vpad = the bytes skipped at the end of the lap), vbytes_take hands the piece out and
+// returns its physical offset.  The rows are reserved in between, so that a refused call leaves both rings as they were.
+static int vbytes_fit(const agr_handle* h, uint64_t bytes, uint64_t* vpad) {
+    *vpad = 0;
+    if (!is_ring(h)) {
+        if (h->vused + bytes > h->vcap) return fail(AGR_ENOSPC, "byte slab full");
+        return 0;
+    }
+    if (bytes > h->vcap / 2) return fail(AGR_EINVAL, "batch larger than half the byte slab");
+    if (!ring_fits(h->vused, h->vtail, h->vcap, bytes, vpad)) return fail(AGR_ENOSPC, "byte slab full: agr_expire + agr_reclaim release bytes at the tail");
+    if (!ring_fits_pinned(h, h->vused, h->vtail, h->pin_vtail, h->vcap, bytes)) return fail(AGR_ENOSPC, std::string("byte slab ") + PINNED_FULL);
+    return 0;
+}
+static uint64_t vbytes_take(agr_handle* h, uint64_t bytes, uint64_t vpad) {
+    h->vused += vpad;
+    const uint64_t base = is_ring(h) ? h->vused % h->vcap : h->vused;
+    h->vused += bytes;
+    return base;
+}
+
+// n rows and, on a variable-length engine, their n consecutive 512-byte slots.  listed: the rows wait for agr_fill_rows /
+// agr_ingest_rows (agr_reserve_rows), so they go on the resv list; the exchange's own reservations are decided in the same
+// call and are not listed.
+int reserve_run_locked(agr_handle* h, uint32_t n, bool listed, slot_run* run) {
+    const bool varlen = (h->cfg.flags & AGR_CFG_VARLEN) != 0 && n;
+    uint64_t vpad = 0;
+    if (varlen) TRY(vbytes_fit(h, (uint64_t)n * AGR_REC, &vpad));
+    TRY(reserve_rows_locked(h, n, &run->first));
+    run->n = n;
+    run->vbase = varlen ? vbytes_take(h, (uint64_t)n * AGR_REC, vpad) : 0;
+    if (listed && n) {
+        resv_run* b = h->resv.empty() ? nullptr : &h->resv.back();
+        if (b && runs_adjoin(h, b->first, b->end, b->vbase, run->first, run->vbase)) b->end += n;   // back-to-back reservations merge
+        else h->resv.push_back(resv_run{run->first, run->first + n, run->vbase});
+    }
     return 0;
 }
 
@@ -516,6 +589,34 @@ int launch_k1_locked(agr_handle* h, uint64_t first, uint32_t n, agr_verdict* d_o
     CK(cudaGetLastError());
     return 0;
 }
+
+// K1v and its post pass over rows [first, first + n) of a variable-length engine, whose records lie at physical byte `base` of
+// the byte slab, record i at d_off[i] .. d_off[i + 1] from there (`bytes` in all)
+static int launch_k1v_locked(agr_handle* h, uint64_t first, uint32_t n, uint64_t base, const uint32_t* d_off, uint64_t bytes,
+                             agr_verdict* d_out, uint8_t* d_ids) {
+    cudaStream_t st = h->stream;
+    sync_window(h);
+    flip_batch_words(h);
+    cudaEvent_t e0 = nullptr, e1 = nullptr;
+    if (h->cfg.flags & AGR_CFG_TIMING) {
+        TRY(claim_k1_events(h, &e0, &e1));
+        CK(cudaEventRecord(e0, st));
+    }
+    CK(agr_launch_k1_var(h->d, h->d.slab + base, d_off, n, bytes, h->d_tile_first, (uint32_t)phys_row(h, first), base, h->sm_count, st, h->cfg.k1_variant));
+    if (e1) CK(cudaEventRecord(e1, st));
+    agr_launch_k1_post(h->d, (uint32_t)phys_row(h, first), n, h->sm_count, st, d_out, d_ids);
+    h->k1_launches += 3;
+    CK(cudaGetLastError());
+    return 0;
+}
+
+// K1 over one run: the fixed-stride kernel, or K1v reading the run's 512-byte slots as a blob with offsets 512 i
+int decide_run_locked(agr_handle* h, const slot_run& r, agr_verdict* d_out) {
+    if (!(h->cfg.flags & AGR_CFG_VARLEN)) return launch_k1_locked(h, r.first, r.n, d_out);
+    if (r.n == 0) return 0;
+    if (r.n > h->slot_off_max) return fail(AGR_EINVAL, "more slots in one run than K1v's offsets reach");
+    return launch_k1v_locked(h, r.first, r.n, r.vbase, h->d_slot_off, (uint64_t)r.n * AGR_REC, d_out, nullptr);
+}
 }  // namespace agr_impl
 extern "C" {
 
@@ -523,7 +624,19 @@ static int ingest_rows_locked(agr_handle* h, uint64_t first, uint32_t n, agr_ver
     if (first + n > h->rows_used) return fail(AGR_EINVAL, "rows not reserved");
     if (n > h->cfg.max_batch) return fail(AGR_EINVAL, "n exceeds max_batch");
     if (n == 0) return 0;
-    TRY(launch_k1_locked(h, first, n, out ? h->d_verdicts : nullptr));
+    if (!(h->cfg.flags & AGR_CFG_VARLEN)) {
+        TRY(launch_k1_locked(h, first, n, out ? h->d_verdicts : nullptr));
+    } else {
+        // one K1v per run of back-to-back slots: a range across a skip of the byte ring is decided as the reservations on either
+        // side of the skip would be on their own
+        std::vector<slot_run> runs;
+        TRY(row_runs(h, first, n, runs));
+        uint32_t done = 0;
+        for (const slot_run& r : runs) {
+            TRY(decide_run_locked(h, r, out ? h->d_verdicts + done : nullptr));
+            done += r.n;
+        }
+    }
     if (!h->resv.empty()) resv_remove(h, first, first + n);
     if (out) {
         TRY(d2h_staged(h, out, h->d_verdicts, (size_t)n * sizeof(agr_verdict), h->h_verdicts));
@@ -547,19 +660,27 @@ int agr_mint_ids(agr_handle* h, uint64_t first_rid, uint32_t n, uint8_t (*ids)[1
 int agr_reserve_rows(agr_handle* h, uint32_t n, uint64_t* first_rid) {
     if (!h || !first_rid) return fail(AGR_EINVAL, "NULL argument");
     HLock lk(h);
-    TRY(reserve_rows_locked(h, n, first_rid));
-    if (n) {
-        if (!h->resv.empty() && h->resv.back().second == *first_rid) h->resv.back().second += n;   // back-to-back reservations merge
-        else h->resv.emplace_back(*first_rid, *first_rid + n);
-    }
+    slot_run r;
+    TRY(reserve_run_locked(h, n, true, &r));
+    *first_rid = r.first;
     return 0;
 }
 int agr_fill_rows(agr_handle* h, uint64_t first_rid, const agr_record* recs, uint32_t n) {
     if (!h || (n && !recs)) return fail(AGR_EINVAL, "NULL argument");
     HLock lk(h);
     CK(cudaSetDevice(h->device));
-    if (h->cfg.flags & AGR_CFG_VARLEN) return fail(AGR_EINVAL, "fixed-stride engines only");
     if (first_rid + n > h->rows_used || first_rid < h->tail) return fail(AGR_EINVAL, "rows not reserved");
+    if (h->cfg.flags & AGR_CFG_VARLEN) {                         // into the rows' slots of the byte ring
+        std::vector<slot_run> runs;
+        TRY(row_runs(h, first_rid, n, runs));
+        uint32_t done = 0;
+        for (const slot_run& r : runs) {
+            CK(cudaMemcpyAsync(run_ptr(h, r), recs + done, (size_t)r.n * AGR_REC, cudaMemcpyHostToDevice, h->stream));
+            done += r.n;
+        }
+        CK(cudaStreamSynchronize(h->stream));
+        return 0;
+    }
     if (n == 0) return 0;
     if (phys_row(h, first_rid) + n > h->cfg.slab_rows) return fail(AGR_EINVAL, "row range wraps");
     CK(cudaMemcpyAsync(h->d.slab + phys_row(h, first_rid) * AGR_REC, recs, (size_t)n * AGR_REC, cudaMemcpyHostToDevice, h->stream));
@@ -587,6 +708,11 @@ int agr_sync(agr_handle* h) {
 void* agr_stream(agr_handle* h) { return h ? (void*)h->stream : nullptr; }
 void* agr_slab_ptr(agr_handle* h, uint64_t rid) {
     if (!h || rid >= h->rows_used || rid < h->tail) return nullptr;
+    if (h->cfg.flags & AGR_CFG_VARLEN) {                         // a reserved row that awaits its record: its 512-byte slot
+        HLock lk(h);
+        for (const auto& r : h->resv)
+            if (r.first <= rid && rid < r.end) return (void*)(h->d.slab + r.vbase + (rid - r.first) * AGR_REC);
+    }
     return (void*)(h->d.slab + phys_row(h, rid) * AGR_REC);
 }
 
@@ -971,33 +1097,14 @@ int agr_ingest_var(agr_handle* h, const uint8_t* blob, const uint32_t* offsets, 
             return fail(AGR_EINVAL, "record " + std::to_string(i) + ": length must be a multiple of 16 in [96, 8192]");
     }
     uint64_t vpad = 0;
-    if (!is_ring(h)) {
-        if (h->vused + bytes > h->vcap) return fail(AGR_ENOSPC, "byte slab full");
-    } else {                                                      // byte ring: a blob never wraps either
-        if (bytes > h->vcap / 2) return fail(AGR_EINVAL, "batch larger than half the byte slab");
-        if (!ring_fits(h->vused, h->vtail, h->vcap, bytes, &vpad)) return fail(AGR_ENOSPC, "byte slab full: agr_expire + agr_reclaim release bytes at the tail");
-        if (!ring_fits_pinned(h, h->vused, h->vtail, h->pin_vtail, h->vcap, bytes)) return fail(AGR_ENOSPC, std::string("byte slab ") + PINNED_FULL);
-    }
+    TRY(vbytes_fit(h, bytes, &vpad));                             // (byte ring: a blob never wraps either)
     TRY(reserve_rows_locked(h, n, &first));
     if (first_rid) *first_rid = first;
-    h->vused += vpad;
-    const uint64_t base = is_ring(h) ? h->vused % h->vcap : h->vused;          // physical byte offset of the blob
-    h->vused += bytes;
+    const uint64_t base = vbytes_take(h, bytes, vpad);            // physical byte offset of the blob
     cudaStream_t st = h->stream;
     CK(cudaMemcpyAsync(h->d.slab + base, blob, bytes, cudaMemcpyHostToDevice, st));
     TRY(h2d_staged(h, h->d_voffsets, offsets, ((size_t)n + 1) * 4, h->h_voffsets));
-    sync_window(h);
-    flip_batch_words(h);
-    cudaEvent_t e0 = nullptr, e1 = nullptr;
-    if (h->cfg.flags & AGR_CFG_TIMING) {
-        TRY(claim_k1_events(h, &e0, &e1));
-        CK(cudaEventRecord(e0, st));
-    }
-    CK(agr_launch_k1_var(h->d, h->d.slab + base, h->d_voffsets, n, bytes, h->d_tile_first, (uint32_t)phys_row(h, first), base, h->sm_count, st, h->cfg.k1_variant));
-    if (e1) CK(cudaEventRecord(e1, st));
-    agr_launch_k1_post(h->d, (uint32_t)phys_row(h, first), n, h->sm_count, st, out ? h->d_verdicts : nullptr, ids ? h->d_ids : nullptr);
-    h->k1_launches += 3;
-    CK(cudaGetLastError());
+    TRY(launch_k1v_locked(h, first, n, base, h->d_voffsets, bytes, out ? h->d_verdicts : nullptr, ids ? h->d_ids : nullptr));
     if (out) CK(cudaMemcpyAsync(h->h_verdicts, h->d_verdicts, (size_t)n * sizeof(agr_verdict), cudaMemcpyDeviceToHost, st));
     if (ids) CK(cudaMemcpyAsync(h->h_ids, h->d_ids, (size_t)n * 16, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
@@ -1310,7 +1417,11 @@ static int reclaim_apply(agr_handle* h, uint64_t* released) {
         h->resp_tail = h->resp_used - span;
         h->k3_launches += 1;
     }
-    if (h->cfg.flags & AGR_CFG_VARLEN) {                          // the byte ring's tail follows: first byte of the first live record
+    // The byte ring's tail follows: first byte of the first live record.  It never passes the slot of a reserved row that K1 has
+    // not decided yet: the scan stops at `bound` (ingested_bound: the first such row), bytes are handed out in row order under the
+    // handle mutex (reserve_run_locked, agr_ingest_var), so the live record found below the bound lies before every such slot,
+    // and with none found the tail moves to vused only when no row is reserved at all.
+    if (h->cfg.flags & AGR_CFG_VARLEN) {
         if (r.off == 0xffffffffu) h->vtail = (bound == h->rows_used) ? h->vused : h->vtail;
         else {
             uint64_t used = (h->vused % h->vcap + h->vcap - r.voff) % h->vcap;
@@ -1579,6 +1690,8 @@ int agr_synth_fill_rows(agr_handle* h, const agr_synth* s, uint64_t first_index,
     HLock lk(h);
     CK(cudaSetDevice(h->device));
     if (first_rid + n > h->rows_used) return fail(AGR_EINVAL, "rows not reserved");
+    std::vector<slot_run> runs;                                  // (variable-length engines: the rows' slots)
+    TRY(row_runs(h, first_rid, n, runs));
     const unsigned long long* dcdf = nullptr;
     if (s->zipf_milli) {
         std::vector<unsigned long long> cdf;
@@ -1588,7 +1701,11 @@ int agr_synth_fill_rows(agr_handle* h, const agr_synth* s, uint64_t first_index,
         CK(cudaStreamSynchronize(h->stream));
         dcdf = h->d_cdf.p;
     }
-    agr_launch_synth(h->d.slab + phys_row(h, first_rid) * AGR_REC, synth_params(s, dcdf), first_index, n, h->stream);
+    uint32_t done = 0;
+    for (const slot_run& r : runs) {
+        agr_launch_synth(run_ptr(h, r), synth_params(s, dcdf), first_index + done, r.n, h->stream);
+        done += r.n;
+    }
     CK(cudaGetLastError());                                      // (stream-ordered before whatever reads the rows: no wait here)
     return 0;
 }

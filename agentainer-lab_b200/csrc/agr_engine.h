@@ -36,6 +36,18 @@ struct exchange_plan {
     uint32_t recv_res_base = 0;      // index of the first received item's result in the result array
 };
 
+// Rows [first, first + n) whose records lie back to back.  On a variable-length engine a row that agr_reserve_rows (or the
+// exchange) hands out owns a 512-byte slot of the byte ring: the record of row first + i is at physical byte vbase + 512 i.
+struct slot_run {
+    uint64_t first = 0;
+    uint32_t n = 0;
+    uint64_t vbase = 0;          // (variable-length engines only)
+};
+// a reservation of agr_reserve_rows that K1 has not decided yet: rows [first, end), slots from vbase (variable-length engines)
+struct resv_run {
+    uint64_t first, end, vbase;
+};
+
 // grow-only scratch: a buffer and the element count it was allocated with (regrow sets both)
 template <typename T>
 struct scratch {
@@ -130,7 +142,7 @@ struct agr_handle {
     uint32_t* d_hrid = nullptr;                // rows found by the single-key resolve (k_resolve)
     uint32_t* h_k2flag = nullptr;              // pinned: k2_append's overflow flag of the last batch
     agr_dop* d_ops = nullptr;
-    std::vector<std::pair<uint64_t, uint64_t>> resv;   // rows handed out by agr_reserve_rows and not ingested yet: [first, end)
+    std::vector<resv_run> resv;                // rows handed out by agr_reserve_rows and not ingested yet, in row order
     // K3
     scratch<uint32_t> d_matrix, d_cta_matrix;
     scratch<uint32_t> d_selmask;               // one selection bit per scanned item (k3_mark -> k3_place)
@@ -167,6 +179,8 @@ struct agr_handle {
     uint64_t vtail = 0;                        // ring: logical offset of the first byte that has not been released
     uint32_t* d_voffsets = nullptr; uint32_t* d_tile_first = nullptr;   // per-batch offsets [max_batch+1], tile index
     uint32_t* h_voffsets = nullptr;
+    uint32_t* d_slot_off = nullptr;            // 512 i for i = 0 .. slot_off_max: the offsets of a run of 512-byte slots (K1v)
+    uint32_t slot_off_max = 0;
     scratch<uint32_t> d_lens; scratch<unsigned long long> d_goffs;      // gather scratch
     // multi-GPU exchange (K4)
     ncclComm_t comm = nullptr; int rank = 0, world = 1;
@@ -287,9 +301,15 @@ int set_agent_state_locked(agr_handle* h, const char* agent_id, uint8_t status, 
 uint64_t ingested_bound(const agr_handle* h);
 void resv_remove(agr_handle* h, uint64_t first, uint64_t end);
 int reserve_rows_locked(agr_handle* h, uint32_t n, uint64_t* first);
+int reserve_run_locked(agr_handle* h, uint32_t n, bool listed, slot_run* run);
+int row_runs(agr_handle* h, uint64_t first, uint32_t n, std::vector<slot_run>& out);
 int op_time_begin(agr_handle* h, int g);
 int op_time_end(agr_handle* h, int g);
 int launch_k1_locked(agr_handle* h, uint64_t first, uint32_t n, agr_verdict* d_out, uint8_t* d_ids = nullptr);
+int decide_run_locked(agr_handle* h, const slot_run& r, agr_verdict* d_out);
+static inline uint8_t* run_ptr(const agr_handle* h, const slot_run& r) {   // where the run's first record lies
+    return (h->cfg.flags & AGR_CFG_VARLEN) ? h->d.slab + r.vbase : h->d.slab + phys_row(h, r.first) * AGR_REC;
+}
 int resp_reserve_locked(agr_handle* h, uint64_t need, uint64_t len, unsigned long long* off);
 int check_segments(const agr_outcome* outs, uint32_t n, const uint64_t* offsets, const uint32_t* hdr_lens, uint64_t* total,
                    uint64_t* max_len);

@@ -181,20 +181,34 @@ static void exchange_fill_info(const exchange_plan& x, uint32_t n, uint64_t firs
 // Its stages: K4 count + scan over the rows, then (after the counts are known) sharded_rows_local, the all-to-all of the records,
 // K1 over the received rows, the all-to-all of their verdicts, and sharded_rows_finish.  agr_debug_exchange_begin / _end run the
 // same stages with the test in place of the two all-to-alls.
-static uint8_t* batch_rows(agr_handle* h, uint64_t first) { return h->d.slab + phys_row(h, first) * AGR_REC; }
+// Variable-length engines: the batch's rows own 512-byte slots of the byte ring, and records cross shards in that fixed form (a
+// cross-shard record is a replay re-injection: only its header decides it).  K4 bins the slots exactly as it bins slab rows, and
+// K1v decides them (decide_run_locked).  The batch's slots must lie back to back: a row range across a skip of the byte ring is
+// refused.
+static int exchange_run(agr_handle* h, uint64_t first, uint32_t n, slot_run* run) {
+    *run = slot_run{first, n, 0};
+    if (!(h->cfg.flags & AGR_CFG_VARLEN) || n == 0) return 0;
+    std::vector<slot_run> runs;
+    TRY(row_runs(h, first, n, runs));
+    if (runs.size() != 1)
+        return fail(AGR_EINVAL, "the rows' 512-byte slots are not back to back (the byte ring skipped to its start between two "
+                                "reservations): exchange each reservation on its own");
+    *run = runs[0];
+    return 0;
+}
 // rows for the records that arrive, the peers' records packed for shipping, K1 over the batch's own rows (the rows of the records
 // K4 packed are holes: K1 skips them by K4's owner array, AGR_CFGI_HOLES) — runs while the all-to-all moves the peers' records
-static int sharded_rows_local(agr_handle* h, uint64_t first, exchange_plan& x, uint64_t* first2) {
+static int sharded_rows_local(agr_handle* h, const slot_run& own, exchange_plan& x, slot_run* recv) {
     const uint32_t n = x.p.n;
-    *first2 = h->rows_used;
-    if (x.n_recv) TRY(reserve_rows_locked(h, x.n_recv, first2));
+    *recv = slot_run{h->rows_used, 0, 0};
+    if (x.n_recv) TRY(reserve_run_locked(h, x.n_recv, false, recv));
     const uint32_t n_remote = n - x.n_local;
     x.p.local_dst = nullptr; x.p.send_dst = h->d_send;
     if (n_remote) { agr_launch_k4_scatter(x.p, h->stream); h->k4_launches += 1; CK(cudaGetLastError()); }
     if (n) {
         const uint32_t keep = h->d.cfg_flags;
         if (n_remote) h->d.cfg_flags |= AGR_CFGI_HOLES;
-        const int rc = launch_k1_locked(h, first, n, h->d_xverd);
+        const int rc = decide_run_locked(h, own, h->d_xverd);
         h->d.cfg_flags = keep;
         TRY(rc);
     }
@@ -208,18 +222,19 @@ static int sharded_rows_finish(agr_handle* h, const exchange_plan& x, uint64_t f
     exchange_fill_info(x, n, first, first2, info);
     return 0;
 }
-static int sharded_rows_locked(agr_handle* h, uint64_t first, uint32_t n, agr_verdict* out, agr_exchange_info* info) {
+static int sharded_rows_locked(agr_handle* h, const slot_run& own, agr_verdict* out, agr_exchange_info* info) {
+    const uint32_t n = own.n;
     exchange_plan x;
-    TRY(exchange_begin(h, batch_rows(h, first), AGR_REC, AGR_OFF_AGENT_ID, n, true, x));
-    uint64_t first2 = 0;
-    TRY(sharded_rows_local(h, first, x, &first2));
-    // the all-to-all: every peer segment to its owner, landing directly in the owner's slab rows
-    TRY(exchange_payload(h, x, h->d_send, batch_rows(h, first2), AGR_REC));
+    TRY(exchange_begin(h, run_ptr(h, own), AGR_REC, AGR_OFF_AGENT_ID, n, true, x));
+    slot_run recv;
+    TRY(sharded_rows_local(h, own, x, &recv));
+    // the all-to-all: every peer segment to its owner, landing directly in the owner's slab rows (slots)
+    TRY(exchange_payload(h, x, h->d_send, run_ptr(h, recv), AGR_REC));
     // K1 at the owner over the received rows (own host's records first, then peers by rank: the merge order)
-    if (x.n_recv) TRY(launch_k1_locked(h, first2, x.n_recv, h->d_xverd + n));
+    if (x.n_recv) TRY(decide_run_locked(h, recv, h->d_xverd + n));
     // verdicts back to where the records came from, restored to the caller's order
     TRY(exchange_results(h, x, (const uint8_t*)h->d_xverd, (uint8_t*)h->d_vback, (uint8_t*)h->d_vout, sizeof(agr_verdict)));
-    return sharded_rows_finish(h, x, first, first2, out, info);
+    return sharded_rows_finish(h, x, own.first, recv.first, out, info);
 }
 
 int agr_ingest_sharded(agr_handle* h, const agr_record* recs, uint32_t n, agr_verdict* out, agr_exchange_info* info) {
@@ -228,19 +243,19 @@ int agr_ingest_sharded(agr_handle* h, const agr_record* recs, uint32_t n, agr_ve
     CK(cudaSetDevice(h->device));
     if (!h->comm) return fail(AGR_ECOMM, "agr_comm_init has not been called on this handle");
     if (n > h->cfg.max_batch) return fail(AGR_EINVAL, "n exceeds max_batch");
-    uint64_t first = h->rows_used;
+    slot_run own{h->rows_used, 0, 0};
     if (n) {
-        TRY(reserve_rows_locked(h, n, &first));
-        // the batch goes STRAIGHT into its slab rows, on the copy stream
+        TRY(reserve_run_locked(h, n, false, &own));
+        // the batch goes STRAIGHT into its slab rows (slots), on the copy stream
         TRY(grow_events(h->chunk_ev, 2));
         CK(cudaEventRecord(h->chunk_ev[0], h->stream));
         CK(cudaStreamWaitEvent(h->copy_stream, h->chunk_ev[0], 0));
         int bk = 0;
-        TRY(upload_rows(h, batch_rows(h, first), (const uint8_t*)recs, (size_t)n * AGR_REC, is_pinned(recs), bk));
+        TRY(upload_rows(h, run_ptr(h, own), (const uint8_t*)recs, (size_t)n * AGR_REC, is_pinned(recs), bk));
         CK(cudaEventRecord(h->chunk_ev[1], h->copy_stream));
         CK(cudaStreamWaitEvent(h->stream, h->chunk_ev[1], 0));
     }
-    return sharded_rows_locked(h, first, n, out, info);
+    return sharded_rows_locked(h, own, out, info);
 }
 // The same over rows the caller reserved (agr_reserve_rows) and filled on the device: the exchange with the batch resident in HBM.
 int agr_ingest_sharded_rows(agr_handle* h, uint64_t first_rid, uint32_t n, agr_verdict* out, agr_exchange_info* info) {
@@ -250,8 +265,10 @@ int agr_ingest_sharded_rows(agr_handle* h, uint64_t first_rid, uint32_t n, agr_v
     if (!h->comm) return fail(AGR_ECOMM, "agr_comm_init has not been called on this handle");
     if (first_rid + n > h->rows_used) return fail(AGR_EINVAL, "rows not reserved");
     if (n > h->cfg.max_batch) return fail(AGR_EINVAL, "n exceeds max_batch");
+    slot_run own;
+    TRY(exchange_run(h, first_rid, n, &own));
     if (!h->resv.empty()) resv_remove(h, first_rid, first_rid + n);
-    return sharded_rows_locked(h, first_rid, n, out, info);
+    return sharded_rows_locked(h, own, out, info);
 }
 
 int agr_complete_sharded(agr_handle* h, const agr_outcome* outs, uint32_t n, int32_t* results, agr_exchange_info* info) {
@@ -353,18 +370,20 @@ int agr_debug_exchange_begin(agr_handle* h, uint64_t first_rid, uint32_t n, agr_
     if (!h->d_k4cnt || h->comm) return fail(AGR_EINVAL, "agr_debug_world has not been called on this handle");
     if (h->xdbg_open) return fail(AGR_EINVAL, "an agr_debug_exchange_begin is waiting for its agr_debug_exchange_end");
     if (first_rid + n > h->rows_used) return fail(AGR_EINVAL, "rows not reserved");
+    slot_run own;
+    TRY(exchange_run(h, first_rid, n, &own));
     if (!h->resv.empty()) resv_remove(h, first_rid, first_rid + n);
     exchange_plan& x = h->xdbg;
     x = exchange_plan{};
-    TRY(exchange_count(h, batch_rows(h, first_rid), AGR_REC, AGR_OFF_AGENT_ID, n, true, x));
+    TRY(exchange_count(h, run_ptr(h, own), AGR_REC, AGR_OFF_AGENT_ID, n, true, x));
     CK(cudaMemsetAsync(k4_rcnt(h), 0, 32 * sizeof(uint32_t), h->stream));   // the peers' records arrive through agr_ingest_rows instead
     TRY(exchange_layout(h, x));
-    uint64_t first2 = 0;
-    TRY(sharded_rows_local(h, first_rid, x, &first2));
+    slot_run recv;
+    TRY(sharded_rows_local(h, own, x, &recv));
     const uint32_t n_sent = n - x.n_local;
     if (n_sent) CK(cudaMemcpyAsync(send_out, h->d_send, (size_t)n_sent * AGR_REC, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
-    exchange_fill_info(x, n, first_rid, first2, info);
+    exchange_fill_info(x, n, first_rid, recv.first, info);
     h->xdbg_first = first_rid; h->xdbg_n = n; h->xdbg_open = true;
     return 0;
 }

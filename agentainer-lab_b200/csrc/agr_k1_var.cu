@@ -367,6 +367,15 @@ cudaError_t agr_launch_k1_var(const agr_dev& d, const uint8_t* blob, const uint3
     k1_ingest_var<WARPS><<<blocks, WARPS * 32, smem, st>>>(d, blob, off, tile_first, ntiles, first_rid, blob_base);
     return cudaGetLastError();
 }
+// A run of rows reserved with agr_reserve_rows (or by the exchange) on a variable-length engine holds 512-byte records back to
+// back: K1v reads it as a blob whose offsets are 512 i.
+__global__ void __launch_bounds__(256) k1v_slot_offsets(uint32_t* __restrict__ off, const uint32_t n) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i <= n) off[i] = i * (uint32_t)AGR_REC;
+}
+void agr_launch_slot_offsets(uint32_t* off, uint32_t n, cudaStream_t st) {
+    k1v_slot_offsets<<<(n + 1 + 255u) / 256u, 256, 0, st>>>(off, n);
+}
 void agr_launch_var_lens(const agr_dev& d, const uint32_t* rids, uint32_t n, uint32_t* lens, cudaStream_t st) {
     if (n) k_var_lens<<<(n + 255u) / 256u, 256, 0, st>>>(d, rids, n, lens);
 }

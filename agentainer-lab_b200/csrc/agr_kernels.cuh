@@ -130,6 +130,8 @@ struct agr_k3_params {
 cudaError_t agr_launch_k1_var(const agr_dev& d, const uint8_t* blob, const uint32_t* off, uint32_t n, unsigned long long blob_bytes,
                               uint32_t* tile_first, uint32_t first_rid, unsigned long long blob_base, int sm_count, cudaStream_t st,
                               uint32_t variant = 0 /* k1_variant: bit 0x20 = LSU form */);
+// off[i] = 512 i for i = 0 .. n: the offsets K1v reads a run of 512-byte slots by
+void agr_launch_slot_offsets(uint32_t* off, uint32_t n, cudaStream_t st);
 void agr_launch_var_lens(const agr_dev& d, const uint32_t* rids, uint32_t n, uint32_t* lens, cudaStream_t st);
 void agr_launch_var_copy(const agr_dev& d, const uint32_t* rids, uint32_t n, const unsigned long long* out_off, uint8_t* out, cudaStream_t st);
 #define AGR_VT_TILE 8192u   // lower bound of the tile size used by agr_k1_var.cu (sizes the tile index)

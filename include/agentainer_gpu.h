@@ -493,7 +493,15 @@ int agr_mint_ids(agr_handle* h, uint64_t first_rid, uint32_t n, uint8_t (*ids)[1
 
 /* Split form of agr_ingest for callers that keep the batch resident on the device (bench "value" leg, and the
  * receive side of the multi-GPU exchange): reserve rows, fill them (agr_synth_fill_rows or a DMA of the caller's
- * own), then run K1 over them.  verdicts may be NULL (they stay on the device). */
+ * own), then run K1 over them.  verdicts may be NULL (they stay on the device).
+ * AGR_CFG_VARLEN: every reserved row owns a 512-byte slot of the byte slab, the slots of one reservation back to back (in
+ * ring mode they never wrap: the byte ring skips to its start as for an agr_ingest_var blob; AGR_ENOSPC when the byte slab is
+ * full or would reach the window of an online snapshot being written, AGR_EINVAL above half the byte ring).  A filled slot is
+ * decided by the variable-length kernel as a record of stored length 512 (payload rule of agr_record: path + headers + body
+ * > 416 B is AGR_VF_BAD_LEN): the result is that of agr_ingest_var with the same records as one blob at offsets 512 i, and the
+ * *_var reads return such a record as 512 bytes.  agr_fill_rows, agr_ingest_rows(_async) and agr_synth_fill_rows take
+ * reserved rows that have not been decided yet (AGR_EINVAL otherwise); a range across a skip of the byte ring is decided
+ * as the reservations on either side of it would be on their own. */
 int agr_reserve_rows(agr_handle* h, uint32_t n, uint64_t* first_rid);
 int agr_fill_rows(agr_handle* h, uint64_t first_rid, const agr_record* recs, uint32_t n);   /* DMA host records into reserved rows (no K1) */
 int agr_ingest_rows(agr_handle* h, uint64_t first_rid, uint32_t n, agr_verdict* out);
@@ -512,7 +520,8 @@ int agr_kernel_time(agr_handle* h, double* sum_ms, uint64_t* launches);
  * of the packed totals between them.  AGR_ENOTFOUND when the group has not run (which = 3 before any cut, which = 4 when h
  * was not made by a relocating restore). */
 int agr_op_time(agr_handle* h, int which, double* ms);
-void* agr_slab_ptr(agr_handle* h, uint64_t rid); /* device address of a slab row */
+void* agr_slab_ptr(agr_handle* h, uint64_t rid); /* device address of a slab row (AGR_CFG_VARLEN: of a reserved, undecided row's
+                                                   512-byte slot; any other row: byte slab + 512 x its physical row) */
 
 /* ------------------------------------------------------------ multi-GPU exchange (K4) */
 /* One handle per GPU; shard owner of an agent = agr_agent_shard(id, world).  Fresh traffic is steered to the owner by
@@ -535,7 +544,11 @@ typedef struct agr_exchange_info {
     uint64_t recv_first_rid;                   /* rows [recv_first_rid, +n_received): the records received, grouped by source rank */
 } agr_exchange_info;
 int agr_ingest_sharded(agr_handle* h, const agr_record* recs, uint32_t n, agr_verdict* out, agr_exchange_info* info);
-/* The same exchange over a batch that is already resident in rows [first_rid, +n) (agr_reserve_rows + a fill on the device). */
+/* The same exchange over a batch that is already resident in rows [first_rid, +n) (agr_reserve_rows + a fill on the device).
+ * AGR_CFG_VARLEN (both calls): records cross shards in the fixed 512-byte form.  The batch lies in 512-byte slots of the byte
+ * slab, and the received records land in slots reserved at their owner; the variable-length kernel decides both
+ * (see agr_reserve_rows).  The slots of rows [first_rid, +n) must lie back to back: a range across a skip of the byte ring is
+ * AGR_EINVAL.  agr_complete_sharded does not depend on the record form. */
 int agr_ingest_sharded_rows(agr_handle* h, uint64_t first_rid, uint32_t n, agr_verdict* out, agr_exchange_info* info);
 /* The same route for outcomes (cross-shard replay reconciliation): an outcome reported at a shard that does not own the
  * agent (the worker of shard A replayed through shard B's proxy) is shipped to the owner, applied there by K2 in
