@@ -12,7 +12,7 @@ OBJDIR = os.path.join(LIBDIR, "obj")
 LIBNAME = "libagentainer_b200.so"
 SOURCES = ["agr_kernels.cu", "agr_k1_tma.cu", "agr_k1_var.cu", "agr_k4.cu", "agr_k5_json.cu", "agr_svc.cu", "agr_json_host.cpp", "agr_engine.cu",
            "agr_front.cu", "agr_snapshot.cu", "agr_exchange.cu", "agr_relayout.cu"]
-HEADERS = ["agr_common.h", "agr_synth.h", "agr_kernels.cuh", "agr_device.cuh", "agr_svc.h", "agr_ring.hpp", "agr_engine.h",
+HEADERS = ["agr_common.h", "agr_agents.hpp", "agr_synth.h", "agr_kernels.cuh", "agr_device.cuh", "agr_svc.h", "agr_ring.hpp", "agr_engine.h",
            os.path.join("..", "..", "include", "agentainer_gpu.h")]
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]   # H100 (Hopper): TMA, mbarrier
 NVCC_FLAGS = GENCODE + ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC"]

@@ -111,12 +111,6 @@ int chunk_bounds_unknown(agr_handle* h) {
 
 static uint64_t next_pow2(uint64_t v) { uint64_t p = 1; while (p < v) p <<= 1; return p; }
 
-static void pack_agent_id(const char* id, unsigned long long w[4]) {
-    char buf[AGR_AGENT_ID_BYTES];
-    memset(buf, 0, sizeof buf);
-    strncpy(buf, id, AGR_AGENT_ID_BYTES - 1);
-    memcpy(w, buf, 32);
-}
 }  // namespace agr_impl
 
 extern "C" {
@@ -333,6 +327,112 @@ int push_agent_status(agr_handle* h, uint32_t slot, uint8_t status) {
     return 0;
 }
 
+// ---- slot reuse.  A slot is held while a row of the live window [tail, rows_used) records a decision for it (verdict code != 0 and
+// the route word's slot): AGR_V_NOT_FOUND rows (RT_SLOT_NONE), exchange holes, rows skipped at the end of a lap, released rows and
+// reserved rows not decided yet hold nothing.  Once every slot has been handed out, a new agent id takes the lowest removed slot
+// that is not held.  The table changes only under the handle lock, between calls, and a slot changes hands only when no live row
+// carries it, so within a call agent ids and slots stay one to one (K1's in-batch replay rule relies on it; DESIGN.md section 4).
+
+// the held-slot scan: removed slots up (one bit each), k_slot_refs over the window's physical ranges, held slots back
+static int scan_held_locked(agr_handle* h, std::vector<uint32_t>& held) {
+    const uint32_t nslots = (uint32_t)h->agent_names.size(), words = (nslots + 31) / 32;
+    std::vector<uint32_t> cand(words, 0u);
+    bool any = false;
+    for (uint32_t s = 0; s < nslots; ++s)
+        if (h->agent_status[s] == AG_STATUS_REMOVED) { cand[s >> 5] |= 1u << (s & 31); any = true; }
+    held.assign(words, 0u);
+    if (!any) return 0;
+    if (!h->d_slot_cand) {
+        const size_t cap = ((size_t)h->cfg.max_agents + 31) / 32;
+        TRY(dev_alloc(h, &h->d_slot_cand, cap, false));
+        TRY(dev_alloc(h, &h->d_slot_held, cap, false));
+    }
+    CK(cudaMemcpyAsync(h->d_slot_cand, cand.data(), (size_t)words * 4, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemsetAsync(h->d_slot_held, 0, (size_t)words * 4, h->stream));
+    const uint64_t live = h->rows_used - h->tail, p0 = phys_row(h, h->tail);
+    const uint64_t n0 = is_ring(h) ? std::min<uint64_t>(live, h->cfg.slab_rows - p0) : live;   // a ring's window wraps at most once
+    agr_launch_slot_refs(h->d.route, p0, n0, h->d_slot_cand, nslots, h->d_slot_held, h->sm_count, h->stream);
+    if (live > n0) agr_launch_slot_refs(h->d.route, 0, live - n0, h->d_slot_cand, nslots, h->d_slot_held, h->sm_count, h->stream);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(held.data(), h->d_slot_held, (size_t)words * 4, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    return 0;
+}
+
+// The slot for an agent id the table does not hold: the next never-used one, else the lowest removed slot that is not held, else
+// AGR_ENOSPC.  One scan lists every removed, unheld slot (lowest last).  Each entry stays removed and unheld (a removed agent gets
+// no new rows, and a revived one leaves the list), so the lowest entry is the answer unless a lower slot has been freed since the
+// scan: that takes an event that can free a slot (agent_gen: a drop, a release of rows, a restore) and a removed slot below that
+// entry.  Only then is the window scanned again, so a table full of live agents refuses without a scan and a run of
+// registrations after one release shares one scan.
+static int take_slot_locked(agr_handle* h, uint32_t* slot) {
+    if (h->agent_names.size() < h->cfg.max_agents) { *slot = (uint32_t)h->agent_names.size(); return 0; }
+    if (h->free_gen != h->agent_gen) {
+        const uint32_t head = h->free_slots.empty() ? (uint32_t)h->agent_names.size() : h->free_slots.back();
+        bool lower = false;
+        for (uint32_t s = 0; s < head && !lower; ++s) lower = h->agent_status[s] == AG_STATUS_REMOVED;
+        if (lower) {
+            std::vector<uint32_t> held;
+            TRY(scan_held_locked(h, held));
+            h->free_gen = h->agent_gen;
+            h->free_slots.clear();
+            for (uint32_t s = (uint32_t)h->agent_names.size(); s-- > 0;)
+                if (h->agent_status[s] == AG_STATUS_REMOVED && !((held[s >> 5] >> (s & 31)) & 1u)) h->free_slots.push_back(s);
+        }
+    }
+    if (!h->free_slots.empty()) {
+        *slot = h->free_slots.back();
+        h->free_slots.pop_back();
+        return 0;
+    }
+    // (every removed slot is held now: the list is empty, and a slot removed since the last scan would have caused one)
+    const size_t held = std::count(h->agent_status.begin(), h->agent_status.end(), (uint8_t)AG_STATUS_REMOVED);
+    return fail(AGR_ENOSPC, "agent table full (" + std::to_string(held) +
+                                " removed agents' slots are still held by live rows: agr_expire + agr_reclaim release them)");
+}
+
+// puts the key of slot (its name and status set) into the key table; upload: status first, then the key that makes the slot
+// reachable, both stream-ordered before the next kernel
+static int insert_key_locked(agr_handle* h, uint32_t slot, bool upload) {
+    agr_agent_key key{};
+    agt_pack(h->agent_names[slot].c_str(), key.w);
+    key.slot = slot;
+    key.status = h->agent_status[slot];
+    const uint32_t idx = agt_insert(h->akeys_host.data(), h->d.amask, key);
+    h->akey_index[slot] = idx;
+    if (upload) {
+        CK(cudaMemcpyAsync(h->d.astatus + slot, &h->agent_status[slot], 1, cudaMemcpyHostToDevice, h->stream));
+        CK(cudaMemcpyAsync(h->d.akeys + idx, &h->akeys_host[idx], sizeof key, cudaMemcpyHostToDevice, h->stream));
+    }
+    return 0;
+}
+
+// Forgets the agent of a handed-out slot: its name leaves the map and its key leaves the key table by backward shift (the entries
+// of the probe cluster that moved go up with it).  The slot stays handed out; agent_bind_locked gives it its next agent.
+int agent_forget_locked(agr_handle* h, uint32_t slot, bool upload) {
+    const uint32_t idx = h->akey_index[slot], mask = h->d.amask;
+    auto it = h->slot_of.find(h->agent_names[slot]);
+    if (it != h->slot_of.end() && it->second == slot) h->slot_of.erase(it);
+    const uint32_t count = agt_delete(h->akeys_host.data(), mask, idx);
+    for (uint32_t k = 0; k < count; ++k) {
+        const uint32_t j = (idx + k) & mask;
+        if (!agt_empty(h->akeys_host[j])) h->akey_index[h->akeys_host[j].slot] = j;
+    }
+    if (upload) {
+        const uint32_t n0 = std::min(count, mask + 1 - idx);
+        CK(cudaMemcpyAsync(h->d.akeys + idx, &h->akeys_host[idx], (size_t)n0 * sizeof(agr_agent_key), cudaMemcpyHostToDevice, h->stream));
+        if (count > n0) CK(cudaMemcpyAsync(h->d.akeys, &h->akeys_host[0], (size_t)(count - n0) * sizeof(agr_agent_key), cudaMemcpyHostToDevice, h->stream));
+    }
+    return 0;
+}
+// registers agent_id (not in the table) on a handed-out slot whose agent was forgotten
+int agent_bind_locked(agr_handle* h, uint32_t slot, const char* agent_id, uint8_t status, bool upload) {
+    h->agent_names[slot] = agent_id;
+    h->agent_status[slot] = status;
+    h->slot_of[std::string(agent_id)] = slot;
+    return insert_key_locked(h, slot, upload);
+}
+
 // core of agr_set_agent_state; `upload` = push the change to the device now (the bulk call uploads the tables once instead)
 int set_agent_state_locked(agr_handle* h, const char* agent_id, uint8_t status, bool upload) {
     size_t len = strnlen(agent_id, AGR_AGENT_ID_BYTES);
@@ -340,30 +440,28 @@ int set_agent_state_locked(agr_handle* h, const char* agent_id, uint8_t status, 
     if (status > AGR_AGENT_FAILED) return fail(AGR_EINVAL, "bad agent status");
     int slot = agent_find(h, agent_id);
     if (slot < 0) {
-        if (h->agent_names.size() >= h->cfg.max_agents) return fail(AGR_ENOSPC, "agent table full");
-        slot = (int)h->agent_names.size();
+        uint32_t s = 0;
+        TRY(take_slot_locked(h, &s));
+        if (s < h->agent_names.size()) {
+            TRY(agent_forget_locked(h, s, upload));
+            TRY(agent_bind_locked(h, s, agent_id, status, upload));
+            return (int)s;
+        }
         h->agent_names.emplace_back(agent_id);
         h->agent_status.push_back(status);
-        h->slot_of.emplace(std::string(agent_id), (uint32_t)slot);
-        agr_agent_key key{};
-        pack_agent_id(agent_id, key.w);
-        key.slot = (uint32_t)slot;
-        key.status = status;
-        uint32_t idx = (uint32_t)agr_hash_agent(key.w[0], key.w[1], key.w[2], key.w[3]) & h->d.amask;
-        while (h->akeys_host[idx].w[0] | h->akeys_host[idx].w[1] | h->akeys_host[idx].w[2] | h->akeys_host[idx].w[3])
-            idx = (idx + 1) & h->d.amask;
-        h->akeys_host[idx] = key;
-        h->akey_index.push_back(idx);
-        if (upload) {
-            // status first, then the key that makes the slot reachable; both are stream-ordered before the next kernel
-            CK(cudaMemcpyAsync(h->d.astatus + slot, &status, 1, cudaMemcpyHostToDevice, h->stream));
-            CK(cudaMemcpyAsync(h->d.akeys + idx, &key, sizeof key, cudaMemcpyHostToDevice, h->stream));
-        }
-    } else {
-        h->agent_status[slot] = status;
-        if (upload) TRY(push_agent_status(h, (uint32_t)slot, status));
-        else h->akeys_host[h->akey_index[slot]].status = status;
+        h->akey_index.push_back(0);
+        h->slot_of.emplace(std::string(agent_id), s);
+        TRY(insert_key_locked(h, s, upload));
+        return (int)s;
     }
+    if (h->agent_status[slot] == AG_STATUS_REMOVED) {
+        // revived on its slot: off the free list, which a later drop does not put it back on (its rows from now on may hold it)
+        auto it = std::find(h->free_slots.begin(), h->free_slots.end(), (uint32_t)slot);
+        if (it != h->free_slots.end()) h->free_slots.erase(it);
+    }
+    h->agent_status[slot] = status;
+    if (upload) TRY(push_agent_status(h, (uint32_t)slot, status));
+    else h->akeys_host[h->akey_index[slot]].status = status;
     return slot;
 }
 }  // namespace agr_impl
@@ -411,6 +509,7 @@ int agr_drop_agent(agr_handle* h, const char* agent_id) {
     if (slot < 0) return fail(AGR_ENOTFOUND, "agent not found");
     h->agent_status[slot] = AG_STATUS_REMOVED;
     TRY(push_agent_status(h, (uint32_t)slot, AG_STATUS_REMOVED));                          // DEL agent:{id} (agent.go:344)
+    h->agent_gen++;                                                                        // the slot may be free once its rows are gone
     unsigned long long lens[2];
     TRY(read_log_lens(h, lens));
     agr_launch_drop_agent(h->d, (uint32_t)slot, rows_span(h), std::max(lens[0], lens[1]), h->stream);
@@ -1394,6 +1493,7 @@ static int reclaim_apply(agr_handle* h, uint64_t* released) {
     }
     h->tail += count;
     h->released_total += count;
+    h->agent_gen++;                                            // released rows may have held removed agents' slots
     if (h->scan_lo < h->tail) h->scan_lo = h->tail;
     sync_window(h);
     if (!(h->cfg.flags & AGR_CFG_MINT_IDS)) {

@@ -18,6 +18,7 @@
 #include <unordered_map>
 #include <vector>
 #include "../../include/agentainer_gpu.h"
+#include "agr_agents.hpp"
 #include "agr_kernels.cuh"
 #include "agr_svc.h"
 
@@ -129,7 +130,13 @@ struct agr_handle {
     std::vector<std::string> agent_names;
     std::vector<uint8_t> agent_status;
     std::vector<agr_agent_key> akeys_host;
-    std::vector<uint32_t> akey_index;          // slot -> index of its entry in the open-addressing key table
+    std::vector<uint32_t> akey_index;          // slot -> index of its entry in the open-addressing key table (agr_agents.hpp)
+    // slot reuse once every slot has been handed out (set_agent_state_locked): the removed slots no live row carried at the last
+    // held-slot scan, highest first (taken from the back), and the generations of the events that can free a slot (agr_drop_agent,
+    // a release of rows, a restore) now and at that scan
+    std::vector<uint32_t> free_slots;
+    uint64_t agent_gen = 0, free_gen = ~0ull;
+    uint32_t *d_slot_cand = nullptr, *d_slot_held = nullptr;   // the scan's bitmaps, max_agents bits each (allocated on first use)
     // staging
     uint8_t* bounce[2] = {nullptr, nullptr};   // pinned, for pageable caller buffers
     cudaEvent_t bounce_ev[2] = {nullptr, nullptr};
@@ -298,6 +305,8 @@ int grow_events(std::vector<cudaEvent_t>& ev, size_t k);
 int chunk_bounds_unknown(agr_handle* h);
 int push_agent_status(agr_handle* h, uint32_t slot, uint8_t status);
 int set_agent_state_locked(agr_handle* h, const char* agent_id, uint8_t status, bool upload);
+int agent_forget_locked(agr_handle* h, uint32_t slot, bool upload);
+int agent_bind_locked(agr_handle* h, uint32_t slot, const char* agent_id, uint8_t status, bool upload);
 uint64_t ingested_bound(const agr_handle* h);
 void resv_remove(agr_handle* h, uint64_t first, uint64_t end);
 int reserve_rows_locked(agr_handle* h, uint32_t n, uint64_t* first);

@@ -952,6 +952,50 @@ void agr_launch_drop_agent(const agr_dev& d, uint32_t slot, unsigned long long r
     if (max_log_len) k_drop_logs<<<(unsigned)((max_log_len + 255) / 256), 256, 0, st>>>(d, slot);
 }
 
+// ------------------------------------------------------------------------------------------------ agent slot reuse
+// Which candidate slots (removed agents) a decided row of physical rows [p0, p0 + n) still carries.  A lane reads four route words
+// with one 16-byte load (from p0 rounded down to a multiple of 4; the rows outside the range are masked).  Only a decided row whose
+// slot is a candidate issues an atomic, and the lanes of a warp that hit the same slot issue one between them (match_any), so a run
+// of one agent's rows costs one atomicOr per warp step.  SMEM: the candidate bitmap is staged in shared memory (up to 2^18 slots),
+// else it is read through L2.
+template <bool SMEM>
+__global__ void __launch_bounds__(256) k_slot_refs(const uint32_t* __restrict__ route, const unsigned long long p0, const unsigned long long n,
+                                                   const uint32_t* __restrict__ cand, const uint32_t nslots, uint32_t* __restrict__ held) {
+    extern __shared__ uint32_t s_cand[];
+    if (SMEM) {
+        for (uint32_t i = threadIdx.x; i < (nslots + 31u) >> 5; i += blockDim.x) s_cand[i] = cand[i];
+        __syncthreads();
+    }
+    const uint32_t* cb = SMEM ? s_cand : cand;
+    const int lane = threadIdx.x & 31;
+    const unsigned long long e = p0 + n, stride = 4ull * gridDim.x * blockDim.x;
+    for (unsigned long long q = (p0 & ~3ull) + 4ull * (blockIdx.x * blockDim.x + threadIdx.x);; q += stride) {
+        const bool in = q < e;
+        if (!__any_sync(FULL, in)) break;                                  // (the lanes of a warp cover 128 consecutive rows)
+        const uint4 v = in ? __ldcs(reinterpret_cast<const uint4*>(route + q)) : make_uint4(0u, 0u, 0u, 0u);
+        const uint32_t w4[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const uint32_t s = rt_slot(w4[i]);
+            const bool hit = q + i >= p0 && q + i < e && rt_code(w4[i]) != 0u && s < nslots && ((cb[s >> 5] >> (s & 31u)) & 1u);
+            if (!__any_sync(FULL, hit)) continue;
+            const uint32_t peers = __match_any_sync(FULL, hit ? s : 0xffffffffu);
+            if (hit && lane == __ffs(peers) - 1) atomicOr(held + (s >> 5), 1u << (s & 31u));
+        }
+    }
+}
+#define SLOT_REFS_SMEM_WORDS 8192u   // 32 KiB: 2^18 slots
+void agr_launch_slot_refs(const uint32_t* route, unsigned long long p0, unsigned long long n, const uint32_t* cand, uint32_t nslots,
+                          uint32_t* held, int sm_count, cudaStream_t st) {
+    if (!n || !nslots) return;
+    const unsigned long long lanes = ((p0 & 3ull) + n + 3ull) / 4ull;
+    const unsigned long long want = (lanes + 255ull) / 256ull, cap = (unsigned long long)sm_count * 8ull;
+    const unsigned blocks = (unsigned)(want < cap ? want : cap);
+    const uint32_t words = (nslots + 31u) >> 5;
+    if (words <= SLOT_REFS_SMEM_WORDS) k_slot_refs<true><<<blocks, 256, words * 4u, st>>>(route, p0, n, cand, nslots, held);
+    else k_slot_refs<false><<<blocks, 256, 0, st>>>(route, p0, n, cand, nslots, held);
+}
+
 // ------------------------------------------------------------------------------------------------ online snapshot cut
 // blockIdx.y = section; the blocks of a section stride over it in 16 B pieces, four independent loads in flight per thread,
 // and block 0 copies the tail (< 16 B).  The log lengths are read here, on the device, so the host never waits to learn them.

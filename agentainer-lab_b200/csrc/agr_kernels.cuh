@@ -212,6 +212,11 @@ void agr_launch_k3_gather(const agr_dev& d, const uint32_t* rids, const uint32_t
                           uint8_t* out_ids /*nullable, 16 B each*/, cudaStream_t st);
 void agr_launch_drop_agent(const agr_dev& d, uint32_t slot, unsigned long long rows, unsigned long long max_log_len,
                            cudaStream_t st);
+// The held-slot scan: sets bit s of held (cleared by the caller) for every candidate slot s (bit s of cand, nslots bits) that
+// the route word of a decided row among physical rows [p0, p0 + n) carries.  route is the engine's route array (4 words of
+// padding past its end).
+void agr_launch_slot_refs(const uint32_t* route, unsigned long long p0, unsigned long long n, const uint32_t* cand, uint32_t nslots,
+                          uint32_t* held, int sm_count, cudaStream_t st);
 void agr_launch_synth(uint8_t* dst, agr_synth_dev s, unsigned long long first_index, uint32_t n, cudaStream_t st);
 
 // Online snapshot (AGR_CFG_ONLINE_SNAPSHOT): the cut copies the sections that later calls rewrite in place (per-row words, the

@@ -447,14 +447,34 @@ int agr_snapshot(agr_handle* h, const char* path) {
 
 // ---- restore: a full file, then the deltas of its chain, oldest first
 // The agent table of a file: entry a is slot a.  An agent the engine already has (registered before the parent's cut) keeps its
-// name and slot, and only its status changes; a new one is registered in table order, so that the slots match.
+// name and slot, and only its status changes; a new one is registered in table order, so that the slots match.  A delta may name
+// another agent than its parent on a slot: the slot was reused between the two cuts (its agent removed before the parent's cut or
+// after it, and its rows released), so the old names are forgotten first and the new ones bound to their slots.  The delta was
+// written on this parent (restore_locked compares the digests first), so a name that differs can mean nothing else; a name that
+// would then stand on two slots is refused.
 static int restore_agents_locked(agr_handle* h, FILE* f, uint32_t n) {
+    if (n > h->cfg.max_agents) return fail(AGR_ENOSPC, "agent table full");
+    std::vector<std::string> names(n);
+    std::vector<uint8_t> sts(n);
     for (uint32_t a = 0; a < n; ++a) {
-        char name[AGR_AGENT_ID_BYTES]; uint8_t st;
-        if (fread(name, 1, AGR_AGENT_ID_BYTES, f) != AGR_AGENT_ID_BYTES || fread(&st, 1, 1, f) != 1) return fail(AGR_EINVAL, "restore: short read");
+        char name[AGR_AGENT_ID_BYTES];
+        if (fread(name, 1, AGR_AGENT_ID_BYTES, f) != AGR_AGENT_ID_BYTES || fread(&sts[a], 1, 1, f) != 1) return fail(AGR_EINVAL, "restore: short read");
         name[AGR_AGENT_ID_BYTES - 1] = 0;
+        names[a] = name;
+    }
+    if (n < h->agent_names.size()) return fail(AGR_EINVAL, "restore: the agent table of a delta does not extend its parent's");
+    std::vector<uint32_t> reused;
+    for (uint32_t a = 0; a < h->agent_names.size(); ++a)
+        if (h->agent_names[a] != names[a]) reused.push_back(a);
+    for (uint32_t a : reused) TRY(agent_forget_locked(h, a, true));
+    for (uint32_t a : reused) {
+        if (h->slot_of.count(names[a])) return fail(AGR_EINVAL, "restore: an agent appears twice in the agent table");
+        TRY(agent_bind_locked(h, a, names[a].c_str(), AG_STATUS_REMOVED, true));
+    }
+    for (uint32_t a = 0; a < n; ++a) {
+        const char* name = names[a].c_str();
+        const uint8_t st = sts[a];
         const bool removed = (st == AG_STATUS_REMOVED), known = a < h->agent_names.size();
-        if (known && h->agent_names[a] != name) return fail(AGR_EINVAL, "restore: the agent table of a delta does not extend its parent's");
         if (!known || !removed) {
             const int s = set_agent_state_locked(h, name, removed ? (uint8_t)AGR_AGENT_STOPPED : st, true);
             if (s < 0) return s;
@@ -561,6 +581,7 @@ static int restore_locked(agr_handle* h, FILE* f, const snap_header& full, const
     h->rows_used = hd.rows_used; h->vused = hd.vused; h->vtail = hd.vtail; h->scan_lo = hd.scan_lo;
     h->d.shard_id = hd.shard; h->d.id_gen = hd.gen; h->tail = hd.tail; h->released_total = hd.released_total; sync_window(h);
     h->d.idx_base = h->tail;
+    h->agent_gen++;                                   // another window: which removed agents' slots it holds is scanned afresh
     TRY(chunk_bounds_unknown(h));
     if (index && !(hd.flags & AGR_CFG_MINT_IDS) && R) {   // hash-id mode: rebuild the dedupe index from the restored rows
         agr_launch_reindex(h->d, (uint32_t)R, h->stream);

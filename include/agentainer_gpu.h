@@ -154,16 +154,21 @@ const char* agr_strerror(int code);
 /* Agent status mirror.  Replaces the per-request GET agent:{id} + Unmarshal of agent.Manager.GetAgent
  * (agent.go:372-390) read at server.go:498 and replay_worker.go:166-189.  Called from wherever the host
  * writes Agent.Status (saveAgent agent.go:510-530, state sync).  Registers the agent on first use; slots are
- * handed out in registration order.  Returns the slot (>= 0) or a negative error. */
+ * handed out in registration order.  Once all max_agents slots have been handed out, a new agent takes the lowest slot
+ * whose agent was removed (agr_drop_agent) and that no row of the live window still records a decision for; with none,
+ * AGR_ENOSPC (agr_last_error counts the removed slots live rows still hold).  A removed agent's name is forgotten when its
+ * slot is reused.  Returns the slot (>= 0) or a negative error. */
 enum { AGR_AGENT_CREATED = 0, AGR_AGENT_RUNNING = 1, AGR_AGENT_STOPPED = 2, AGR_AGENT_PAUSED = 3, AGR_AGENT_FAILED = 4 };  /* agent.go:23-29 */
 int agr_set_agent_state(agr_handle* h, const char* agent_id, uint8_t status);
 /* The same for a batch of status writes (the periodic state sync, sync/state_sync.go:190-210, and quick sync,
  * pkg/agentsync/quick_sync.go:89-102, walk every agent): ids are fixed-stride NUL-padded strings; slots (nullable)
  * receives the slot or the negative error of each entry; the return value is 0 or the first error.  More than 16
- * entries are applied to the host mirror and uploaded as two table copies instead of one small copy per agent. */
+ * entries are applied to the host mirror and uploaded as two table copies instead of one small copy per agent.  New
+ * agents take slots by the rule of agr_set_agent_state, as if the entries were set one by one. */
 int agr_set_agent_states(agr_handle* h, const char (*agent_ids)[AGR_AGENT_ID_BYTES], const uint8_t* statuses, uint32_t n, int32_t* slots);
 /* replaces the queue cleanup of agent.Manager.Remove (agent.go:343-359): DEL agent:{id} and the three lists.
- * Records are left orphaned exactly like the reference (Q17). */
+ * Records are left orphaned exactly like the reference (Q17).  The slot stays with the removed agent (agr_set_agent_state
+ * revives it there) until a new agent reuses it, which needs every row that records a decision for it released. */
 int agr_drop_agent(agr_handle* h, const char* agent_id);
 int agr_agent_slot(agr_handle* h, const char* agent_id);   /* slot or AGR_ENOTFOUND */
 
