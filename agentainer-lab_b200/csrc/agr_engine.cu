@@ -111,6 +111,21 @@ int chunk_bounds_unknown(agr_handle* h) {
 
 static uint64_t next_pow2(uint64_t v) { uint64_t p = 1; while (p < v) p <<= 1; return p; }
 
+// Hash-id ring: the dedupe index rebuilt from the window's rows that still hold a record (ST_STORED in the state word), over
+// the window's one or two physical runs.  Open addressing has no cheap delete, so a release rebuilds the index instead of
+// taking the released rows' ids out; a restore of a ring rebuilds it the same way, so that the restored index is the one a
+// release leaves (an expired row's id is in neither).
+int ring_reindex_locked(agr_handle* h) {
+    CK(cudaMemsetAsync(h->d.table, 0, (size_t)(h->d.table_mask + 1) * sizeof(agr_slot), h->stream));
+    h->d.idx_base = h->tail;                                              // row words of the rebuilt index are relative to the tail
+    const uint64_t R = h->cfg.slab_rows, live = h->rows_used - h->tail, p0 = h->tail % R;
+    const uint64_t n0 = std::min<uint64_t>(live, R - p0);
+    agr_launch_reindex_range(h->d, (uint32_t)p0, (uint32_t)n0, h->stream);
+    if (live > n0) agr_launch_reindex_range(h->d, 0, (uint32_t)(live - n0), h->stream);
+    CK(cudaGetLastError());
+    h->k1_launches += 2;
+    return 0;
+}
 }  // namespace agr_impl
 
 extern "C" {
@@ -1496,18 +1511,8 @@ static int reclaim_apply(agr_handle* h, uint64_t* released) {
     h->agent_gen++;                                            // released rows may have held removed agents' slots
     if (h->scan_lo < h->tail) h->scan_lo = h->tail;
     sync_window(h);
-    if (!(h->cfg.flags & AGR_CFG_MINT_IDS)) {
-        // hash-id mode: the released rows' ids must leave the dedupe index before their rows are reused.  Open addressing
-        // has no cheap delete; a release is a periodic event, so the index is rebuilt from the live window instead.
-        CK(cudaMemsetAsync(h->d.table, 0, (size_t)(h->d.table_mask + 1) * sizeof(agr_slot), h->stream));
-        h->d.idx_base = h->tail;                                              // row words of the rebuilt index are relative to the new tail
-        const uint64_t R = h->cfg.slab_rows, live = h->rows_used - h->tail, p0 = h->tail % R;
-        const uint64_t n0 = std::min<uint64_t>(live, R - p0);
-        agr_launch_reindex_range(h->d, (uint32_t)p0, (uint32_t)n0, h->stream);
-        if (live > n0) agr_launch_reindex_range(h->d, 0, (uint32_t)(live - n0), h->stream);
-        CK(cudaGetLastError());
-        h->k1_launches += 2;
-    }
+    // hash-id mode: the released rows' ids must leave the dedupe index before their rows are reused
+    if (!(h->cfg.flags & AGR_CFG_MINT_IDS)) TRY(ring_reindex_locked(h));
     if (h->resp_used != h->resp_tail) {   // the response / error byte ring: its tail follows the oldest blob a live row still refers to
         CK(cudaMemsetAsync(count_slot(h), 0, 8, h->stream));
         agr_launch_bytes_span(h->d, h->resp_used % h->resp_cap, h->resp_cap, h->d_resp_off, h->d_resp_len, h->d_err_off, h->d_err_len, count_slot(h), h->stream);

@@ -303,6 +303,7 @@ int upload_rows(agr_handle* h, uint8_t* dst, const uint8_t* src, size_t bytes, b
 int read_log_lens(agr_handle* h, unsigned long long lens[2]);
 int grow_events(std::vector<cudaEvent_t>& ev, size_t k);
 int chunk_bounds_unknown(agr_handle* h);
+int ring_reindex_locked(agr_handle* h);
 int push_agent_status(agr_handle* h, uint32_t slot, uint8_t status);
 int set_agent_state_locked(agr_handle* h, const char* agent_id, uint8_t status, bool upload);
 int agent_forget_locked(agr_handle* h, uint32_t slot, bool upload);

@@ -63,7 +63,7 @@ __global__ void __launch_bounds__(256) k1_post(const agr_dev d, const uint32_t f
 }
 
 // The dedupe-index insert of every stored row, one thread per row at full occupancy (agr_launch_reindex: rebuilds the index
-// after a restore).  A row whose id is already present becomes a provisional duplicate (k1_post decides).
+// after the restore of an append-only engine, whose index holds every row K1 ever stored).  A row whose id is already present becomes a provisional duplicate (k1_post decides).
 __global__ void __launch_bounds__(256) k1_index(const agr_dev d, const uint32_t first_rid, const uint32_t n) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     const int lane = threadIdx.x & 31;
@@ -362,7 +362,8 @@ void agr_launch_log_compact(const agr_dev& d, const uint32_t* log, unsigned long
 void agr_launch_verify(const agr_dev& d, unsigned long long rows, unsigned long long* bad, cudaStream_t st) {
     if (rows) k_verify<<<(unsigned)((rows * 32 + 255) / 256), 256, 0, st>>>(d, rows, bad);
 }
-// hash-id ring: rebuild of the dedupe index over a range of physical rows — only rows that still hold a record go in
+// hash-id ring: rebuild of the dedupe index over a range of physical rows — only rows that still hold a record go in (a release,
+// a restore: ring_reindex_locked)
 __global__ void __launch_bounds__(256) k_reindex_range(const agr_dev d, const uint32_t first, const uint32_t n) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -381,7 +382,7 @@ __global__ void __launch_bounds__(256) k_reindex_range(const agr_dev d, const ui
 void agr_launch_reindex_range(const agr_dev& d, uint32_t first, uint32_t n, cudaStream_t st) {
     if (n) k_reindex_range<<<(n + 255u) / 256u, 256, 0, st>>>(d, first, n);
 }
-// rebuild of the dedupe index from restored rows (hash-id mode): k1_index over every stored row
+// rebuild of the dedupe index from restored rows (hash-id mode, append-only): k1_index over every row K1 stored
 void agr_launch_reindex(const agr_dev& d, uint32_t rows, cudaStream_t st) {
     if (rows) k1_index<<<(rows + 255u) / 256u, 256, 0, st>>>(d, 0u, rows);
 }

@@ -584,8 +584,11 @@ static int restore_locked(agr_handle* h, FILE* f, const snap_header& full, const
     h->agent_gen++;                                   // another window: which removed agents' slots it holds is scanned afresh
     TRY(chunk_bounds_unknown(h));
     if (index && !(hd.flags & AGR_CFG_MINT_IDS) && R) {   // hash-id mode: rebuild the dedupe index from the restored rows
-        agr_launch_reindex(h->d, (uint32_t)R, h->stream);
-        h->k1_launches += 1;
+        if (is_ring(h)) TRY(ring_reindex_locked(h));     // a ring: the index a release leaves (rows that hold a record)
+        else {                                            // append-only: the index never shrinks, so every row K1 stored is in it
+            agr_launch_reindex(h->d, (uint32_t)R, h->stream);
+            h->k1_launches += 1;
+        }
         if (cudaStreamSynchronize(h->stream) != cudaSuccess) return fail(AGR_ECUDA, "restore: reindex");
     }
     if (chain || !dh.empty()) {
@@ -677,11 +680,7 @@ static int relocate_locked(agr_handle* h, agr_handle* s, const snap_header& hd) 
     h->resp_used = tot[1]; h->resp_tail = 0;
     h->d.idx_base = h->tail;
     TRY(chunk_bounds_unknown(h));
-    const uint64_t R = rows_span(h);
-    if (!(hd.flags & AGR_CFG_MINT_IDS) && R) {                 // hash-id mode: the dedupe index of the moved rows
-        agr_launch_reindex(h->d, (uint32_t)R, h->stream);
-        h->k1_launches += 1;
-    }
+    if (!(hd.flags & AGR_CFG_MINT_IDS) && n) TRY(ring_reindex_locked(h));   // hash-id mode: the index a release leaves
     if (cudaStreamSynchronize(h->stream) != cudaSuccess) return fail(AGR_ECUDA, "restore: relocation");
     return 0;
 }

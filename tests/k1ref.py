@@ -138,6 +138,7 @@ class Ref:
         self.route = np.zeros(cap, dtype=np.uint32)
         self.slot = np.full(cap, RT_SLOT_NONE, dtype=np.int64)
         self.created = np.zeros(cap, dtype=np.uint64)
+        self.mtime = np.zeros(cap, dtype=np.uint64)             # last SET after the ingest (a completion); 0: none
         self.idb = np.zeros((cap, 16), dtype=np.uint8)           # caller ids (hash mode)
         self.head = 0                                            # rows handed out (arrival numbers < head)
         self.tail = 0                                            # rows released (ring)
@@ -151,7 +152,7 @@ class Ref:
         if need <= cap:
             return
         new = max(need, 2 * cap)
-        for name in ("state", "route", "slot", "created", "idb"):
+        for name in ("state", "route", "slot", "created", "mtime", "idb"):
             a = getattr(self, name)
             b = np.zeros((new,) + a.shape[1:], dtype=a.dtype) if name != "slot" else np.full(new, RT_SLOT_NONE, dtype=np.int64)
             b[:cap] = a
@@ -266,10 +267,14 @@ class Ref:
         return lo + np.nonzero(self.state[lo:self.head] & ST_STORED)[0]
 
     # ---- the ring's TTL sweep and release
+    def touch(self, rows, now):
+        """a completion (StoreResponse, MarkRequestFailed) of these rows at time now: their last SET moves to now"""
+        self.mtime[np.asarray(rows, dtype=np.int64)] = now
+
     def expire(self, now, ttl):
-        """stored rows whose created_at is ttl or more before now lose ST_STORED (K2 never ran: mtime = created_at)"""
+        """stored rows whose last SET (the completion's time, else created_at) is ttl or more before now lose ST_STORED"""
         r = self.stored_rows()
-        t = np.maximum(self.created[r], 1)
+        t = np.maximum(np.where(self.mtime[r] != 0, self.mtime[r], self.created[r]), 1)
         gone = r[(now >= t) & (now - t >= ttl)]
         self.state[gone] &= ~np.uint32(ST_STORED)
         return len(gone)
@@ -281,9 +286,20 @@ class Ref:
         new = int(r[0]) if len(r) else self.head
         released, self.tail = new - self.tail, new
         if released and not self.mint:
-            self.owner, self.index = {}, set()
-            for x in r.tolist():
-                k = self.idb[x].tobytes()
-                self.owner.setdefault(k, x)
-                self.index.add(k)
+            self._reindex(r)
         return released
+
+    def restore(self, ring):
+        """the dedupe index after a snapshot of this state is restored (caller ids): a ring's is rebuilt as a release rebuilds
+        it, from the window's rows that hold a record, so the ids of rows that expired since the last release leave it; an
+        append-only engine's index never shrinks, and it comes back as it was.  Returns index_used()."""
+        if ring and not self.mint:
+            self._reindex(self.stored_rows())
+        return self.index_used()
+
+    def _reindex(self, rows):
+        self.owner, self.index = {}, set()
+        for x in rows.tolist():
+            k = self.idb[x].tobytes()
+            self.owner.setdefault(k, x)
+            self.index.add(k)

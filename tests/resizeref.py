@@ -26,9 +26,79 @@ def src_logical(hd, p):
     return tail + (p - tail % S) % S
 
 
+def _header(hd, flags, slab_rows, vcap, resp_cap, var, rec_total, rsp_total):
+    out = np.zeros(1, dtype=hd.dtype)[0]
+    for name in hd.dtype.names:
+        out[name] = hd[name]
+    out["flags"] = flags & (K.AGR_CFG_PERSISTENCE | K.AGR_CFG_MINT_IDS | V | R)
+    out["slab_rows"], out["vcap"], out["resp_cap"] = slab_rows, vcap if var else 0, resp_cap
+    out["vused"], out["vtail"] = rec_total, 0
+    out["resp_used"], out["resp_tail"] = rsp_total, 0
+    return out
+
+
+def _gather(dst, src, dst_at, src_at, n):
+    """dst[dst_at[k]: + n[k]] = src[src_at[k]: + n[k]] for every k, in one indexed copy"""
+    n = np.asarray(n, dtype=np.int64)
+    total = int(n.sum())
+    if total == 0:
+        return
+    start = np.cumsum(n) - n
+    step = np.arange(total, dtype=np.int64) - np.repeat(start, n)
+    dst[np.repeat(np.asarray(dst_at, dtype=np.int64), n) + step] = src[np.repeat(np.asarray(src_at, dtype=np.int64), n) + step]
+
+
 def relocate(hd, agents, sec, flags, slab_rows, vcap, resp_cap):
     """(header, agent table, sections) of the full file an engine of these flags and capacities writes right after restoring
-    the file (hd, agents, sec) with relocation.  Raises NoSpace for what agr_restore refuses with AGR_ENOSPC."""
+    the file (hd, agents, sec) with relocation.  Raises NoSpace for what agr_restore refuses with AGR_ENOSPC.  The same rules
+    as relocate_loop, one array operation per step, so that windows of 2^19 rows and more take seconds."""
+    var = bool(int(hd["flags"]) & V)
+    tail, used = int(hd["tail"]), int(hd["rows_used"])
+    if used - tail > slab_rows:
+        raise NoSpace("window")
+    L = np.arange(tail, used, dtype=np.int64)
+    ps = L % int(hd["slab_rows"]) if int(hd["flags"]) & R else L
+    pt = L % slab_rows
+    live = sec["state"][ps] != 0
+    vlen = np.where(live, sec["vlen"][ps].astype(np.int64), 0) if var else None
+    # per window row: its response segment then its error segment, each from a 16 B boundary; dead rows take no bytes
+    seg = np.stack([np.where(live, sec[ln][ps].astype(np.int64), 0) for ln in ("resp_len", "err_len")], axis=1).reshape(-1)
+    seg16 = (seg + 15) & ~15
+    rec_total = int(vlen.sum()) if var else 0
+    rsp_total = int(seg16.sum())
+    if var and rec_total > vcap:
+        raise NoSpace("vslab_bytes")
+    if rsp_total > resp_cap:
+        raise NoSpace("resp_bytes")
+
+    out = _header(hd, flags, slab_rows, vcap, resp_cap, var, rec_total, rsp_total)
+    new = {name: np.zeros(count, dtype=dt) for name, dt, count in sections(out)}
+    for w in WORDS:
+        if len(new[w]):
+            new[w][pt] = sec[w][ps]
+    if var:
+        rec_at = np.cumsum(vlen) - vlen
+        new["voff"][pt] = np.where(live, rec_at, 0)
+        _gather(new["slab"], sec["slab"], rec_at, sec["voff"][ps], vlen)
+    else:
+        new["slab"].reshape(-1, 512)[pt] = sec["slab"].reshape(-1, 512)[ps]
+    rsp_at = np.cumsum(seg16) - seg16
+    src_at = np.stack([sec["resp_off"][ps], sec["err_off"][ps]], axis=1).reshape(-1).astype(np.int64)
+    at = np.where(seg > 0, rsp_at, 0).reshape(-1, 2)
+    new["resp_off"][pt], new["err_off"][pt] = at[:, 0], at[:, 1]
+    _gather(new["resp"], sec["resp"], rsp_at, src_at, seg)
+    for name in ("completed_log", "failed_log"):
+        e = sec[name].astype(np.int64)
+        none = e == 0xFFFFFFFF
+        if int(hd["flags"]) & R:
+            S = int(hd["slab_rows"])
+            e = tail + (e - tail % S) % S
+        new[name][:] = np.where(none, 0xFFFFFFFF, e % slab_rows)
+    return out, agents, new
+
+
+def relocate_loop(hd, agents, sec, flags, slab_rows, vcap, resp_cap):
+    """relocate, one row at a time: the form the rules are easiest to read in (and the one relocate is checked against)."""
     var = bool(int(hd["flags"]) & V)
     tail, used = int(hd["tail"]), int(hd["rows_used"])
     if used - tail > slab_rows:
@@ -42,14 +112,7 @@ def relocate(hd, agents, sec, flags, slab_rows, vcap, resp_cap):
     if rsp_total > resp_cap:
         raise NoSpace("resp_bytes")
 
-    out = np.zeros(1, dtype=hd.dtype)[0]
-    for name in hd.dtype.names:
-        out[name] = hd[name]
-    out["flags"] = flags & (K.AGR_CFG_PERSISTENCE | K.AGR_CFG_MINT_IDS | V | R)
-    out["slab_rows"], out["vcap"], out["resp_cap"] = slab_rows, vcap if var else 0, resp_cap
-    out["vused"], out["vtail"] = rec_total, 0
-    out["resp_used"], out["resp_tail"] = rsp_total, 0
-
+    out = _header(hd, flags, slab_rows, vcap, resp_cap, var, rec_total, rsp_total)
     new = {name: np.zeros(count, dtype=dt) for name, dt, count in sections(out)}
     slab = new["slab"]
     rec_at = rsp_at = 0

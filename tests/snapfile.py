@@ -3,6 +3,7 @@ what a delta should hold given the full files of its parent's cut and of its own
 import numpy as np
 
 from agentainer_lab_b200 import constants as K
+from k1ref import fmix64
 
 R, V = K.AGR_CFG_RING, K.AGR_CFG_VARLEN
 BLOCK_ROWS, LOG_BLOCK = 256, 1024
@@ -30,6 +31,42 @@ def sections(hd):
             ("completed_log", "<u4", int(hd["log_len"][0])), ("failed_log", "<u4", int(hd["log_len"][1])),
             ("resp", np.uint8, resp), ("resp_off", "<u8", rows), ("resp_len", "<u4", rows), ("resp_hlen", "<u4", rows),
             ("err_off", "<u8", rows), ("err_len", "<u4", rows), ("ptime", "<u8", rows), ("mtime", "<u8", rows)]
+
+
+LOGS = ("completed_log", "failed_log")
+PHI, DIGEST_C = 0x9E3779B97F4A7C15, 0x632BE59BD9B4E019
+U64 = (1 << 64) - 1
+
+
+def digest_sections(hd, sec):
+    """(section id, bytes) of what the compare cut sums: every per-row word section that holds bytes, then the two logs; the
+    id is the section's place in the file's section table (so the logs are 7 and 8)."""
+    names = [name for name, _, _ in sections(hd)]
+    out = [(k, sec[name].tobytes()) for k, name in enumerate(names) if name in WORDS and len(sec[name])]
+    return out + [(names.index(name), sec[name].tobytes()) for name in LOGS]
+
+
+def digest(hd, sec, key):
+    """The 128-bit keyed digest of k_snap_cmp over the sections of a full file (parse): per section s, with the key
+    fmix64(key ^ ((s + 1) << 56)), every 16 B piece i (a short last piece zero-padded) as two little-endian u64 a, b adds
+    fmix64(fmix64(t ^ a) ^ b) to the first sum and fmix64(fmix64((t + C) ^ b) ^ a) to the second, t = fmix64(skey + i * phi);
+    both sums mod 2^64.  The sum does not depend on the order the device adds pieces in."""
+    h = [0, 0]
+    u = np.uint64
+    for s, b in digest_sections(hd, sec):
+        n = (len(b) + 15) // 16
+        if n == 0:
+            continue
+        w = np.frombuffer(b + bytes(16 * n - len(b)), dtype="<u8").reshape(n, 2)
+        a, bb = w[:, 0], w[:, 1]
+        skey = fmix64(u((int(key) ^ ((s + 1) << 56)) & U64))
+        with np.errstate(over="ignore"):
+            t = fmix64(skey + np.arange(n, dtype=u) * u(PHI))
+            h0 = fmix64(fmix64(t ^ a) ^ bb)
+            h1 = fmix64(fmix64((t + u(DIGEST_C)) ^ bb) ^ a)
+        h[0] = (h[0] + int(h0.sum(dtype=u))) & U64
+        h[1] = (h[1] + int(h1.sum(dtype=u))) & U64
+    return tuple(h)
 
 
 def parse(data: bytes):
@@ -142,22 +179,29 @@ def expected_blocks(sec_a, hd_a, sec_b, hd_b):
     return sorted(b for b in dirty if b * BLOCK_ROWS < Rb), logs
 
 
+def _mark(mask, at, n):
+    """mask[at[k]: at[k] + n[k]] = True for every k"""
+    n = np.asarray(n, dtype=np.int64)
+    if n.sum():
+        start = np.cumsum(n) - n
+        mask[np.repeat(np.asarray(at, dtype=np.int64), n) + np.arange(int(n.sum())) - np.repeat(start, n)] = True
+
+
 def referenced(sec, hd, var):
     """Byte masks of the slab and the response bytes that some row of the cut's window refers to (everything else there
-    is unspecified: outside the window, skipped at a lap's end, or never written by either engine, such as 16 B padding)."""
+    is unspecified: outside the window, skipped at a lap's end, or never written by either engine, such as 16 B padding),
+    and the physical rows of the window that hold a row (state != 0)."""
     ring = bool(hd["flags"] & R)
     S, used, tail = int(hd["slab_rows"]), int(hd["rows_used"]), int(hd["tail"])
-    live = [(L % S) if ring else L for L in range(tail, used)]
-    live = [p for p in live if sec["state"][p] != 0]
+    L = np.arange(tail, used, dtype=np.int64)
+    live = L % S if ring else L
+    live = live[sec["state"][live] != 0]
     slab = np.zeros(len(sec["slab"]), dtype=bool)
     resp = np.zeros(len(sec["resp"]), dtype=bool)
-    for p in live:
-        if var:
-            o = int(sec["voff"][p]); slab[o: o + int(sec["vlen"][p])] = True
-        else:
-            slab[p * 512: (p + 1) * 512] = True
-        for off, ln in (("resp_off", "resp_len"), ("err_off", "err_len")):
-            n = int(sec[ln][p])
-            if n:
-                o = int(sec[off][p]); resp[o: o + n] = True
-    return slab, resp, live
+    if var:
+        _mark(slab, sec["voff"][live], sec["vlen"][live])
+    else:
+        slab.reshape(-1, 512)[live] = True
+    for off, ln in (("resp_off", "resp_len"), ("err_off", "err_len")):
+        _mark(resp, sec[off][live], sec[ln][live])
+    return slab, resp, live.tolist()

@@ -1,5 +1,7 @@
 """The plain dedupe-hit reference (tests/k1ref.py) on hand-worked batches that cover the in-batch and earlier-batch cases, with
 ids from the id reference (tests/mintref.py).  The GPU test of K1's replay decision runs the same batches.  CPU only."""
+import copy
+
 import numpy as np
 import pytest
 
@@ -155,6 +157,52 @@ def test_hand_rows_expire_reclaim():
     assert ref.expire(60, 40) == 0 and ref.reclaim() == 0 and ref.index_used() == 2
     assert ref.expire(100, 40) == 1 and ref.reclaim() == 1 and ref.index_used() == 1
     assert ref.expire(200, 40) == 1 and ref.reclaim() == 2 and ref.index_used() == 0 and ref.tail == 4
+
+
+def test_hand_rows_restore_index():
+    """the index a restore leaves: Z (expires), P (completed later, so it does not), A carrying X (expires behind P); the
+    release stops at P and leaves A out of the index; C carries X again and is stored.  A ring's restore rebuilds the index
+    from the rows that hold a record (C owns X; the ids of A and Y, expired but not released, are gone); an append-only
+    engine's comes back as it was"""
+    X, Y, W = rid_of(1), rid_of(2), rid_of(3)
+    recs = np.zeros(5, dtype=record_dtype)
+    _rec(recs, 0, "agent-run", rid_of(9), seq=10)         # Z
+    _rec(recs, 1, "agent-run", W, seq=10)                  # P
+    _rec(recs, 2, "agent-run", X, seq=10)                  # A
+    _rec(recs, 3, "agent-stop", Y, seq=10)                 # expires behind P, its id never comes back
+    _rec(recs, 4, "agent-run", rid_of(8), seq=95)          # stays stored
+    ref = _ref()
+    ref.ingest(recs)
+    ref.touch([1], 90)                                     # P's StoreResponse
+    assert ref.expire(100, 50) == 3 and ref.stored_rows().tolist() == [1, 4]
+    assert ref.reclaim() == 1 and ref.tail == 1 and ref.index_used() == 2     # the index of P onward: W and rid_of(8)
+    c = np.zeros(3, dtype=record_dtype)
+    _rec(c, 0, "agent-run", X, seq=100)                    # C: X is free again
+    _rec(c, 1, "agent-run", replay_of=X, seq=100)          # names C: a hit
+    _rec(c, 2, "agent-other", X, seq=100)                  # X again: DUP_ID
+    S, T, KN, D, RP = K.AGR_VF_STORED, K.AGR_VF_TRACKED, K.AGR_VF_KNOWN, K.AGR_VF_DUP_ID, K.AGR_VF_REPLAY
+    assert ref.ingest(c)["verdict"]["flags"].tolist() == [S | T, RP | T | KN, D]
+    assert ref.owner[X] == 5 and ref.index_used() == 3
+    flat = copy.deepcopy(ref)
+    assert ref.restore(ring=True) == 3 and ref.owner == {W: 1, rid_of(8): 4, X: 5}
+    assert flat.restore(ring=False) == 3 and flat.owner == ref.owner
+    # after a ring restore: Y is free, X still names C; a later release leaves the same index as the restore did
+    r2 = np.zeros(3, dtype=record_dtype)
+    _rec(r2, 0, "agent-stop", Y, seq=100)
+    _rec(r2, 1, "agent-run", X, seq=100)
+    _rec(r2, 2, "agent-run", replay_of=X, seq=100)
+    assert ref.ingest(r2)["verdict"]["flags"].tolist() == [S | T, D, RP | T | KN]
+    assert ref.owner[Y] == 8 and ref.owner[X] == 5
+    # an id of a row that expired after the last release: in the index of an engine that never restarted, not after a
+    # ring restore
+    live = _ref()
+    live.ingest(recs[:3])
+    live.expire(100, 50)
+    assert live.index_used() == 3 and live.restore(ring=True) == 0
+    again = _ref()
+    again.ingest(recs[:3])
+    again.expire(100, 50)
+    assert again.restore(ring=False) == 3                   # append-only: X, W and rid_of(9) stay
 
 
 def test_hand_rows_minted_ids():

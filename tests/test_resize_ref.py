@@ -3,7 +3,7 @@ import numpy as np
 import pytest
 
 from agentainer_lab_b200 import constants as K
-from resizeref import NoSpace, content, log_rows, relocate
+from resizeref import NoSpace, content, log_rows, relocate, relocate_loop
 from snapfile import HEADER, WORDS, sections
 
 P, M, V, R = K.AGR_CFG_PERSISTENCE, K.AGR_CFG_MINT_IDS, K.AGR_CFG_VARLEN, K.AGR_CFG_RING
@@ -147,3 +147,96 @@ def test_the_three_refusals():
         relocate(hd, ag, sec, P | M | V | R, 20, need_v - 1, 4096)
     with pytest.raises(NoSpace, match="resp"):
         relocate(hd, ag, sec, P | M | V | R, 20, 4096, 20 * 32 - 1)
+
+
+def random_file(seed, flags, S, tail, window, vcap=1 << 14, resp_cap=1 << 14):
+    """A parsed full file with random words on every row of the window: about a third of the rows dead (state 0) but keeping
+    their lengths and offsets, response / error lengths from 0 up (many 0), the live rows' bytes laid out from a random point
+    of each byte ring (wrapping), logs of random window rows and 0xFFFFFFFF entries."""
+    rng = np.random.default_rng(seed)
+    ring, var = bool(flags & R), bool(flags & V)
+    used = tail + window
+    hd = np.zeros(1, dtype=HEADER)[0]
+    hd["magic"], hd["flags"], hd["shard"], hd["gen"], hd["id_secret"] = b"AGRSNAP3", flags, 1, 1, 5
+    hd["tail"], hd["rows_used"], hd["released_total"], hd["scan_lo"] = tail, used, tail, tail
+    hd["slab_rows"], hd["vcap"], hd["resp_cap"] = S if ring else used, vcap if var else 0, resp_cap
+    nlog = [int(rng.integers(0, 300)), int(rng.integers(0, 40))]
+    hd["log_len"] = nlog
+    hd["vused"], hd["resp_used"] = (vcap + 77 if ring else vcap) if var else 0, resp_cap + 33 if ring else resp_cap
+    sec = {name: rng.integers(0, 1 << 31, count).astype(dt) if name in WORDS else np.zeros(count, dtype=dt)
+           for name, dt, count in sections(hd)}
+    sec["slab"][:] = rng.integers(0, 256, len(sec["slab"]), dtype=np.uint8)
+    sec["resp"][:] = rng.integers(0, 256, len(sec["resp"]), dtype=np.uint8)
+    cap = int(hd["slab_rows"])
+    phys = [(L % cap) if ring else L for L in range(tail, used)]
+    vat, rat = int(rng.integers(0, vcap)), int(rng.integers(0, resp_cap)) & ~15
+    for p in phys:
+        live = rng.random() > 0.35
+        sec["state"][p] = (0x20 | 1) if live else 0
+        for ln in ("resp_len", "err_len"):
+            sec[ln][p] = rng.choice([0, 0, 1, 15, 16, 17, 40])
+        if var:
+            sec["vlen"][p] = int(rng.integers(1, 30))
+        if not live:
+            continue
+        if var:
+            n = int(sec["vlen"][p])
+            if not ring and vat + n > vcap:
+                vat = 0
+            sec["voff"][p] = vat % vcap if ring else vat
+            if ring and vat % vcap + n > vcap:                # a record never straddles the ring's end
+                vat += vcap - vat % vcap
+                sec["voff"][p] = 0
+            vat += n
+        for off, ln in (("resp_off", "resp_len"), ("err_off", "err_len")):
+            n = int(sec[ln][p])
+            if ring and rat % resp_cap + n > resp_cap:
+                rat += resp_cap - rat % resp_cap
+            if not ring and rat + n > resp_cap:
+                rat = 0
+            sec[off][p] = rat % resp_cap
+            rat += (n + 15) & ~15
+    for j, name in enumerate(("completed_log", "failed_log")):
+        e = rng.choice(phys, nlog[j]).astype(np.uint32) if phys else np.zeros(nlog[j], dtype=np.uint32)
+        e[rng.random(nlog[j]) < 0.2] = NONE
+        sec[name][:] = e
+    return hd, b"ag", sec
+
+
+@pytest.mark.parametrize("seed", range(6))
+@pytest.mark.parametrize("case", ["ring_mid", "ring_wraps", "ring_at_0", "append"])
+@pytest.mark.parametrize("flags", [P | M | R, P | V | R, P | M | V | R])
+def test_vector_form_is_the_loop(flags, case, seed):
+    S = 97
+    tail, window, src_flags = {"ring_mid": (2 * S + 10, 60, flags), "ring_wraps": (3 * S + 70, S - 3, flags),
+                               "ring_at_0": (5 * S, S, flags), "append": (0, 120, flags & ~R)}[case]
+    hd, ag, sec = random_file(seed, src_flags, S, tail, window)
+    for slab_rows in (window, window + 1, 64 + seed, 256, 1000):
+        try:
+            want = relocate_loop(hd, ag, sec, flags, slab_rows, 1 << 14, 1 << 14)
+        except NoSpace as e:
+            with pytest.raises(NoSpace, match=str(e)):
+                relocate(hd, ag, sec, flags, slab_rows, 1 << 14, 1 << 14)
+            continue
+        got = relocate(hd, ag, sec, flags, slab_rows, 1 << 14, 1 << 14)
+        assert got[0].tobytes() == want[0].tobytes() and got[1] == want[1]
+        for name in want[2]:
+            assert np.array_equal(got[2][name], want[2][name]), (slab_rows, name)
+    if window:
+        assert (sec["state"] == 0).any() and (sec["resp_len"][sec["state"] == 0] > 0).any()
+        assert (sec["completed_log"] == NONE).any() or len(sec["completed_log"]) < 5
+
+
+@pytest.mark.parametrize("flags", [P | M | R, P | M | V | R])
+def test_vector_form_refuses_like_the_loop(flags):
+    hd, ag, sec = random_file(3, flags, 64, 200, 50)
+    _, _, packed = relocate_loop(hd, ag, sec, flags, 64, 1 << 20, 1 << 20)
+    need_v, need_r = (len(packed["slab"]) if flags & V else 0), len(packed["resp"])
+    for args, word in (((49, 1 << 20, 1 << 20), "window"), ((64, 1 << 20, need_r - 1), "resp"), ((64, 1 << 20, need_r), None)) + \
+            ((((64, need_v - 1, 1 << 20), "vslab"), ((64, need_v, 1 << 20), None)) if flags & V else ()):
+        for fn in (relocate, relocate_loop):
+            if word is None:
+                fn(hd, ag, sec, flags, *args)
+            else:
+                with pytest.raises(NoSpace, match=word):
+                    fn(hd, ag, sec, flags, *args)
