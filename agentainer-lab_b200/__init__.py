@@ -7,6 +7,6 @@ Engine without an sm_90 device raises."""
 from .build import build_native, build_host, lib_path   # noqa: F401
 from .binding import (                              # noqa: F401
     Engine, AgrError, load_library, record_dtype, header_dtype, outcome_dtype, verdict_dtype, dispatch_dtype,
-    synth_fill_host, synth_agent_id, agent_hash, agent_shard, comm_unique_id, json_decode, ABI_SYMBOLS,
+    synth_fill_host, synth_agent_id, var_record_len, agent_hash, agent_shard, comm_unique_id, json_decode, ABI_SYMBOLS,
 )
 from . import constants                             # noqa: F401

@@ -244,6 +244,14 @@ def comm_unique_id() -> bytes:
     return bytes(buf)
 
 
+def var_record_len(rec: np.ndarray) -> int:
+    """Stored length of the variable-length record whose 96-byte header starts rec (uint8): 96 + its payload rounded up to 16
+    bytes, capped at AGR_VAR_MAX_RECORD (include/agentainer_gpu.h)."""
+    h = np.frombuffer(np.ascontiguousarray(rec[: K.AGR_HEADER_BYTES]).tobytes(), dtype=header_dtype)[0]
+    p = int(h["path_len"]) + int(h["hdr_len"]) + int(h["body_len"])
+    return min(K.AGR_VAR_MAX_RECORD, K.AGR_HEADER_BYTES + (p + 15) // 16 * 16)
+
+
 def agent_hash(agent_id: str) -> int:
     return load_library().agr_agent_hash(agent_id.encode())
 
@@ -544,10 +552,16 @@ class Engine:
         return rc, res
 
     # ---- tickets (AGR_CFG_COMBINE)
-    def submit_ingest(self, rec: np.ndarray) -> int:
-        """agr_submit_ingest: one record into the request ring; collect its answer with poll()."""
-        assert rec.dtype == record_dtype
-        r = np.ascontiguousarray(rec.reshape(1))
+    def submit_ingest(self, rec) -> int:
+        """agr_submit_ingest: one record into the request ring; collect its answer with poll().  On a variable-length engine rec
+        is one variable-length record, bytes or a uint8 array holding at least the stored length its header gives."""
+        if isinstance(rec, (bytes, bytearray)) or (isinstance(rec, np.ndarray) and rec.dtype == np.uint8):
+            r = np.frombuffer(bytes(rec), dtype=np.uint8) if isinstance(rec, (bytes, bytearray)) else np.ascontiguousarray(rec).reshape(-1)
+            if len(r) < K.AGR_HEADER_BYTES or len(r) < var_record_len(r):
+                raise ValueError("a variable-length record shorter than the stored length its header gives")
+        else:
+            assert rec.dtype == record_dtype
+            r = np.ascontiguousarray(rec.reshape(1))
         t = C.c_uint64()
         while True:
             rc = self.lib.agr_submit_ingest(self.h, _ptr(r), C.byref(t))

@@ -289,7 +289,7 @@ static int create_impl(const agr_config* cfg_in, agr_handle* h) {
     TRY(dev_alloc(h, &h->d_min_inq, (size_t)1, false));
     if (c.flags & AGR_CFG_ONLINE_SNAPSHOT) TRY(snap_online_create(h));
     CK(cudaStreamSynchronize(h->stream));
-    if ((c.flags & AGR_CFG_COMBINE) && !varlen) TRY(svc_create(h));
+    if (c.flags & AGR_CFG_COMBINE) TRY(svc_create(h));
     return 0;
 }
 
@@ -623,7 +623,7 @@ int reserve_rows_locked(agr_handle* h, uint32_t n, uint64_t* first) {
 // The byte ring of a variable-length engine takes `bytes` as one piece (a blob of agr_ingest_var, or the slots of one row
 // reservation): vbytes_fit checks (*vpad = the bytes skipped at the end of the lap), vbytes_take hands the piece out and
 // returns its physical offset.  The rows are reserved in between, so that a refused call leaves both rings as they were.
-static int vbytes_fit(const agr_handle* h, uint64_t bytes, uint64_t* vpad) {
+int vbytes_fit(const agr_handle* h, uint64_t bytes, uint64_t* vpad) {
     *vpad = 0;
     if (!is_ring(h)) {
         if (h->vused + bytes > h->vcap) return fail(AGR_ENOSPC, "byte slab full");
@@ -634,7 +634,7 @@ static int vbytes_fit(const agr_handle* h, uint64_t bytes, uint64_t* vpad) {
     if (!ring_fits_pinned(h, h->vused, h->vtail, h->pin_vtail, h->vcap, bytes)) return fail(AGR_ENOSPC, std::string("byte slab ") + PINNED_FULL);
     return 0;
 }
-static uint64_t vbytes_take(agr_handle* h, uint64_t bytes, uint64_t vpad) {
+uint64_t vbytes_take(agr_handle* h, uint64_t bytes, uint64_t vpad) {
     h->vused += vpad;
     const uint64_t base = is_ring(h) ? h->vused % h->vcap : h->vused;
     h->vused += bytes;
@@ -1198,6 +1198,14 @@ int agr_ingest_var(agr_handle* h, const uint8_t* blob, const uint32_t* offsets, 
                    uint64_t* first_rid) {
     if (!h || (n && (!blob || !offsets))) return fail(AGR_EINVAL, "NULL argument");
     if (!(h->cfg.flags & AGR_CFG_VARLEN)) return fail(AGR_EINVAL, "engine was not created with AGR_CFG_VARLEN");
+    if (h->svc && n >= 1 && n <= SVC_MAX_CALL && offsets[0] == 0) {
+        // single-request front end when every record is in the compact form (its length is the one its header gives): such a
+        // record is a record span of the ring (agr_svc.h); any other blob is one locked batch
+        bool compact = true;
+        for (uint32_t i = 0; i < n && compact; ++i) compact = offsets[i + 1] >= offsets[i] + AGR_HEADER_BYTES;
+        for (uint32_t i = 0; i < n && compact; ++i) compact = offsets[i + 1] - offsets[i] == svc_rec_len_at(blob + offsets[i]);
+        if (compact) return svc_ingest_var(h, blob, offsets, n, out, ids, first_rid);
+    }
     HLock lk(h);
     CK(cudaSetDevice(h->device));
     if (n > h->cfg.max_batch) return fail(AGR_EINVAL, "n exceeds max_batch");

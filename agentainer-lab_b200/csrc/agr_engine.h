@@ -311,6 +311,8 @@ int agent_bind_locked(agr_handle* h, uint32_t slot, const char* agent_id, uint8_
 uint64_t ingested_bound(const agr_handle* h);
 void resv_remove(agr_handle* h, uint64_t first, uint64_t end);
 int reserve_rows_locked(agr_handle* h, uint32_t n, uint64_t* first);
+int vbytes_fit(const agr_handle* h, uint64_t bytes, uint64_t* vpad);
+uint64_t vbytes_take(agr_handle* h, uint64_t bytes, uint64_t vpad);
 int reserve_run_locked(agr_handle* h, uint32_t n, bool listed, slot_run* run);
 int row_runs(agr_handle* h, uint64_t first, uint32_t n, std::vector<slot_run>& out);
 int op_time_begin(agr_handle* h, int g);
@@ -330,6 +332,8 @@ constexpr const char* K2_LOG_FULL =
 int svc_create(agr_handle* h);
 void svc_destroy(agr_handle* h);
 int svc_ingest(agr_handle* h, const agr_record* recs, uint32_t n, agr_verdict* out, uint8_t (*ids)[16], uint64_t* first_rid);
+int svc_ingest_var(agr_handle* h, const uint8_t* blob, const uint32_t* offsets, uint32_t n, agr_verdict* out, uint8_t (*ids)[16],
+                   uint64_t* first_rid);
 int svc_complete(agr_handle* h, const agr_outcome* outs, uint32_t n, int32_t* results);
 int svc_complete_ex(agr_handle* h, const agr_outcome* outs, uint32_t n, const uint8_t* bytes, const uint64_t* offsets,
                     const uint32_t* hdr_lens, int32_t* results);

@@ -6,7 +6,7 @@
 // Host side of agr_svc.h.  Lock-free for the callers: one fetch_add claims ring slots, the payload is written into pinned
 // device-mapped memory, a release store publishes it, and the caller waits on a word the GPU writes.  One dispatcher thread
 // per handle turns the published prefix of the ring into batch descriptors; the resident service kernel (k_svc) does the rest.
-cudaError_t agr_launch_svc(const agr_dev& d, const svc_dev& v, const agr_k2_scratch& k2, unsigned long long next_seq, cudaStream_t st);
+cudaError_t agr_launch_svc(const agr_dev& d, const svc_dev& v, const agr_k2_scratch& k2, unsigned long long next_seq, bool var, cudaStream_t st);
 unsigned long long agr_svc_desc_check(const svc_desc* dsc);
 
 namespace agr_impl __attribute__((visibility("hidden"))) {
@@ -64,7 +64,7 @@ static int svc_start_locked(agr_handle* h) {
     sync_window(h);
     // resume at the first batch the previous incarnation did not run (normally none is pending; a batch published right
     // before this launch is)
-    cudaError_t e = agr_launch_svc(h->d, v, s->k2, s->ctl->done_seq + 1, h->stream);
+    cudaError_t e = agr_launch_svc(h->d, v, s->k2, s->ctl->done_seq + 1, (h->cfg.flags & AGR_CFG_VARLEN) != 0, h->stream);
     if (e != cudaSuccess) { s->fatal = AGR_ECUDA; return fail(AGR_ECUDA, std::string("service kernel launch: ") + cudaGetErrorString(e)); }
     s->running = true;
     s->starts++;
@@ -83,8 +83,14 @@ static void svc_dispatcher(agr_handle* h) {
     uint64_t to = s->taken;
     uint32_t nstaged = 0;                                        // records + outcomes with bytes: one 512 B stage slot of k_svc each
     uint32_t kinds[SVC_MAX_OPS / 16] = {0}, conts[SVC_MAX_OPS / 32] = {0};
+    // variable-length engines: records are record spans, and a batch's record bytes (one piece of the byte ring) stay within what
+    // vbytes_fit takes in one piece
+    const bool var = (h->cfg.flags & AGR_CFG_VARLEN) != 0;
+    const uint64_t rec_bytes_max = is_ring(h) ? h->vcap / 2 : ~0ULL;
+    uint64_t rec_bytes = 0;
     while (!s->shutdown.load(std::memory_order_acquire)) {
-        svc_scan(s, s->taken, &to, &nstaged, kinds, 128u, conts); // (csrc/agr_ring.hpp: shared with the CPU simulation of the ring)
+        // (csrc/agr_ring.hpp: shared with the CPU simulations of the ring)
+        svc_scan(s, s->taken, &to, &nstaged, kinds, 128u, conts, var ? &rec_bytes : nullptr, rec_bytes_max);
         const auto now = std::chrono::steady_clock::now();
         if (to == s->taken) {
             const auto idle = std::chrono::duration_cast<std::chrono::microseconds>(now - last_work).count();
@@ -117,7 +123,7 @@ static void svc_dispatcher(agr_handle* h) {
         std::lock_guard<std::mutex> hl(h->mu);
         if (s->fatal.load()) {
             svc_fail_ops(s, s->taken, to, s->fatal.load(), false, conts);
-            s->taken = to; nstaged = 0; memset(kinds, 0, sizeof kinds); memset(conts, 0, sizeof conts);
+            s->taken = to; nstaged = 0; rec_bytes = 0; memset(kinds, 0, sizeof kinds); memset(conts, 0, sizeof conts);
             continue;
         }
         if (s->running && s->ctl->state != 1u) {                // it left on its own (safety timeout): note it and start another
@@ -129,12 +135,13 @@ static void svc_dispatcher(agr_handle* h) {
         // records, and the outcomes with bytes with their segments' region (16 B-rounded, in ring order; a span's length is
         // clamped to the slots the batch holds of it, as the kernel does)
         const uint32_t count = (uint32_t)(to - s->taken);
-        uint32_t nrec = 0, nbytes = 0, ncont = 0;
+        uint32_t nrec = 0, rec_slots = 0, nbytes = 0, ncont = 0;  // records (rows), their ring slots (record spans' continuations too)
         uint64_t byte_total = 0;
         for (uint32_t k = 0; k < count; ++k) {
             const uint32_t kd = (kinds[k >> 4] >> ((k & 15u) * 2u)) & 3u;
-            if (kd == SVC_OP_RECORD) nrec++;
+            if (kd == SVC_OP_RECORD) rec_slots++;
             if ((conts[k >> 5] >> (k & 31u)) & 1u) { ncont++; continue; }
+            if (kd == SVC_OP_RECORD) nrec++;
             if (kd == SVC_OP_OUTCOME_BYTES) {                    // (the slot's payload is visible: its ready word was acquired)
                 uint32_t len;
                 memcpy(&len, s->payload + (size_t)((s->taken + k) & (SVC_SLOTS - 1u)) * SVC_PAYLOAD + SVC_BYTES_HDR + 4, 4);
@@ -144,10 +151,16 @@ static void svc_dispatcher(agr_handle* h) {
         }
         uint64_t first = 0;
         bool have_rows = true;
-        if (nrec) {
-            if (reserve_rows_locked(h, nrec, &first) < 0) { svc_fail_ops(s, s->taken, to, AGR_ENOSPC, true, conts); have_rows = false; }
-        }
         svc_desc dsc{};
+        if (nrec) {
+            // rows, and on a variable-length engine the records' bytes, as one piece in agr_ingest_var's order: a refusal leaves
+            // both rings as they were (the scan kept the bytes within vbytes_fit's limit unless one record alone exceeds it)
+            uint64_t vpad = 0;
+            int rc = var ? vbytes_fit(h, rec_bytes, &vpad) : 0;
+            if (rc == 0) rc = reserve_rows_locked(h, nrec, &first) < 0 ? AGR_ENOSPC : 0;
+            if (rc == 0 && var) dsc.vbase = vbytes_take(h, rec_bytes, vpad);
+            if (rc < 0) { svc_fail_ops(s, s->taken, to, rc, true, conts); have_rows = false; }
+        }
         for (uint32_t k = 0; k < (uint32_t)(to - s->taken); ++k) {
             uint32_t kd = (kinds[k >> 4] >> ((k & 15u) * 2u)) & 3u;
             if (kd == SVC_OP_RECORD && !have_rows) kd = SVC_OP_SKIP;
@@ -159,7 +172,7 @@ static void svc_dispatcher(agr_handle* h) {
             unsigned long long off;
             if (resp_reserve_locked(h, byte_total, byte_total, &off) == 0) dsc.resp_base = off;
         }
-        dsc.from = s->taken; dsc.count = count; dsc.n_records = have_rows ? nrec : 0u;
+        dsc.from = s->taken; dsc.count = count; dsc.n_records = have_rows ? nrec : 0u; dsc.rec_slots = have_rows ? rec_slots : 0u;
         dsc.first_l = first; dsc.first_p = (uint32_t)phys_row(h, first);
         dsc.tail = h->tail; dsc.head_l = h->rows_used; dsc.tail_phys = is_ring(h) ? (uint32_t)(h->tail % h->cfg.slab_rows) : 0u;
         dsc.idx_base = h->d.idx_base;
@@ -179,7 +192,7 @@ static void svc_dispatcher(agr_handle* h) {
         s->ops.fetch_add(dsc.count - ncont, std::memory_order_relaxed);     // operations: a span counts once
         h->k1_launches += nrec ? 1 : 0;                         // accounting: batches with records / with outcomes served by k_svc
         h->k2_launches += (dsc.count > nrec) ? 1 : 0;
-        nstaged = 0; memset(kinds, 0, sizeof kinds); memset(conts, 0, sizeof conts);
+        nstaged = 0; rec_bytes = 0; memset(kinds, 0, sizeof kinds); memset(conts, 0, sizeof conts);
         if (!s->running && svc_start_locked(h) < 0) {
             // could not launch: nothing will ever process this batch — fail it from here
             svc_fail_ops(s, dsc.from, to, AGR_ECUDA, false, dsc.cont);
@@ -267,10 +280,9 @@ static inline void svc_request_id(agr_handle* h, uint64_t a, uint64_t rid, uint8
     } else memcpy(id, h->svc->payload + (size_t)(a & (SVC_SLOTS - 1u)) * SVC_PAYLOAD, 16);
 }
 
-int svc_ingest(agr_handle* h, const agr_record* recs, uint32_t n, agr_verdict* out, uint8_t (*ids)[16], uint64_t* first_rid) {
+// collects the answers of the records a blocking call handed over (ring slots pos[0..n), in call order)
+static int svc_collect_records(agr_handle* h, const uint64_t* pos, uint32_t n, agr_verdict* out, uint8_t (*ids)[16], uint64_t* first_rid) {
     svc_host* s = h->svc;
-    uint64_t pos[SVC_MAX_CALL];
-    for (uint32_t i = 0; i < n; ++i) while (!svc_submit_one(s, SVC_OP_RECORD, &recs[i], sizeof(agr_record), &pos[i])) {}   // in call order
     int rc = 0;
     for (uint32_t i = 0; i < n; ++i) {
         svc_answer r; svc_wait(s, pos[i], &r);
@@ -283,8 +295,21 @@ int svc_ingest(agr_handle* h, const agr_record* recs, uint32_t n, agr_verdict* o
         }
         svc_release(s, pos[i]);
     }
+    if (rc == AGR_EINVAL) return fail(rc, "record larger than half the byte slab");
     if (rc < 0) return fail(rc, rc == AGR_ENOSPC ? "slab full" : "single-request front end: CUDA error");
     return 0;
+}
+int svc_ingest(agr_handle* h, const agr_record* recs, uint32_t n, agr_verdict* out, uint8_t (*ids)[16], uint64_t* first_rid) {
+    uint64_t pos[SVC_MAX_CALL];
+    for (uint32_t i = 0; i < n; ++i) while (!svc_submit_one(h->svc, SVC_OP_RECORD, &recs[i], sizeof(agr_record), &pos[i])) {}   // in call order
+    return svc_collect_records(h, pos, n, out, ids, first_rid);
+}
+// agr_ingest_var through the ring: record i is the svc_rec_len bytes at blob + offsets[i] (the caller checked that they are)
+int svc_ingest_var(agr_handle* h, const uint8_t* blob, const uint32_t* offsets, uint32_t n, agr_verdict* out, uint8_t (*ids)[16],
+                   uint64_t* first_rid) {
+    uint64_t pos[SVC_MAX_CALL];
+    for (uint32_t i = 0; i < n; ++i) while (!svc_submit_record(h->svc, blob + offsets[i], &pos[i])) {}
+    return svc_collect_records(h, pos, n, out, ids, first_rid);
 }
 int svc_complete(agr_handle* h, const agr_outcome* outs, uint32_t n, int32_t* results) {
     svc_host* s = h->svc;
@@ -353,7 +378,13 @@ static int submit_one(agr_handle* h, uint32_t kind, const void* item, size_t byt
     *ticket = a | (kind == SVC_OP_OUTCOME ? TICKET_OUTCOME : 0ULL);
     return 0;
 }
-int agr_submit_ingest(agr_handle* h, const agr_record* rec, agr_ticket* ticket) { return submit_one(h, SVC_OP_RECORD, rec, sizeof(agr_record), ticket); }
+int agr_submit_ingest(agr_handle* h, const agr_record* rec, agr_ticket* ticket) {
+    if (!h || !rec || !ticket || !h->svc || !(h->cfg.flags & AGR_CFG_VARLEN)) return submit_one(h, SVC_OP_RECORD, rec, sizeof(agr_record), ticket);
+    uint64_t a = 0;                                              // a variable-length record: a record span of its stored length
+    if (!svc_submit_record(h->svc, reinterpret_cast<const uint8_t*>(rec), &a)) return AGR_EAGAIN;
+    *ticket = a;
+    return 0;
+}
 int agr_submit_complete(agr_handle* h, const agr_outcome* outcome, agr_ticket* ticket) { return submit_one(h, SVC_OP_OUTCOME, outcome, sizeof(agr_outcome), ticket); }
 static int collect(agr_handle* h, agr_ticket ticket, const svc_answer& r, agr_result* out) {
     svc_host* s = h->svc;

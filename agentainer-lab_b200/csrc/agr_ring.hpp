@@ -1,7 +1,8 @@
 // agr_ring.hpp — the CALLERS' side of the single-request ring (AGR_CFG_COMBINE; layout and protocol: agr_svc.h).
 //
 // Everything a calling thread does to hand one operation over and to collect its answer, as templates over the host-side ring
-// object H (agr_engine.h's svc_host; the stand-ins of tests/ring_sim.cpp, tests/ring_sim_bytes.cpp and tests/ring_sim_span.cpp).
+// object H (agr_engine.h's svc_host; the stand-ins of tests/ring_sim.cpp, tests/ring_sim_bytes.cpp, tests/ring_sim_span.cpp and
+// tests/ring_sim_var.cpp).
 // H provides:
 //   svc_res* res; uint8_t* payload; std::atomic<uint32_t>* ready;          pinned, device-mapped in the engine
 //   std::atomic<uint64_t> head, scanned; std::atomic<uint32_t> waiters; uint32_t spin_cpus;
@@ -111,17 +112,11 @@ static inline void svc_copy_seg(uint8_t* dst, const uint8_t* a, uint32_t a_len, 
     }
     if (n) memcpy(dst, b + (off - a_len), n);
 }
-// hands over ONE outcome whose segment a | b may be longer than a slot holds (agr_submit_complete_large).  Up to SVC_BYTES_MAX
-// bytes it is svc_submit_outcome_bytes; above that a SPAN (agr_svc.h) of 1 + svc_span_conts(len) consecutive slots, claimed with
-// one fetch_add (slot numbers wrap past the ring's end like any other).  It is handed over only if every slot of it is free;
-// otherwise all of them go out as no-ops and the result is false, as for svc_submit_one.  a_len + b_len <=
-// AGR_OUT_TICKET_MAX_BYTES (the caller checks).
-template <class H>
-static bool svc_submit_outcome_span(H* s, const void* outcome, uint32_t hdr_len, const uint8_t* a, uint32_t a_len, const uint8_t* b,
-                                    uint32_t b_len, uint64_t* abs) {
-    const uint32_t len = a_len + b_len;
-    if (len <= SVC_BYTES_MAX) return svc_submit_outcome_bytes(s, outcome, hdr_len, a, a_len, b, b_len, abs);
-    const uint32_t n = 1u + svc_span_conts(len);
+// hands over ONE operation that takes n consecutive slots (a SPAN, agr_svc.h), claimed with one fetch_add (slot numbers wrap past
+// the ring's end like any other); write(j, slot) streams the bytes of its j-th slot.  It is handed over only if every slot of
+// it is free; otherwise all of them go out as no-ops and the result is false, as for svc_submit_one.
+template <class H, class W>
+static bool svc_submit_span(H* s, uint32_t kind, uint32_t n, W&& write, uint64_t* abs) {
     const uint64_t a0 = s->head.fetch_add(n, std::memory_order_relaxed);
     // every slot is looked at, also after one that is not free: a slot's ready word may be written again only once the
     // dispatcher has consumed its previous lap (svc_slot_free waits for that before it answers false)
@@ -131,23 +126,11 @@ static bool svc_submit_outcome_span(H* s, const void* outcome, uint32_t hdr_len,
         ok = svc_slot_free(s, x, (uint32_t)(x & (SVC_SLOTS - 1u)), (uint32_t)(x / SVC_SLOTS)) && ok;
     }
     if (ok) {
-        alignas(16) uint8_t item[SVC_PAYLOAD];
-        memcpy(item, outcome, SVC_BYTES_HDR);                         // head: outcome, hdr_len, len, the first SVC_BYTES_MAX bytes
-        memcpy(item + SVC_BYTES_HDR, &hdr_len, 4);
-        memcpy(item + SVC_BYTES_HDR + 4, &len, 4);
-        svc_copy_seg(item + SVC_BYTES_DATA, a, a_len, b, 0u, SVC_BYTES_MAX);
-        svc_stream_slot(s, (uint32_t)(a0 & (SVC_SLOTS - 1u)), item, SVC_PAYLOAD);
-        for (uint32_t j = 1; j < n; ++j) {                            // continuations: SVC_PAYLOAD bytes each, the last one 16 B-rounded
-            const uint32_t off = SVC_BYTES_MAX + (j - 1u) * SVC_PAYLOAD, m = len - off < SVC_PAYLOAD ? len - off : SVC_PAYLOAD;
-            const uint32_t used = (m + 15u) & ~15u;
-            svc_copy_seg(item, a, a_len, b, off, m);
-            memset(item + m, 0, used - m);
-            svc_stream_slot(s, (uint32_t)((a0 + j) & (SVC_SLOTS - 1u)), item, used);
-        }
+        for (uint32_t j = 0; j < n; ++j) write(j, (uint32_t)((a0 + j) & (SVC_SLOTS - 1u)));
         _mm_sfence();
     }
     // the continuations first, the head last: the dispatcher, which consumes slots in order, finds a published head complete
-    const uint32_t kind = ok ? (uint32_t)SVC_OP_OUTCOME_BYTES : (uint32_t)SVC_OP_SKIP;
+    if (!ok) kind = SVC_OP_SKIP;
     for (uint32_t j = n; j-- > 0;) {
         const uint64_t x = a0 + j;
         s->ready[x & (SVC_SLOTS - 1u)].store(((uint32_t)(x / SVC_SLOTS) + 1u) << 2 | kind, std::memory_order_release);
@@ -155,6 +138,42 @@ static bool svc_submit_outcome_span(H* s, const void* outcome, uint32_t hdr_len,
     if (s->sleeping.load(std::memory_order_seq_cst)) { std::lock_guard<std::mutex> lk(s->smu); s->scv.notify_one(); }
     *abs = a0;
     return ok;
+}
+// hands over ONE outcome whose segment a | b may be longer than a slot holds (agr_submit_complete_large).  Up to SVC_BYTES_MAX
+// bytes it is svc_submit_outcome_bytes; above that a span of 1 + svc_span_conts(len) slots.  a_len + b_len <=
+// AGR_OUT_TICKET_MAX_BYTES (the caller checks).
+template <class H>
+static bool svc_submit_outcome_span(H* s, const void* outcome, uint32_t hdr_len, const uint8_t* a, uint32_t a_len, const uint8_t* b,
+                                    uint32_t b_len, uint64_t* abs) {
+    const uint32_t len = a_len + b_len;
+    if (len <= SVC_BYTES_MAX) return svc_submit_outcome_bytes(s, outcome, hdr_len, a, a_len, b, b_len, abs);
+    return svc_submit_span(s, SVC_OP_OUTCOME_BYTES, 1u + svc_span_conts(len), [&](uint32_t j, uint32_t slot) {
+        alignas(16) uint8_t item[SVC_PAYLOAD];
+        if (j == 0) {                                                 // head: outcome, hdr_len, len, the first SVC_BYTES_MAX bytes
+            memcpy(item, outcome, SVC_BYTES_HDR);
+            memcpy(item + SVC_BYTES_HDR, &hdr_len, 4);
+            memcpy(item + SVC_BYTES_HDR + 4, &len, 4);
+            svc_copy_seg(item + SVC_BYTES_DATA, a, a_len, b, 0u, SVC_BYTES_MAX);
+            svc_stream_slot(s, slot, item, SVC_PAYLOAD);
+            return;
+        }
+        // continuations: SVC_PAYLOAD bytes each, the last one 16 B-rounded
+        const uint32_t off = SVC_BYTES_MAX + (j - 1u) * SVC_PAYLOAD, m = len - off < SVC_PAYLOAD ? len - off : SVC_PAYLOAD;
+        const uint32_t used = (m + 15u) & ~15u;
+        svc_copy_seg(item, a, a_len, b, off, m);
+        memset(item + m, 0, used - m);
+        svc_stream_slot(s, slot, item, used);
+    }, abs);
+}
+// hands over ONE variable-length record (agr_svc.h: record span): the svc_rec_len_at(rec) bytes at rec, 512 per slot, the last
+// slot holding the 16 B-rounded rest.  Only for a ring whose dispatcher scans with record spans (svc_scan's rec_bytes).
+template <class H>
+static bool svc_submit_record(H* s, const uint8_t* rec, uint64_t* abs) {
+    const uint32_t len = svc_rec_len_at(rec);
+    return svc_submit_span(s, SVC_OP_RECORD, svc_rec_slots(len), [&](uint32_t j, uint32_t slot) {
+        const uint32_t off = j * SVC_PAYLOAD;
+        svc_stream_slot(s, slot, rec + off, len - off < SVC_PAYLOAD ? len - off : SVC_PAYLOAD);
+    }, abs);
 }
 // A record's answer carries the low 48 bits of its row (arrival number): svc_answer.rid.  svc_row rebuilds the full row from H's
 // rows_out (rows handed out so far, stored with release by the dispatcher before it publishes the batch that names the row).
@@ -212,18 +231,24 @@ static inline void svc_release(H* s, uint64_t a) {       // everything of the an
 // continuations were published before it) says how many continuation slots follow; they count against both budgets, take the
 // head's kind in kinds[] and are marked in conts[] (1 bit per op, svc_desc.cont).  Callers that never hand over spans may pass
 // no conts.
+// rec_bytes (rings of a variable-length engine only): records are record spans too, and *rec_bytes sums their svc_rec_len; a record
+// that would take the sum above max_rec_bytes ends the batch unless it is the batch's first (the byte ring takes a batch's
+// records as one piece, and a piece above half a ring is refused outright — a lone record still gets its answer from there).
 template <class H>
 static inline void svc_scan(H* s, const uint64_t taken, uint64_t* to, uint32_t* nstaged, uint32_t* kinds, const uint32_t max_staged,
-                            uint32_t* conts = nullptr) {
+                            uint32_t* conts = nullptr, uint64_t* rec_bytes = nullptr, const uint64_t max_rec_bytes = 0) {
     while (*to - taken < SVC_MAX_OPS) {
         const uint32_t slot = (uint32_t)(*to & (SVC_SLOTS - 1u));
         const uint32_t rw = s->ready[slot].load(std::memory_order_acquire), kind = rw & 3u;
         if ((rw >> 2) != (uint32_t)(*to / SVC_SLOTS) + 1u) break;
-        uint32_t n = 1u;                                                  // slots the op takes
+        uint32_t n = 1u, rlen = 0u;                                       // slots the op takes, a record's stored length
         if (kind == SVC_OP_OUTCOME_BYTES) {
             uint32_t len;
             memcpy(&len, s->payload + (size_t)slot * SVC_PAYLOAD + SVC_BYTES_HDR + 4, 4);
             n += svc_span_conts(len);
+        } else if (kind == SVC_OP_RECORD && rec_bytes) {
+            rlen = svc_rec_len_at(s->payload + (size_t)slot * SVC_PAYLOAD);
+            n = svc_rec_slots(rlen);
         }
         if (n > 1u) {
             if (*to - taken + n > SVC_MAX_OPS) break;
@@ -232,7 +257,11 @@ static inline void svc_scan(H* s, const uint64_t taken, uint64_t* to, uint32_t* 
                 all = (s->ready[(slot + j) & (SVC_SLOTS - 1u)].load(std::memory_order_acquire) >> 2) == (uint32_t)((*to + j) / SVC_SLOTS) + 1u;
             if (!all) break;
         }
-        if (kind == SVC_OP_RECORD || kind == SVC_OP_OUTCOME_BYTES) { if (*nstaged + n > max_staged) break; *nstaged += n; }
+        const bool staged = kind == SVC_OP_RECORD || kind == SVC_OP_OUTCOME_BYTES;
+        if (staged && *nstaged + n > max_staged) break;
+        if (rlen && *rec_bytes && *rec_bytes + rlen > max_rec_bytes) break;
+        if (staged) *nstaged += n;
+        if (rlen) *rec_bytes += rlen;
         for (uint32_t j = 0; j < n; ++j, ++*to) {
             kinds[(*to - taken) >> 4] |= kind << (((*to - taken) & 15u) * 2u);
             if (j) conts[(*to - taken) >> 5] |= 1u << ((*to - taken) & 31u);

@@ -51,8 +51,10 @@ __host__ __device__ __forceinline__ unsigned long long svc_mix_word(uint32_t w, 
     return ((unsigned long long)w + 0x9e3779b97f4a7c15ULL * (i + 1u)) * (0xbf58476d1ce4e5b9ULL + 2ULL * i);
 }
 
-extern "C" __global__ void __launch_bounds__(SVC_THREADS, 1)
-k_svc(const agr_dev d0, const svc_dev v, const agr_k2_scratch k2, const unsigned long long first_seq) {
+// VAR: the record form of the engine.  false = fixed-stride records, one 512 B slot each; true = variable-length records, each a
+// record span (agr_svc.h) of svc_rec_len bytes, stored back to back from the batch's byte base with K1v's per-row words.
+template <bool VAR>
+__device__ __forceinline__ void svc_body(const agr_dev& d0, const svc_dev& v, const agr_k2_scratch& k2, const unsigned long long first_seq) {
     extern __shared__ __align__(128) uint8_t smem[];
     __shared__ __align__(16) uint32_t s_dw[2][64];           // the accepted descriptors, as words
     __shared__ uint32_t s_go[2], s_nout[2], s_nbyt[2];
@@ -60,6 +62,10 @@ k_svc(const agr_dev d0, const svc_dev v, const agr_k2_scratch k2, const unsigned
     // continuation slots, in ring order (so a span's slots lie next to each other)
     __shared__ uint16_t s_rec_op[2][SVC_MAX_RECS], s_out_op[2][SVC_MAX_OPS];
     __shared__ uint16_t s_out_stage[2][SVC_MAX_OPS];         // outcome -> its stage slot (outcomes with bytes), 0xffff = none
+    // VAR: record i -> the stage slot of its head (its span's slots follow it); its stored length and its place after the batch's
+    // byte base (a running sum of the lengths in ring order)
+    __shared__ uint8_t s_rhead[2][SVC_MAX_RECS];
+    __shared__ uint32_t s_rlen[SVC_MAX_RECS], s_roff[SVC_MAX_RECS], s_rsum[4];
     __shared__ uint32_t s_wc[12], s_wf[12];
     __shared__ unsigned long long s_wsum[12];
     __shared__ unsigned long long s_logbase[2];
@@ -111,8 +117,9 @@ k_svc(const agr_dev d0, const svc_dev v, const agr_k2_scratch k2, const unsigned
                 if (go == 1u) {
                     // op -> (record i | outcome j, and stage slot of an outcome with bytes) maps: thirty-two ops per step, running offsets
                     const svc_desc& D = *reinterpret_cast<const svc_desc*>(s_dw[st]);
-                    uint32_t br = 0, bo = 0, bb = 0;
+                    uint32_t br = 0, bo = 0, bb = 0, bh = 0;
                     const uint32_t lt = (1u << lane) - 1u;
+                    const uint32_t rslots = VAR ? D.rec_slots : D.n_records;       // stage slots of the records
                     for (uint32_t base = 0; base < D.count; base += 32u) {
                         const uint32_t op = base + lane;
                         const uint32_t kind = (op < D.count) ? ((D.kinds[op >> 4] >> ((op & 15u) * 2u)) & 3u) : 0u;
@@ -121,14 +128,19 @@ k_svc(const agr_dev d0, const svc_dev v, const agr_k2_scratch k2, const unsigned
                         const uint32_t mr = __ballot_sync(FULL, kind == SVC_OP_RECORD), mo = __ballot_sync(FULL, is_out);
                         const uint32_t mb = __ballot_sync(FULL, kind == SVC_OP_OUTCOME_BYTES);
                         if (kind == SVC_OP_RECORD) s_rec_op[st][br + __popc(mr & lt)] = (uint16_t)op;
+                        if (VAR) {                                                 // a record span's head
+                            const uint32_t mh = __ballot_sync(FULL, kind == SVC_OP_RECORD && !cont);
+                            if (kind == SVC_OP_RECORD && !cont) s_rhead[st][bh + __popc(mh & lt)] = (uint8_t)(br + __popc(mr & lt));
+                            bh += __popc(mh);
+                        }
                         if (is_out) {
                             const uint32_t oi = bo + __popc(mo & lt);
                             uint16_t sp = 0xffffu;
-                            if (kind == SVC_OP_OUTCOME_BYTES) sp = (uint16_t)(D.n_records + bb + __popc(mb & lt));
+                            if (kind == SVC_OP_OUTCOME_BYTES) sp = (uint16_t)(rslots + bb + __popc(mb & lt));
                             s_out_op[st][oi] = (uint16_t)op;
                             s_out_stage[st][oi] = sp;
                         }
-                        if (kind == SVC_OP_OUTCOME_BYTES) s_rec_op[st][D.n_records + bb + __popc(mb & lt)] = (uint16_t)op;
+                        if (kind == SVC_OP_OUTCOME_BYTES) s_rec_op[st][rslots + bb + __popc(mb & lt)] = (uint16_t)op;
                         br += __popc(mr); bo += __popc(mo); bb += __popc(mb);
                     }
                     nout = bo; nbyt = bb;
@@ -145,7 +157,7 @@ k_svc(const agr_dev d0, const svc_dev v, const agr_k2_scratch k2, const unsigned
             if (go == 1u) {
                 // pull the payloads out of host memory: eight 16-byte loads in flight per thread
                 const svc_desc& D = *reinterpret_cast<const svc_desc*>(s_dw[st]);
-                const uint32_t rec_chunks = (D.n_records + s_nbyt[st]) * 32u, total = rec_chunks + s_nout[st] * 4u;
+                const uint32_t rec_chunks = ((VAR ? D.rec_slots : D.n_records) + s_nbyt[st]) * 32u, total = rec_chunks + s_nout[st] * 4u;
                 const unsigned long long from = D.from;
                 for (uint32_t cb = tid; cb < total; cb += SVC_LOADERS * 8u) {
                     uint4 val[8];
@@ -202,31 +214,72 @@ k_svc(const agr_dev d0, const svc_dev v, const agr_k2_scratch k2, const unsigned
         const uint32_t lt = (1u << lane) - 1u;
 
         // ------------------------------------------------------------------ records: slab rows + checksum (warp per record)
-        for (uint32_t i = wwarp; i < nrec; i += SVC_WORKERS / 32u) {
-            const uint32_t rid = D.first_p + i;
-            const uint4 x = lds_v4(s_rec + (size_t)i * 512u + lane * 16u);
-            *reinterpret_cast<uint4*>(d.slab + (size_t)rid * AGR_REC + lane * 16u) = x;
-            uint32_t c0 = x.x + x.y + x.z + x.w;
-            uint32_t c1 = (4u * lane + 1u) * x.x + (4u * lane + 2u) * x.y + (4u * lane + 3u) * x.z + (4u * lane + 4u) * x.w;
-            c0 = __reduce_add_sync(FULL, c0); c1 = __reduce_add_sync(FULL, c1);
-            if (lane == 0) d.cksum[rid] = agr_cksum_pack(c0, c1);
+        if (!VAR) {
+            for (uint32_t i = wwarp; i < nrec; i += SVC_WORKERS / 32u) {
+                const uint32_t rid = D.first_p + i;
+                const uint4 x = lds_v4(s_rec + (size_t)i * 512u + lane * 16u);
+                *reinterpret_cast<uint4*>(d.slab + (size_t)rid * AGR_REC + lane * 16u) = x;
+                uint32_t c0 = x.x + x.y + x.z + x.w;
+                uint32_t c1 = (4u * lane + 1u) * x.x + (4u * lane + 2u) * x.y + (4u * lane + 3u) * x.z + (4u * lane + 4u) * x.w;
+                c0 = __reduce_add_sync(FULL, c0); c1 = __reduce_add_sync(FULL, c1);
+                if (lane == 0) d.cksum[rid] = agr_cksum_pack(c0, c1);
+            }
+        } else if (nrec) {
+            // the records' places: a running sum of their lengths in ring order (the dispatcher reserved the same total, from the
+            // same svc_rec_len); nrec <= SVC_MAX_RECS, so the first four worker warps hold them all
+            uint32_t len = 0u;
+            if (wt < nrec) {
+                const uint8_t* hp = s_rec + (size_t)s_rhead[st][wt] * 512u;
+                len = svc_rec_len(*reinterpret_cast<const uint32_t*>(hp + AGR_OFF_PATH_LEN), *reinterpret_cast<const uint32_t*>(hp + AGR_OFF_BODY_LEN));
+            }
+            uint32_t incl = len;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(FULL, incl, o); if ((int)lane >= o) incl += y; }
+            if (lane == 31u && wwarp < 4u) s_rsum[wwarp] = incl;
+            bar_sync(BAR_WORK, SVC_WORKERS);
+            if (wt < nrec) {
+                uint32_t pre = 0u;
+                for (uint32_t w = 0; w < wwarp; ++w) pre += s_rsum[w];
+                s_rlen[wt] = len; s_roff[wt] = pre + incl - len;
+            }
+            bar_sync(BAR_WORK, SVC_WORKERS);
+            // copy + checksum, warp per record: the record's L bytes lie contiguously in its span's stage slots; K1v's
+            // position-weighted checksum over its L / 16 chunks, and K1v's per-row place words
+            for (uint32_t i = wwarp; i < nrec; i += SVC_WORKERS / 32u) {
+                const uint32_t rid = D.first_p + i, chunks = s_rlen[i] >> 4;
+                const uint8_t* src = s_rec + (size_t)s_rhead[st][i] * 512u;
+                const unsigned long long off = D.vbase + s_roff[i];
+                uint4* dst = reinterpret_cast<uint4*>(d.slab + off);
+                uint32_t c0 = 0u, c1 = 0u;
+                for (uint32_t c = lane; c < chunks; c += 32u) {
+                    const uint4 x = lds_v4(src + (size_t)c * 16u);
+                    dst[c] = x;
+                    c0 += x.x + x.y + x.z + x.w;
+                    c1 += (4u * c + 1u) * x.x + (4u * c + 2u) * x.y + (4u * c + 3u) * x.z + (4u * c + 4u) * x.w;
+                }
+                c0 = __reduce_add_sync(FULL, c0); c1 = __reduce_add_sync(FULL, c1);
+                if (lane == 0) { d.cksum[rid] = agr_cksum_pack(c0, c1); d.voff[rid] = off; d.vlen[rid] = s_rlen[i]; }
+            }
         }
         // ------------------------------------------------------------------ records: decision chain, one record per thread
         uint32_t lc[K1_NLC + 1];
 #pragma unroll
         for (int c = 0; c <= K1_NLC; ++c) lc[c] = 0;
         if (wt < nrec) {
-            const uint8_t* hp = s_rec + (size_t)wt * 512u;
+            const uint8_t* hp = s_rec + (size_t)(VAR ? s_rhead[st][wt] : wt) * 512u;
             const uint4 h0 = lds_v4(hp), h1 = lds_v4(hp + 16), h2 = lds_v4(hp + 32), h3 = lds_v4(hp + 48), h4 = lds_v4(hp + 64), h5 = lds_v4(hp + 80);
             const uint32_t rid = D.first_p + wt;
+            // the payload bound: what the record form holds (K1v passes the stored length - 96)
+            const uint32_t cap = VAR ? s_rlen[wt] - AGR_OFF_PAYLOAD : AGR_REC - AGR_OFF_PAYLOAD;
             k1_ctx cx;
-            k1_begin(d, k1_agent_issue(d, h2, h3), h0, h1, h2, h3, h4, h5.x, AGR_REC - AGR_OFF_PAYLOAD, false, 0ULL, 0ULL, wt, cx);
+            k1_begin(d, k1_agent_issue(d, h2, h3), h0, h1, h2, h3, h4, h5.x, cap, false, 0ULL, 0ULL, wt, cx);
             const k1_result r = k1_finish(d, rid, h1, h5, cx, lc);
             d.state[rid] = r.state;
             d.route[rid] = r.route;
             // TTL bookkeeping of every record row, as the batch kernel keeps it (k1_note_time): a row k1_post_one promotes below
-            // is stored without having been stored here
-            if (d.cfg_flags & AGR_CFG_RING) {
+            // is stored without having been stored here.  Variable-length engines keep none in K1v (agr_expire resets the bounds
+            // of the chunks filled since its last call), and none here either.
+            if (!VAR && (d.cfg_flags & AGR_CFG_RING)) {
                 unsigned long long t = pack64(h4.x, h4.y);
                 atomicMin(d.cmin + rid / AGR_CHUNK_ROWS, t == 0ULL ? 1ULL : t == ~0ULL ? ~0ULL - 1ULL : t);   // 0 unknown, ~0 empty
                 d.mtime[rid] = t;
@@ -240,7 +293,7 @@ k_svc(const agr_dev d0, const svc_dev v, const agr_k2_scratch k2, const unsigned
             if (wt < nrec) {
                 const uint32_t rid = D.first_p + wt;
                 const uint32_t r = k1_post_one(d, rid, dupfix, delta, false, D.first_l);
-                const unsigned long long slot_abs = from + s_rec_op[st][wt], lrow = D.first_l + wt;
+                const unsigned long long slot_abs = from + s_rec_op[st][VAR ? s_rhead[st][wt] : wt], lrow = D.first_l + wt;
                 const uint2 vw = k1_verdict_word(r);
                 st_res(v.res + (slot_abs & (SVC_SLOTS - 1u)), vw.x, vw.y, (uint32_t)lrow, (uint32_t)((lrow >> 32) & 0xffffu) | (svc_tag(slot_abs) << 16));
             }
@@ -256,8 +309,9 @@ k_svc(const agr_dev d0, const svc_dev v, const agr_k2_scratch k2, const unsigned
 
         // ------------------------------------------------------------------ spans' continuation slots: their bytes are in the stage,
         // and nobody collects them — answered as collected, so their slots may be taken for the next lap
-        for (uint32_t i = wt; i < s_nbyt[st]; i += SVC_WORKERS) {
-            const uint32_t op = s_rec_op[st][nrec + i];
+        // (VAR: record spans' continuation slots too, among the records' stage slots)
+        for (uint32_t i = (VAR ? 0u : nrec) + wt; i < (VAR ? D.rec_slots : nrec) + s_nbyt[st]; i += SVC_WORKERS) {
+            const uint32_t op = s_rec_op[st][i];
             if ((D.cont[op >> 5] >> (op & 31u)) & 1u) {
                 const unsigned long long slot_abs = from + op;
                 st_res(v.res + (slot_abs & (SVC_SLOTS - 1u)), 0u, 0u, 0u, (svc_tag(slot_abs) | SVC_COLLECTED) << 16);
@@ -366,14 +420,25 @@ k_svc(const agr_dev d0, const svc_dev v, const agr_k2_scratch k2, const unsigned
     }
 }
 
-cudaError_t agr_launch_svc(const agr_dev& d, const svc_dev& v, const agr_k2_scratch& k2, unsigned long long next_seq, cudaStream_t st) {
-    static bool attr_done = false;
-    if (!attr_done) {
-        cudaError_t e = cudaFuncSetAttribute(k_svc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SVC_SMEM);
+extern "C" __global__ void __launch_bounds__(SVC_THREADS, 1)
+k_svc(const agr_dev d0, const svc_dev v, const agr_k2_scratch k2, const unsigned long long first_seq) {
+    svc_body<false>(d0, v, k2, first_seq);
+}
+extern "C" __global__ void __launch_bounds__(SVC_THREADS, 1)
+k_svc_var(const agr_dev d0, const svc_dev v, const agr_k2_scratch k2, const unsigned long long first_seq) {
+    svc_body<true>(d0, v, k2, first_seq);
+}
+
+// var: the engine's records are variable-length (k_svc_var)
+cudaError_t agr_launch_svc(const agr_dev& d, const svc_dev& v, const agr_k2_scratch& k2, unsigned long long next_seq, bool var, cudaStream_t st) {
+    static bool attr_done[2] = {false, false};
+    if (!attr_done[var]) {
+        cudaError_t e = cudaFuncSetAttribute(var ? k_svc_var : k_svc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SVC_SMEM);
         if (e != cudaSuccess) return e;
-        attr_done = true;
+        attr_done[var] = true;
     }
-    k_svc<<<1, SVC_THREADS, SVC_SMEM, st>>>(d, v, k2, next_seq);
+    if (var) k_svc_var<<<1, SVC_THREADS, SVC_SMEM, st>>>(d, v, k2, next_seq);
+    else k_svc<<<1, SVC_THREADS, SVC_SMEM, st>>>(d, v, k2, next_seq);
     return cudaGetLastError();
 }
 

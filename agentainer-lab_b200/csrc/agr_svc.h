@@ -17,7 +17,8 @@
 // Every other entry point stops the kernel first (it runs on the handle's stream), so the rest of the engine never sees it.
 #pragma once
 #include <stdint.h>
-#include "../../include/agentainer_gpu.h"   // AGR_OUT_TICKET_MAX_BYTES
+#include <string.h>
+#include "../../include/agentainer_gpu.h"   // AGR_OUT_TICKET_MAX_BYTES, AGR_VAR_MAX_RECORD
 #if defined(__CUDACC__)
 #define SVC_HD __host__ __device__
 #else
@@ -60,6 +61,28 @@ SVC_HD static inline uint32_t svc_span_len(uint32_t len, uint32_t conts) {
     const uint32_t cap = SVC_BYTES_MAX + conts * SVC_PAYLOAD;
     return len < cap ? len : cap;
 }
+// A RECORD SPAN (variable-length engines: agr_submit_ingest, agr_ingest_var through the ring): a record of stored length L
+// (svc_rec_len of its header) takes svc_rec_slots(L) consecutive slots, slot k holding bytes [512 k, 512 k + 512) of it — the
+// head holds the 96-byte header and the first 416 payload bytes, which is what a fixed-stride engine receives.  Same rules as an
+// outcome span: continuations published first and the head last, all slots or none, the continuations of kind SVC_OP_RECORD
+// marked in svc_desc.cont.  On a fixed-stride engine a record is one slot, whatever its header says.
+#define SVC_REC_SPAN_MAX (AGR_VAR_MAX_RECORD / SVC_PAYLOAD)   // 16 slots
+static_assert(SVC_REC_SPAN_MAX <= 128u / 2u, "a record span of the longest record must fit a batch that already holds other ops");
+// stored length of a variable-length record whose header holds lens (path_len | hdr_len << 16) and body_len: 96 + its 16 B-rounded
+// payload, capped at AGR_VAR_MAX_RECORD (a header whose lengths exceed that is stored at the cap and decided AGR_VF_BAD_LEN).
+// The submitting side, svc_scan, the dispatcher and the kernel all take a record's length from this one function.
+SVC_HD static inline uint32_t svc_rec_len(uint32_t lens, uint32_t body_len) {
+    const uint64_t p = (uint64_t)(lens & 0xffffu) + (lens >> 16) + body_len;
+    return p > AGR_VAR_MAX_RECORD - AGR_HEADER_BYTES ? AGR_VAR_MAX_RECORD : AGR_HEADER_BYTES + (uint32_t)((p + 15u) & ~15ULL);
+}
+// the same, from a header in memory (any alignment)
+SVC_HD static inline uint32_t svc_rec_len_at(const uint8_t* head) {
+    uint32_t w[2];
+    memcpy(w, head + 76, 8);                                  // path_len, hdr_len | body_len (agr_record)
+    return svc_rec_len(w[0], w[1]);
+}
+SVC_HD static inline uint32_t svc_rec_slots(uint32_t rec_len) { return (rec_len + SVC_PAYLOAD - 1u) / SVC_PAYLOAD; }
+
 // continuations that follow op in a batch of count ops (cont: svc_desc.cont, one bit per op)
 SVC_HD static inline uint32_t svc_conts_after(const uint32_t* cont, uint32_t op, uint32_t count) {
     uint32_t k = 0;
@@ -83,7 +106,11 @@ struct __attribute__((aligned(64))) svc_desc {
     uint64_t resp_base;                   // SVC_OP_OUTCOME_BYTES ops: physical offset of the batch's region of the response byte
                                           // slab (their 16 B-rounded segments in ring order), or SVC_NO_BYTES
     uint32_t cont[SVC_MAX_OPS / 32];      // words 32..39: 1 bit per op, set for a span's continuation slots
-    uint64_t reserved[10];
+    uint64_t vbase;                       // words 40..41, variable-length engines: physical byte offset in the byte slab of the
+                                          // batch's records (back to back in ring order, each svc_rec_len long)
+    uint32_t rec_slots;                   // word 42, variable-length engines: ring slots of the records, continuations included
+    uint32_t pad0;
+    uint64_t reserved[8];
     uint64_t check;                       // words 60..61: XOR of svc_mix_word over words 0..59 and 62..63
     uint64_t seq;                         // words 62..63: batch number; the kernel waits for desc[seq % SVC_DESCS].seq == seq
 };

@@ -11,13 +11,20 @@
 // fused = the bytes travel with the completion, agr_submit_complete_ex (tickets) or agr_complete_ex(n = 1) (blocking), and a
 // body above AGR_OUT_INLINE_BYTES falls back to the locked agr_complete_ex(n = 1); large = the same with
 // agr_submit_complete_large (blocking threads: it and agr_wait), which carries up to AGR_OUT_TICKET_MAX_BYTES in one ticket.
-//   bench_callers <threads> <seconds> [device] [mint|hash] [agents] [inflight per thread, 0 = blocking calls] [none|store|fused|large] [body]
+// With mode `var` the engine holds VARIABLE-LENGTH records (AGR_CFG_VARLEN) with chat bodies of 128 B - 4 KiB, log-uniform and
+// seeded per thread (BASELINE config 5): with <inflight> > 0 the ticket arm (AGR_CFG_COMBINE: agr_submit_ingest of the record ->
+// agr_poll -> agr_submit_complete -> agr_poll), with 0 the locked arm a variable-length deployment has without the ring
+// (agr_ingest_var(n = 1) -> agr_complete(n = 1), each taking the handle mutex and synchronising the stream).  A <body> given
+// with `var` makes every body that long instead.
+//   bench_callers <threads> <seconds> [device] [mint|hash] [agents] [inflight per thread, 0 = blocking calls] [none|store|fused|large|var] [body]
 #include <atomic>
 #include <chrono>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <algorithm>
+#include <cmath>
+#include <cstddef>
 #include <string>
 #include <thread>
 #include <vector>
@@ -39,6 +46,8 @@ int main(int argc, char** argv) {
     const int inflight = argc > 6 ? atoi(argv[6]) : 0;
     const int bytes_mode = argc > 7 ? (strcmp(argv[7], "store") == 0 ? 1 : strcmp(argv[7], "fused") == 0 ? 2 : strcmp(argv[7], "large") == 0 ? 3 : 0) : 0;
     const uint32_t body_len = argc > 8 ? (uint32_t)atoi(argv[8]) : 256u;
+    const bool var = argc > 7 && strcmp(argv[7], "var") == 0;
+    const uint32_t var_body = var && argc > 8 ? (uint32_t)atoi(argv[8]) : 0u;   // var: every body this long (0: the log-uniform mix)
     static constexpr char kHdr[] = "Content-Type: application/json\nX-Trace-Id: 0123456789abcdef0123\n";
     static_assert(sizeof kHdr - 1 == 64, "64 B of headers");
     const std::string hdr = kHdr;
@@ -56,6 +65,10 @@ int main(int argc, char** argv) {
         cfg.slab_rows = 1ull << 25; cfg.log_entries = cfg.slab_rows; cfg.resp_bytes = 32ull << 30;
     }
     cfg.flags = AGR_CFG_PERSISTENCE | AGR_CFG_COMBINE | (mint ? AGR_CFG_MINT_IDS : 0u);
+    if (var) {                                          // ~1.4 KiB per record on average: 16 Mi rows, 24 GiB of record bytes
+        cfg.slab_rows = 1ull << 24; cfg.log_entries = cfg.slab_rows; cfg.vslab_bytes = 24ull << 30;
+        cfg.flags = AGR_CFG_PERSISTENCE | AGR_CFG_VARLEN | (inflight > 0 ? AGR_CFG_COMBINE : 0u) | (mint ? AGR_CFG_MINT_IDS : 0u);
+    }
     agr_handle* h = nullptr;
     if (agr_create(&cfg, &h) < 0) { fprintf(stderr, "agr_create: %s\n", agr_last_error()); return 2; }
     agr_synth sy; memset(&sy, 0, sizeof sy); sy.seed = 7; sy.n_agents = (uint32_t)n_agents;
@@ -66,7 +79,7 @@ int main(int argc, char** argv) {
         if (agr_set_agent_state(h, id, AGR_AGENT_RUNNING) < 0) { fprintf(stderr, "set_agent_state: %s\n", agr_last_error()); return 2; }
     }
     std::atomic<bool> go{false}, stop{false};
-    std::atomic<uint64_t> total{0}, bad{0};
+    std::atomic<uint64_t> total{0}, bad{0}, vbytes{0};
     std::vector<std::vector<uint32_t>> lat(threads);
     std::vector<std::thread> ths;
     for (int t = 0; t < threads; ++t) ths.emplace_back([&, t] {
@@ -76,7 +89,30 @@ int main(int argc, char** argv) {
         agr_synth_fill_host(&s2, 0, 64, recs.data());
         uint64_t x = 0x1234 + t, n = 0;
         auto& my = lat[t]; my.reserve(1 << 20);
+        // var: the same records as variable-length ones, each with its own body (one 8 KiB cell per record)
+        std::vector<uint8_t> vrec(var ? 64u * AGR_VAR_MAX_RECORD : 0u, (uint8_t)'x');
+        std::vector<uint32_t> vlen(var ? 64u : 0u);
+        for (uint32_t k = 0; var && k < 64u; ++k) {
+            uint8_t* p = vrec.data() + (size_t)k * AGR_VAR_MAX_RECORD;
+            const agr_record& r = recs[k];
+            const uint32_t ph = (uint32_t)r.path_len + r.hdr_len;
+            const double u = (double)(splitmix(x) >> 11) * (1.0 / 9007199254740992.0);
+            uint32_t blen = var_body ? var_body : (uint32_t)(128.0 * std::exp(u * std::log(32.0)));   // or log-uniform in [128, 4096]
+            blen = std::min<uint32_t>(blen, AGR_VAR_MAX_RECORD - AGR_HEADER_BYTES - ph);
+            memcpy(p, &r, AGR_HEADER_BYTES);
+            memcpy(p + AGR_HEADER_BYTES, r.payload, ph);
+            memcpy(p + offsetof(agr_record, body_len), &blen, 4);
+            vlen[k] = AGR_HEADER_BYTES + ((ph + blen + 15u) & ~15u);
+            memset(p + AGR_HEADER_BYTES + ph + blen, 0, vlen[k] - AGR_HEADER_BYTES - ph - blen);
+            vbytes += vlen[k];
+        }
         while (!go.load(std::memory_order_acquire)) std::this_thread::yield();
+        auto record_of = [&](uint32_t k) -> agr_record* {               // record k of this thread, with a fresh id and seq
+            agr_record* r = var ? reinterpret_cast<agr_record*>(vrec.data() + (size_t)k * AGR_VAR_MAX_RECORD) : &recs[k];
+            if (!mint) { uint64_t a = splitmix(x), b = splitmix(x) | 1; memcpy(r->request_id, &a, 8); memcpy(r->request_id + 8, &b, 8); }
+            r->seq = n;
+            return r;
+        };
         if (inflight > 0) {
             // Tickets are answered in hand-over order (batch by batch), so the thread keeps its requests in a FIFO and polls only
             // the OLDEST one: a poll that says "not yet" means nothing younger is ready either.
@@ -87,9 +123,7 @@ int main(int argc, char** argv) {
             auto push = [&](const flight& f) { q[(head + count) % q.size()] = f; count++; };
             while (!stop.load(std::memory_order_relaxed)) {
                 while (count < q.size()) {                                 // start requests: StoreRequest + routing decision
-                    flight f; f.rec = (uint32_t)(n & 63); agr_record& r = recs[f.rec];
-                    if (!mint) { uint64_t a = splitmix(x), b = splitmix(x) | 1; memcpy(r.request_id, &a, 8); memcpy(r.request_id + 8, &b, 8); }
-                    r.seq = n;
+                    flight f; f.rec = (uint32_t)(n & 63); agr_record& r = *record_of(f.rec);
                     f.t0 = std::chrono::steady_clock::now();
                     const int rc = agr_submit_ingest(h, &r, &f.t);
                     if (rc == AGR_EAGAIN) break;
@@ -158,12 +192,13 @@ int main(int argc, char** argv) {
             return;
         }
         while (!stop.load(std::memory_order_relaxed)) {
-            agr_record& r = recs[n & 63];
-            if (!mint) { uint64_t a = splitmix(x), b = splitmix(x) | 1; memcpy(r.request_id, &a, 8); memcpy(r.request_id + 8, &b, 8); }
-            r.seq = n;
+            agr_record& r = *record_of((uint32_t)(n & 63));
             agr_verdict v; uint8_t id[1][16]; uint64_t first;
             const auto t0 = std::chrono::steady_clock::now();
-            if (agr_ingest_ex(h, &r, 1, &v, id, &first) < 0 || v.code != AGR_V_FORWARD) { bad++; break; }
+            if (var) {
+                const uint32_t off[2] = {0u, vlen[n & 63]};
+                if (agr_ingest_var(h, reinterpret_cast<const uint8_t*>(&r), off, 1, &v, id, &first) < 0 || v.code != AGR_V_FORWARD) { bad++; break; }
+            } else if (agr_ingest_ex(h, &r, 1, &v, id, &first) < 0 || v.code != AGR_V_FORWARD) { bad++; break; }
             agr_outcome o; memset(&o, 0, sizeof o);
             memcpy(o.request_id, id[0], 16); memcpy(o.agent_id, r.agent_id, AGR_AGENT_ID_BYTES);
             o.kind = AGR_OUT_RESPONSE; o.http_status = 200; o.seq = n + 1;
@@ -203,6 +238,7 @@ int main(int argc, char** argv) {
     std::sort(all.begin(), all.end());
     auto pct = [&](double p) { return all.empty() ? 0.0 : all[(size_t)std::min<double>(all.size() - 1, p * all.size())] / 1000.0; };
     agr_stats s2; agr_stats_get(h, &s2);
+    if (!var)
     printf("{\"threads\": %d, \"seconds\": %.3f, \"round_trips\": %.0f, \"round_trips_per_s\": %.1f, \"ops_per_s\": %.1f, "
            "\"p50_us\": %.2f, \"p99_us\": %.2f, \"latency_samples\": %zu, \"svc_batches\": %llu, \"ops_per_batch\": %.1f, "
            "\"id_mode\": \"%s\", \"agents\": %d, \"inflight_per_thread\": %d, \"response_bytes\": \"%s\", \"hdr_bytes\": %u, \"body_bytes\": %u, \"errors\": %llu, \"stored\": %llu, \"completions\": %llu, \"host_cpus\": %u}\n",
@@ -211,6 +247,13 @@ int main(int argc, char** argv) {
            mint ? "mint" : "hash", n_agents, inflight, bytes_mode == 0 ? "none" : bytes_mode == 1 ? "store" : bytes_mode == 2 ? "fused" : "large",
            bytes_mode ? seg_hlen : 0u, bytes_mode ? body_len : 0u, (unsigned long long)bad.load(), (unsigned long long)s2.stored, (unsigned long long)s2.completions,
            std::thread::hardware_concurrency());
+    if (var)
+        printf("{\"threads\": %d, \"seconds\": %.3f, \"round_trips_per_s\": %.1f, \"p50_us\": %.2f, \"p99_us\": %.2f, \"latency_samples\": %zu, "
+               "\"svc_batches\": %llu, \"arm\": \"%s\", \"id_mode\": \"%s\", \"inflight_per_thread\": %d, \"record_bytes_mean\": %.0f, "
+               "\"errors\": %llu}\n",
+               threads, secs, rt / secs, pct(0.50), pct(0.99), all.size(), (unsigned long long)(s1.svc_batches - s0.svc_batches),
+               inflight > 0 ? "ticket" : "locked", mint ? "mint" : "hash", inflight, (double)vbytes.load() / (64.0 * threads),
+               (unsigned long long)bad.load());
     agr_destroy(h);
     return bad.load() ? 1 : 0;
 }

@@ -101,7 +101,9 @@ typedef struct agr_record {
                                        published, and ONE resident service kernel decides the batch and writes verdicts / ids / result
                                        codes straight back into host memory — no launch, copy or stream sync per request.  Event
                                        order: batch by batch; inside a batch records in ring order, then outcomes in ring order (all
-                                       of them were in flight together).  Fixed-stride engines only (ignored with AGR_CFG_VARLEN). */
+                                       of them were in flight together).  With AGR_CFG_VARLEN the same front end serves
+                                       agr_submit_ingest of one variable-length record and agr_ingest_var of n <= 32 records in the
+                                       compact form (each record spread over consecutive ring slots, up to AGR_VAR_MAX_RECORD). */
 #define AGR_CFG_RING          0x40u /* the slab is a ring (with AGR_CFG_VARLEN the byte slab is a ring too): row ids keep counting arrivals, a
                                        record lives at row id mod slab_rows, and agr_reclaim hands the rows at the tail that no longer hold
                                        a record (agr_expire) back for reuse — a shard then runs indefinitely instead of filling up.
@@ -275,6 +277,11 @@ typedef struct agr_result {
                                   applied, but its completed / failed push did not fit the log, or its bytes found no room), AGR_ECUDA */
     uint32_t is_outcome;
 } agr_result;                  /* 40 B */
+/* agr_submit_ingest on an AGR_CFG_VARLEN engine: rec points to ONE variable-length record (the 96-byte header, then path |
+ * headers | body) and the call reads its stored length L = 96 + round16(path_len + hdr_len + body_len), capped at
+ * AGR_VAR_MAX_RECORD, from rec.  The ticket's result is that of agr_ingest_var of those L bytes as a one-record blob (a header
+ * whose lengths exceed AGR_VAR_MAX_RECORD - 96 is decided AGR_VF_BAD_LEN); AGR_ENOSPC when the rows or the record bytes found no
+ * room, AGR_EINVAL when the record alone exceeds half a ring's byte slab. */
 int agr_submit_ingest(agr_handle* h, const agr_record* rec, agr_ticket* ticket);
 int agr_submit_complete(agr_handle* h, const agr_outcome* outcome, agr_ticket* ticket);
 /* agr_submit_complete with the outcome's bytes in the ticket (agr_complete_ex(n = 1) semantics): headers then body for a
@@ -327,7 +334,10 @@ int agr_list(agr_handle* h, const char* agent_id, int which, uint8_t (*ids)[16],
 /* A variable-length record is the 96-byte header of agr_record (same fields, same offsets) followed by its payload
  * path | headers | body, zero padded to a multiple of 16 bytes; its stored length is 96 + round16(path_len + hdr_len +
  * body_len) <= AGR_VAR_MAX_RECORD.  A batch is one contiguous blob of such records plus offsets[0..n] (bytes from the
- * start of the blob, offsets[n] = blob length; every offset a multiple of 16).  Semantics are those of agr_ingest_ex. */
+ * start of the blob, offsets[n] = blob length; every offset a multiple of 16).  Semantics are those of agr_ingest_ex.
+ * With AGR_CFG_COMBINE, 1 <= n <= 32 and every record in the COMPACT form (offsets[i+1] - offsets[i] = the stored length its
+ * header gives), the call goes through the single-request ring like agr_ingest_ex(n <= 32) does, one record per ticket in
+ * call order (first_rid: the row of record 0); otherwise it is one locked batch. */
 #define AGR_VAR_MAX_RECORD 8192u
 int agr_ingest_var(agr_handle* h, const uint8_t* blob, const uint32_t* offsets, uint32_t n, agr_verdict* out,
                    uint8_t (*ids)[16], uint64_t* first_rid);
