@@ -285,8 +285,9 @@ class Engine:
     def __init__(self, *, device=-1, slab_rows=1 << 16, max_agents=1024, max_batch=0, flags=0, table_slots=0,
                  log_entries=0, k1_variant=0, id_secret=0, vslab_bytes=0, resp_bytes=0, restore_from=None):
         """restore_from: agr_restore of that snapshot instead of agr_create.  slab_rows, vslab_bytes and resp_bytes may differ
-        from the snapshot's (and AGR_CFG_RING may be added to an append-only one): the live window is then moved into the
-        new capacities on the device, and op_time(4) is that move's device time (DESIGN.md section 5)."""
+        from the snapshot's (and AGR_CFG_RING may be added to an append-only one; into a ring, AGR_CFG_VARLEN may differ too,
+        and the records are converted): the live window is then moved into the new capacities on the device, and op_time(4)
+        is that move's device time (DESIGN.md section 5)."""
         self.lib = load_library()
         cfg = AgrConfig(device, flags, slab_rows, table_slots, max_agents, max_batch or min(slab_rows, 1 << 20),
                         log_entries, id_secret, vslab_bytes, resp_bytes, k1_variant, 0)

@@ -264,9 +264,12 @@ void agr_launch_snap_blocks(const agr_snap_blocks& g, uint32_t n, bool gather, c
 // Relocation of a restore into other capacities (agr_relayout.cu).  Row ids [s.tail, s.tail + n) of the source engine s move
 // to row id mod t.ring_rows of the target t with every per-row word; the record bytes (AGR_CFG_VARLEN) and the response / error
 // bytes of the live rows (state != 0) are packed in row-id order from byte 0 of t's byte rings, each response and error
-// segment on a 16 B boundary.  count: per-tile sums, then their exclusive scan and the two totals (record bytes, response
-// bytes) at totals; rows: the words, the 512 B rows and the segment lists; bytes: one byte ring from its segment list
-// (destination offsets non-decreasing); log: one completed / failed log's physical rows.
+// segment on a 16 B boundary.  The record form is the target's (t.voff): a fixed-stride source's live rows go into a
+// variable-length target as their compact records, a variable-length source's records into a fixed-stride target as 512 B
+// rows padded with zeros.  count: per-tile sums, then their exclusive scan and the two totals (record bytes, response bytes)
+// at totals[0..1], and (variable-length into fixed-stride) the count of records longer than 512 B and the least
+// (k << 32 | vlen) of them at totals[2..3]; rows: the words, the 512 B rows and the segment lists; bytes: one byte ring from
+// its segment list (destination offsets non-decreasing); log: one completed / failed log's physical rows.
 struct agr_relayout_words {            // the per-row words of the stored responses, which agr_dev does not carry
     unsigned long long* resp_off; uint32_t* resp_len; uint32_t* resp_hlen;
     unsigned long long* err_off; uint32_t* err_len;
@@ -276,8 +279,8 @@ struct agr_relayout {
     agr_relayout_words sw, tw;
     unsigned long long n;
     unsigned long long* tile_sum;      // [2 * agr_relayout_tiles(n)]
-    unsigned long long* totals;        // [2]
-    unsigned long long *vseg_dst, *vseg_src; uint32_t* vseg_len;   // [n]: row k's record
+    unsigned long long* totals;        // [4]
+    unsigned long long *vseg_dst, *vseg_src; uint32_t* vseg_len;   // [n]: row k's record (either side variable-length)
     unsigned long long *rseg_dst, *rseg_src; uint32_t* rseg_len;   // [2n]: row k's response, then its error text
 };
 uint32_t agr_relayout_tiles(unsigned long long n);

@@ -1,6 +1,8 @@
 // agr_relayout.cu — the relocation of a restore into other capacities (agr_restore, DESIGN.md section 5): the live window
 // of a source engine moves to row id mod the target's slab_rows, and the record / response bytes of its live rows are
-// packed from byte 0 of the target's byte rings.  Everything here is bulk movement over HBM.
+// packed from byte 0 of the target's byte rings.  The target may hold records in the other form: 512 B rows become their
+// compact variable-length records, and variable-length records become 512 B rows padded with zeros.  Everything here is
+// bulk movement over HBM.
 #include "agr_device.cuh"
 
 #define RL_T 256u                       // threads per CTA of the row kernels
@@ -34,7 +36,17 @@ __device__ __forceinline__ void rl_block_scan(unsigned long long& a, unsigned lo
     __syncthreads();                    // (s_w is reused by the next call)
 }
 
-// what row k of the window takes in the target's byte rings: record bytes, and its 16 B-rounded response + error bytes
+// The compact length of a fixed-stride row's record, 96 + round16(path_len + hdr_len + body_len), from the lengths in its
+// header (one sector); capped at the row's 512 B, which K1 never stores a longer record in.
+__device__ __forceinline__ uint32_t rl_compact_len(const uint8_t* row) {
+    const uint32_t ph = __ldg(reinterpret_cast<const uint32_t*>(row + offsetof(agr_record, path_len)));   // path_len | hdr_len << 16
+    const uint32_t body = __ldg(reinterpret_cast<const uint32_t*>(row + offsetof(agr_record, body_len)));
+    const unsigned long long n = AGR_HEADER_BYTES + rl_r16((unsigned long long)(ph & 0xffffu) + (ph >> 16) + body);
+    return (uint32_t)(n < AGR_REC ? n : AGR_REC);
+}
+
+// What row k of the window takes: its record's length (the source's vlen, or with a fixed-stride source and a variable-length
+// target the compact length of its row; 0 for fixed-stride to fixed-stride), and its 16 B-rounded response + error bytes
 struct rl_row {
     uint32_t ps, st, vlen, rlen, elen;
 };
@@ -43,22 +55,29 @@ __device__ __forceinline__ rl_row rl_read(const agr_relayout& p, unsigned long l
     r.ps = row_physical(p.s, p.s.tail + k);
     r.st = p.s.state[r.ps];
     const bool live = r.st != 0u;
-    r.vlen = (p.s.voff && live) ? p.s.vlen[r.ps] : 0u;
+    r.vlen = !live ? 0u : p.s.voff ? p.s.vlen[r.ps] : p.t.voff ? rl_compact_len(p.s.slab + (size_t)r.ps * AGR_REC) : 0u;
     r.rlen = live ? p.sw.resp_len[r.ps] : 0u;
     r.elen = live ? p.sw.err_len[r.ps] : 0u;
     return r;
 }
 
-// per tile of RL_TILE rows: record bytes and response bytes of its live rows
+// per tile of RL_TILE rows: record bytes and response bytes of its live rows.  Into a fixed-stride target from a
+// variable-length source, also the records longer than a 512 B row: their count at totals[2], and the least (k << 32 | vlen)
+// at totals[3] (the caller sets them to 0 and ~0 first).
 __global__ void __launch_bounds__(RL_T) k_rl_count(const agr_relayout p) {
     unsigned long long a = 0, b = 0, ta, tb;
     const unsigned long long k0 = (unsigned long long)blockIdx.x * RL_TILE;
+    const bool to_rows = p.s.voff && !p.t.voff;
 #pragma unroll
     for (uint32_t j = 0; j < RL_PER; ++j) {
         const unsigned long long k = k0 + j * RL_T + threadIdx.x;
         if (k >= p.n) break;
         const rl_row r = rl_read(p, k);
         a += r.vlen; b += rl_r16(r.rlen) + rl_r16(r.elen);
+        if (to_rows && r.vlen > AGR_REC) {               // a refusal: the host reads the totals before anything moves
+            atomicAdd(p.totals + 2, 1ull);
+            atomicMin(p.totals + 3, k << 32 | r.vlen);
+        }
     }
     rl_block_scan(a, b, ta, tb);
     if (threadIdx.x == 0) { p.tile_sum[2 * blockIdx.x] = ta; p.tile_sum[2 * blockIdx.x + 1] = tb; }
@@ -78,8 +97,16 @@ __global__ void __launch_bounds__(RL_T) k_rl_scan(const agr_relayout p, const ui
 
 // Row move.  Thread t of tile T takes the RL_PER consecutive rows k = T * RL_TILE + t * RL_PER + j: their packed offsets are
 // the tile's prefix plus a block scan, written with every other per-row word to the target row (row id mod the target's
-// slab_rows), and the rows' byte segments go to the segment lists of the byte move.  Then (fixed-stride form) each warp copies
-// RL_TILE / 8 of the tile's 512 B rows, one 16 B vector per lane.
+// slab_rows), and the rows' byte segments go to the segment lists of the byte move (a variable-length target: from the
+// source's record bytes, or from its 512 B rows, cut to their compact length).  Then (fixed-stride target) each warp writes
+// RL_TILE / 8 of the tile's 512 B rows, one 16 B vector per lane: copied from the source's rows, or gathered from its record
+// bytes and zero past vlen.
+__device__ __forceinline__ uint4 rl_row16(const agr_relayout& p, unsigned long long k, uint32_t lane) {
+    const uint32_t ps = row_physical(p.s, p.s.tail + k);
+    if (!p.s.voff) return ldg_nc_v4(p.s.slab + (size_t)ps * AGR_REC + lane * 16u);
+    const uint32_t vl = p.s.state[ps] ? p.s.vlen[ps] : 0u;
+    return lane * 16u < vl ? ldg_nc_v4(p.s.slab + p.s.voff[ps] + lane * 16u) : make_uint4(0u, 0u, 0u, 0u);
+}
 __global__ void __launch_bounds__(RL_T) k_rl_rows(const agr_relayout p) {
     const unsigned long long k0 = (unsigned long long)blockIdx.x * RL_TILE + threadIdx.x * RL_PER;
     rl_row r[RL_PER];
@@ -104,11 +131,11 @@ __global__ void __launch_bounds__(RL_T) k_rl_rows(const agr_relayout p) {
         p.t.cksum[pt] = p.s.cksum[ps];
         p.t.ptime[pt] = p.s.ptime[ps];
         p.t.mtime[pt] = p.s.mtime[ps];
-        if (p.s.voff) {
-            const uint32_t vl = p.s.vlen[ps];
-            p.t.vlen[pt] = vl;
+        if (p.t.voff) {
+            p.t.vlen[pt] = p.s.voff ? p.s.vlen[ps] : r[j].vlen;
             p.t.voff[pt] = live ? a : 0ull;
-            p.vseg_dst[k] = a; p.vseg_src[k] = live ? p.s.voff[ps] : 0ull; p.vseg_len[k] = r[j].vlen;
+            p.vseg_dst[k] = a; p.vseg_src[k] = !live ? 0ull : p.s.voff ? p.s.voff[ps] : (unsigned long long)ps * AGR_REC;
+            p.vseg_len[k] = r[j].vlen;
             a += r[j].vlen;
         }
         const uint32_t rl = p.sw.resp_len[ps], el = p.sw.err_len[ps];
@@ -120,7 +147,7 @@ __global__ void __launch_bounds__(RL_T) k_rl_rows(const agr_relayout p) {
         p.rseg_dst[2 * k + 1] = eo; p.rseg_src[2 * k + 1] = r[j].elen ? p.sw.err_off[ps] : 0ull; p.rseg_len[2 * k + 1] = r[j].elen;
         b = eo + rl_r16(r[j].elen);
     }
-    if (p.s.voff) return;
+    if (p.t.voff) return;
     const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
     const unsigned long long w0 = (unsigned long long)blockIdx.x * RL_TILE + warp * (RL_TILE / 8u);
     for (uint32_t q = 0; q < RL_TILE / 8u; q += 4u) {
@@ -128,7 +155,7 @@ __global__ void __launch_bounds__(RL_T) k_rl_rows(const agr_relayout p) {
 #pragma unroll
         for (uint32_t u = 0; u < 4u; ++u) {                 // four rows' loads in flight per lane
             const unsigned long long k = w0 + q + u;
-            if (k < p.n) v[u] = ldg_nc_v4(p.s.slab + (size_t)row_physical(p.s, p.s.tail + k) * AGR_REC + lane * 16u);
+            if (k < p.n) v[u] = rl_row16(p, k, lane);
         }
 #pragma unroll
         for (uint32_t u = 0; u < 4u; ++u) {

@@ -611,9 +611,10 @@ static int restore_locked(agr_handle* h, FILE* f, const snap_header& full, const
 }
 
 // ---- restore into other capacities (DESIGN.md section 5)
-// Whether the restored state of the last cut s has to move: a ring snapshot into other ring capacities, or an append-only
-// snapshot into a ring.  Every other restore loads the file in place.
+// Whether the restored state of the last cut s has to move: a ring snapshot into other ring capacities, an append-only
+// snapshot into a ring, or either into a ring of the other record form.  Every other restore loads the file in place.
 static bool restore_relocates(const agr_handle* h, const snap_header& s) {
+    if ((s.flags ^ h->cfg.flags) & AGR_CFG_VARLEN) return true;     // (agr_restore lets the form differ only into a ring)
     if (!(s.flags & AGR_CFG_RING)) return is_ring(h);
     return s.slab_rows != h->cfg.slab_rows || s.resp_cap != h->resp_cap || ((s.flags & AGR_CFG_VARLEN) && s.vcap != h->vcap);
 }
@@ -621,9 +622,10 @@ static std::string relocation_enomem() {
     return "restore: relocating into other capacities holds the snapshot's engine and the configured one on the device at once, "
            "and both do not fit: " + g_err;
 }
-// Moves the state of the source engine s (the last cut hd, restored in s's own geometry) into h (a ring): the window's rows to
-// row id mod h's slab_rows, the live rows' record and response bytes packed from byte 0, the logs remapped.  The header fields
-// other than the byte rings' cursors stay as hd has them.
+// Moves the state of the source engine s (the last cut hd, restored in s's own geometry and record form) into h (a ring): the
+// window's rows to row id mod h's slab_rows, the live rows' record and response bytes packed from byte 0, the logs remapped.
+// The records take h's form: 512 B rows become compact records, records become 512 B rows (AGR_EINVAL for one longer than
+// that).  The header fields other than the byte rings' cursors stay as hd has them.
 static int relocate_locked(agr_handle* h, agr_handle* s, const snap_header& hd) {
     HLock lk(h);
     CK(cudaSetDevice(h->device));
@@ -635,7 +637,7 @@ static int relocate_locked(agr_handle* h, agr_handle* s, const snap_header& hd) 
         if ((uint32_t)slot != a) return fail(AGR_EINVAL, "restore: an agent appears twice in the agent table");
         if (removed) { h->agent_status[a] = AG_STATUS_REMOVED; TRY(push_agent_status(h, a, AG_STATUS_REMOVED)); }
     }
-    const bool var = (hd.flags & AGR_CFG_VARLEN) != 0;
+    const bool var_s = (hd.flags & AGR_CFG_VARLEN) != 0, var_t = (h->cfg.flags & AGR_CFG_VARLEN) != 0;
     const uint64_t n = hd.rows_used - hd.tail;
     h->rows_used = hd.rows_used; h->tail = hd.tail; h->released_total = hd.released_total; h->scan_lo = hd.scan_lo;
     h->expired_total = hd.expired_total; h->d.shard_id = hd.shard; h->d.id_gen = hd.gen;
@@ -648,27 +650,33 @@ static int relocate_locked(agr_handle* h, agr_handle* s, const snap_header& hd) 
         const size_t tiles = std::max<uint32_t>(agr_relayout_tiles(n), 1), rows = std::max<uint64_t>(n, 1);
         const int rc = [&]() {
             TRY(dev_alloc(s, &p.tile_sum, 2 * tiles, false));
-            TRY(dev_alloc(s, &p.totals, (size_t)2, false));
-            if (var) { TRY(dev_alloc(s, &p.vseg_dst, rows, false)); TRY(dev_alloc(s, &p.vseg_src, rows, false)); TRY(dev_alloc(s, &p.vseg_len, rows, false)); }
+            TRY(dev_alloc(s, &p.totals, (size_t)4, false));
+            if (var_s || var_t) { TRY(dev_alloc(s, &p.vseg_dst, rows, false)); TRY(dev_alloc(s, &p.vseg_src, rows, false)); TRY(dev_alloc(s, &p.vseg_len, rows, false)); }
             TRY(dev_alloc(s, &p.rseg_dst, 2 * rows, false)); TRY(dev_alloc(s, &p.rseg_src, 2 * rows, false)); TRY(dev_alloc(s, &p.rseg_len, 2 * rows, false));
             return 0;
         }();
         if (rc == AGR_ENOMEM) return fail(rc, relocation_enomem());
         TRY(rc);
     }
+    CK(cudaMemsetAsync(p.totals + 2, 0, 8, h->stream));        // k_rl_count's oversized records: none yet, least ~0
+    CK(cudaMemsetAsync(p.totals + 3, 0xff, 8, h->stream));
     TRY(op_time_begin(h, 4));
     agr_launch_relayout_count(p, h->stream);
     CK(cudaGetLastError());
-    unsigned long long tot[2];
+    unsigned long long tot[4];
     TRY(d2h_staged(h, tot, p.totals, sizeof tot, h->h_small));
-    if (var && tot[0] > h->vcap)
+    if (var_s && !var_t && tot[2])
+        return fail(AGR_EINVAL, "restore: " + std::to_string(tot[2]) + " live records are longer than the 512 B rows of the fixed "
+                                "record form, so they cannot be converted (the first: row " + std::to_string(hd.tail + (tot[3] >> 32)) +
+                                    ", " + std::to_string(tot[3] & 0xffffffffull) + " B)");
+    if (var_t && tot[0] > h->vcap)
         return fail(AGR_ENOSPC, "restore: the live records take " + std::to_string(tot[0]) + " B, more than vslab_bytes (" +
                                     std::to_string(h->vcap) + " B) by " + std::to_string(tot[0] - h->vcap) + " B");
     if (tot[1] > h->resp_cap)
         return fail(AGR_ENOSPC, "restore: the live response and error bytes take " + std::to_string(tot[1]) + " B, more than resp_bytes (" +
                                     std::to_string(h->resp_cap) + " B) by " + std::to_string(tot[1] - h->resp_cap) + " B");
     agr_launch_relayout_rows(p, h->stream);
-    if (var) agr_launch_relayout_bytes(s->d.slab, h->d.slab, p.vseg_dst, p.vseg_src, p.vseg_len, n, tot[0], h->stream);
+    if (var_t) agr_launch_relayout_bytes(s->d.slab, h->d.slab, p.vseg_dst, p.vseg_src, p.vseg_len, n, tot[0], h->stream);
     agr_launch_relayout_bytes(s->d_resp, h->d_resp, p.rseg_dst, p.rseg_src, p.rseg_len, 2 * n, tot[1], h->stream);
     agr_launch_relayout_log(s->d, h->d, s->d.completed_log, h->d.completed_log, hd.log_len[0], h->stream);
     agr_launch_relayout_log(s->d, h->d, s->d.failed_log, h->d.failed_log, hd.log_len[1], h->stream);
@@ -676,7 +684,7 @@ static int relocate_locked(agr_handle* h, agr_handle* s, const snap_header& hd) 
     TRY(op_time_end(h, 4));
     const unsigned long long lens[2] = {hd.log_len[0], hd.log_len[1]};
     CK(cudaMemcpyAsync(h->d.log_len, lens, sizeof lens, cudaMemcpyHostToDevice, h->stream));
-    h->vused = var ? tot[0] : 0; h->vtail = 0;
+    h->vused = var_t ? tot[0] : 0; h->vtail = 0;
     h->resp_used = tot[1]; h->resp_tail = 0;
     h->d.idx_base = h->tail;
     TRY(chunk_bounds_unknown(h));
@@ -685,7 +693,7 @@ static int relocate_locked(agr_handle* h, agr_handle* s, const snap_header& hd) 
     return 0;
 }
 // The relocating restore into h: the file (f, past its header) and its deltas go into a source engine of the snapshot's own
-// geometry, which is then moved into h and freed.  The source engine is bare: no single-request front end, no snapshot shadows,
+// geometry and record form, which is then moved into h and freed.  The source engine is bare: no single-request front end, no snapshot shadows,
 // no dedupe index (created in minted-id form, so that it allocates none; nothing of the id mode is in the arrays it holds).
 static int restore_relocate(agr_handle* h, FILE* f, const snap_header& full, const std::vector<std::string>& files, const std::vector<delta_header>& dh) {
     const snap_header& last = dh.empty() ? full : dh.back().cut;
@@ -734,7 +742,8 @@ int agr_restore(const agr_config* cfg, const char* path, agr_handle** out) {
     agr_config c = *cfg;
     if (c.flags == 0) c.flags = AGR_CFG_PERSISTENCE;
     const uint32_t mode_bits = AGR_CFG_MINT_IDS | AGR_CFG_VARLEN | AGR_CFG_RING;
-    const uint32_t form = (hd.flags & AGR_CFG_RING) ? mode_bits : mode_bits & ~AGR_CFG_RING;   // (append-only into a ring relocates)
+    uint32_t form = (hd.flags & AGR_CFG_RING) ? mode_bits : mode_bits & ~AGR_CFG_RING;   // (append-only into a ring relocates)
+    if (c.flags & AGR_CFG_RING) form &= ~AGR_CFG_VARLEN;                                  // (into a ring of the other form converts)
     if ((c.flags & form) != (hd.flags & form)) { fclose(f); return fail(AGR_EINVAL, "restore: id mode / record form differ from the snapshot"); }
     if (c.id_secret == 0) c.id_secret = hd.id_secret;
     if (c.id_secret != hd.id_secret) { fclose(f); return fail(AGR_EINVAL, "restore: id_secret differs from the snapshot"); }

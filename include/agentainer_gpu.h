@@ -444,15 +444,23 @@ int agr_json_decode(const uint8_t* json, uint32_t len, uint8_t* record, uint32_t
  * relocating restore (below), which starts a new chain: its next agr_snapshot is a full file, and deltas follow on that file.
  * Other capacities: agr_restore RELOCATES the restored state instead of loading it in place when the snapshot (the full file,
  * or the last cut of a chain) is a ring and cfg's slab_rows, resp_bytes or (AGR_CFG_VARLEN) vslab_bytes differ from its own,
- * or when the snapshot is append-only and cfg has AGR_CFG_RING.  Every other restore loads in place as before.  The id mode,
- * record form and id_secret must still match, and a ring snapshot does not go into an append-only engine (AGR_EINVAL).  The
+ * or when the snapshot is append-only and cfg has AGR_CFG_RING.  Every other restore loads in place as before.  The id mode
+ * and id_secret must still match, and a ring snapshot does not go into an append-only engine (AGR_EINVAL).  The
  * live window [rows_tail, rows_used) keeps its row ids (minted ids keep resolving, ids outside it keep missing) and moves to
  * row id mod the new slab_rows; the record bytes and the response / error bytes of the rows that hold one are packed from
  * the start of the new byte rings; the completed / failed logs follow their rows (layout: DESIGN.md section 5).
  * AGR_ENOSPC, with agr_last_error naming what did not fit and by how much, when the window is longer than slab_rows or the
  * live record / response bytes exceed vslab_bytes / resp_bytes.  While it runs, the snapshot's state is held on the device
  * in an engine of its own geometry next to the new one (freed before agr_restore returns): peak HBM is both engines, and
- * AGR_ENOMEM (naming the relocation) when both do not fit. */
+ * AGR_ENOMEM (naming the relocation) when both do not fit.
+ * Other record form: when cfg has AGR_CFG_RING and differs from the snapshot (a ring file, an append-only file or the last cut
+ * of a chain) in AGR_CFG_VARLEN, agr_restore relocates as above and CONVERTS the records; capacities may change too.  Fixed
+ * to variable-length: each live row becomes its compact record, the row's first 96 + round16(path_len + hdr_len + body_len)
+ * bytes, packed in row-id order from byte 0 (AGR_ENOSPC naming vslab_bytes when they do not fit).  Variable-length to fixed:
+ * each live record becomes a 512-byte row, its bytes then zeros; AGR_EINVAL, naming how many and the first row id with its
+ * length, when a live record is longer than 512 bytes.  Checksums move unchanged: a fixed row with non-zero bytes past its
+ * compact length (the layout requires zeros) is counted by agr_verify after the conversion.  An append-only target keeps
+ * the snapshot's form (AGR_EINVAL otherwise). */
 int agr_snapshot(agr_handle* h, const char* path);
 int agr_restore(const agr_config* cfg, const char* path, agr_handle** out);
 /* The 24 h TTL of the record keys (SET ... EX 24h at requests.go:106,175,270; every SET restarts it, Q11).  Times are the
