@@ -180,7 +180,9 @@ AGR_HD bool agr_unmint_in_window(unsigned long long lo, unsigned long long hi, u
 }
 
 // ---- record checksum: c0 = sum w_k, c1 = sum (k+1) w_k over the 128 little-endian u32 words, mod 2^32
-// (Fletcher-style; detects any single-word change and any swap of two unequal words).
+// (Fletcher-style).  It detects every single-word change (c0 moves by the change).  A swap of words a and b at distance d
+// leaves c0 alone and moves c1 by d (b - a): it is missed exactly when d (b - a) = 0 mod 2^32, e.g. 0 and 0x80000000 two
+// words apart; so is bit 31 flipped in two words an even distance apart.
 AGR_HD unsigned long long agr_cksum_pack(uint32_t c0, uint32_t c1) {
     return ((unsigned long long)c1 << 32) | c0;
 }

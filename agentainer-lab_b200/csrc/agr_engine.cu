@@ -1581,19 +1581,39 @@ int agr_reclaim_async(agr_handle* h, uint64_t* released) {
     return 0;
 }
 
+// The sweep covers the physical rows [0, rows_span) except those of reservations that agr_ingest_rows has not decided yet:
+// such a row may hold bytes (agr_fill_rows) but no checksum until K1 takes one.  One launch per range between them.
 int agr_verify(agr_handle* h, uint64_t* rows_checked, uint64_t* bad) {
     if (!h || !bad) return fail(AGR_EINVAL, "NULL argument");
     HLock lk(h);
     CK(cudaSetDevice(h->device));
     CK(cudaMemsetAsync(count_slot(h), 0, 8, h->stream));
     sync_window(h);
-    agr_launch_verify(h->d, rows_span(h), count_slot(h), h->stream);
-    h->k3_launches += 1;
+    const uint64_t span = rows_span(h);
+    std::vector<std::pair<uint64_t, uint64_t>> skip;          // physical [first, end) of the undecided rows, a ring's split where it wraps
+    for (const auto& r : h->resv) {
+        const uint64_t p = phys_row(h, r.first), n = r.end - r.first;
+        const uint64_t n0 = is_ring(h) ? std::min<uint64_t>(n, h->cfg.slab_rows - p) : n;
+        skip.emplace_back(p, p + n0);
+        if (n > n0) skip.emplace_back(0, n - n0);
+    }
+    std::sort(skip.begin(), skip.end());
+    uint64_t at = 0, checked = 0;
+    skip.emplace_back(span, span);
+    for (const auto& s : skip) {
+        const uint64_t end = std::min(s.first, span);
+        if (end > at) {
+            agr_launch_verify(h->d, at, end - at, count_slot(h), h->stream);
+            h->k3_launches += 1;
+            checked += end - at;
+        }
+        at = std::max(at, std::min(s.second, span));
+    }
     CK(cudaGetLastError());
     unsigned long long v = 0;
     TRY(read_count(h, &v));
     *bad = v;
-    if (rows_checked) *rows_checked = rows_span(h);
+    if (rows_checked) *rows_checked = checked;
     return 0;
 }
 

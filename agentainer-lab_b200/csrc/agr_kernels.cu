@@ -107,12 +107,14 @@ __global__ void __launch_bounds__(256) k1_index(const agr_dev d, const uint32_t 
     }
 }
 
-// integrity sweep: warp per row, recompute the position-weighted checksum of the stored bytes and compare
-__global__ void __launch_bounds__(256) k_verify(const agr_dev d, const unsigned long long rows, unsigned long long* __restrict__ bad) {
+// integrity sweep over physical rows [first, first + rows): warp per row, recompute the position-weighted checksum of the
+// stored bytes and compare
+__global__ void __launch_bounds__(256) k_verify(const agr_dev d, const unsigned long long first, const unsigned long long rows,
+                                                unsigned long long* __restrict__ bad) {
     const unsigned long long w = ((unsigned long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int lane = threadIdx.x & 31;
     if (w >= rows) return;
-    const uint32_t rid = (uint32_t)w;
+    const uint32_t rid = (uint32_t)(first + w);
     if (d.ring_rows && !(d.state[rid] & ST_STORED)) return;    // ring: released / skipped rows hold no record
     const uint8_t* src = rec_ptr(d, rid);
     const uint32_t chunks = d.voff ? (d.vlen[rid] >> 4) : 32u;
@@ -359,8 +361,8 @@ void agr_launch_log_compact(const agr_dev& d, const uint32_t* log, unsigned long
     k_log_scatter<<<nch, 32, 0, st>>>(d, log, len, released, chunk_cnt, out);
 }
 
-void agr_launch_verify(const agr_dev& d, unsigned long long rows, unsigned long long* bad, cudaStream_t st) {
-    if (rows) k_verify<<<(unsigned)((rows * 32 + 255) / 256), 256, 0, st>>>(d, rows, bad);
+void agr_launch_verify(const agr_dev& d, unsigned long long first, unsigned long long rows, unsigned long long* bad, cudaStream_t st) {
+    if (rows) k_verify<<<(unsigned)((rows * 32 + 255) / 256), 256, 0, st>>>(d, first, rows, bad);
 }
 // hash-id ring: rebuild of the dedupe index over a range of physical rows — only rows that still hold a record go in (a release,
 // a restore: ring_reindex_locked)

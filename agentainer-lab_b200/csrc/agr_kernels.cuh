@@ -196,7 +196,8 @@ void agr_launch_bytes_span(const agr_dev& d, unsigned long long head, unsigned l
 void agr_launch_log_compact(const agr_dev& d, const uint32_t* log, unsigned long long len, uint32_t released, uint32_t* out,
                             uint32_t* chunk_cnt /* [chunks + 1] */, unsigned long long* new_len /* device: receives the kept count */,
                             cudaStream_t st);
-void agr_launch_verify(const agr_dev& d, unsigned long long rows, unsigned long long* bad, cudaStream_t st);
+// physical rows [first, first + rows)
+void agr_launch_verify(const agr_dev& d, unsigned long long first, unsigned long long rows, unsigned long long* bad, cudaStream_t st);
 void agr_launch_reindex(const agr_dev& d, uint32_t rows, cudaStream_t st);
 void agr_launch_reindex_range(const agr_dev& d, uint32_t first, uint32_t n, cudaStream_t st);
 void agr_launch_k1_post(const agr_dev& d, uint32_t first_rid, uint32_t n, int sm_count, cudaStream_t st, void* verdicts, void* ids,

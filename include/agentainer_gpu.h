@@ -483,7 +483,12 @@ int agr_reclaim(agr_handle* h, uint64_t* released);
  * release lags one step, nothing waits for the GPU. */
 int agr_reclaim_async(agr_handle* h, uint64_t* released);
 /* Integrity sweep: recomputes the checksum of every stored record on the device and compares it with the one K1 took at
- * ingest.  *bad = number of rows that differ (0 on a healthy slab). */
+ * ingest.  It sweeps the physical rows that have ever been handed out (rows_used, or at most slab_rows on a ring) except the
+ * rows of reservations that agr_ingest_rows has not decided yet, which hold no checksum.  *rows_checked (nullable) = the rows
+ * in that sweep.  Append-only engines compare every one of them (a row K1 did not store still holds its bytes and their
+ * checksum); a ring compares only the rows that hold a stored record, not released, skipped or expired ones.  A
+ * variable-length row covers its stored bytes (none, and a checksum of 0, when it has none).  *bad = number of rows that
+ * differ (0 on a healthy slab). */
 int agr_verify(agr_handle* h, uint64_t* rows_checked, uint64_t* bad);
 
 /* ------------------------------------------------------------------- stats */
