@@ -398,8 +398,9 @@ class Engine:
 
     def debug_read(self, which: str, first_rid: int, n: int) -> np.ndarray:
         """Per-row words of logical rows [first_rid, +n); "cmin": the TTL sweep's time bounds of physical chunks [first_rid, +n)."""
-        sel = {"state": 0, "route": 1, "aux": 2, "cksum": 3, "verdict": 4, "mtime": 5, "cmin": 6, "index_used": 7}[which]
-        out = np.zeros(n, dtype=verdict_dtype if sel == 4 else np.uint64 if sel in (3, 5, 6, 7) else np.uint32)
+        sel = {"state": 0, "route": 1, "aux": 2, "cksum": 3, "verdict": 4, "mtime": 5, "cmin": 6, "index_used": 7, "voff": 8, "vlen": 9,
+               "resp_off": 10, "resp_len": 11, "err_off": 12, "err_len": 13}[which]
+        out = np.zeros(n, dtype=verdict_dtype if sel == 4 else np.uint64 if sel in (3, 5, 6, 7, 8, 10, 12) else np.uint32)
         _check(self.lib, self.lib.agr_debug_read(self.h, sel, first_rid, n, _ptr(out)))
         return out
 

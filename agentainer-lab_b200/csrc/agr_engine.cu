@@ -1675,8 +1675,15 @@ int agr_debug_read(agr_handle* h, int which, uint64_t first_rid, uint32_t n, voi
         case AGR_DBG_AUX: base = (const uint8_t*)h->d.aux; break;
         case AGR_DBG_CKSUM: base = (const uint8_t*)h->d.cksum; w = 8; break;
         case AGR_DBG_MTIME: base = (const uint8_t*)h->d.mtime; w = 8; break;
+        case AGR_DBG_VOFF: base = (const uint8_t*)h->d.voff; w = 8; break;
+        case AGR_DBG_VLEN: base = (const uint8_t*)h->d.vlen; break;
+        case AGR_DBG_RESP_OFF: base = (const uint8_t*)h->d_resp_off; w = 8; break;
+        case AGR_DBG_RESP_LEN: base = (const uint8_t*)h->d_resp_len; break;
+        case AGR_DBG_ERR_OFF: base = (const uint8_t*)h->d_err_off; w = 8; break;
+        case AGR_DBG_ERR_LEN: base = (const uint8_t*)h->d_err_len; break;
         default: return fail(AGR_EINVAL, "bad array selector");
     }
+    if (!base) return fail(AGR_EINVAL, "engine was not created with AGR_CFG_VARLEN");
     const uint64_t p0 = phys_row(h, first_rid);
     const uint64_t n0 = is_ring(h) ? std::min<uint64_t>(n, h->cfg.slab_rows - p0) : n;          // a logical range may wrap once
     if (n0) CK(cudaMemcpyAsync(dst, base + p0 * w, (size_t)n0 * w, cudaMemcpyDeviceToHost, h->stream));

@@ -588,9 +588,13 @@ int agr_complete_sharded(agr_handle* h, const agr_outcome* outs, uint32_t n, int
  * last-SET time K2 wrote, or — rings — K1; 0 = the TTL sweep takes the record's created_at).  6 cmin (u64) is per physical
  * 4096-row chunk instead: first_rid is a chunk index and first_rid + n <= slab_rows / 4096 + 1; the value is a lower bound of
  * the last-SET times of the chunk's stored rows (0 = unknown, ~0 = no stored row).  7 index used (u64, first_rid 0, n 1): how many
- * slots of the dedupe index hold an id (hash-id mode).  out must hold n elements of that width. */
+ * slots of the dedupe index hold an id (hash-id mode).  Where the row's bytes lie, as physical byte offsets: 8 voff (u64) and
+ * 9 vlen (u32) of the record in the byte slab (AGR_CFG_VARLEN only, AGR_EINVAL otherwise), 10 resp_off (u64) and 11 resp_len
+ * (u32) of the stored response and 12 err_off (u64) and 13 err_len (u32) of the stored error text in the response byte slab
+ * (the offset is meaningless when the length is 0).  out must hold n elements of that width. */
 enum { AGR_DBG_STATE = 0, AGR_DBG_ROUTE = 1, AGR_DBG_AUX = 2, AGR_DBG_CKSUM = 3, AGR_DBG_VERDICT = 4, AGR_DBG_MTIME = 5,
-       AGR_DBG_CMIN = 6, AGR_DBG_INDEX_USED = 7 };
+       AGR_DBG_CMIN = 6, AGR_DBG_INDEX_USED = 7, AGR_DBG_VOFF = 8, AGR_DBG_VLEN = 9, AGR_DBG_RESP_OFF = 10, AGR_DBG_RESP_LEN = 11,
+       AGR_DBG_ERR_OFF = 12, AGR_DBG_ERR_LEN = 13 };
 int agr_debug_read(agr_handle* h, int which, uint64_t first_rid, uint32_t n, void* out);
 /* TEST ONLY: puts an AGR_CFG_RING engine far along its arrival counter without ingesting.  The window must be empty (every row
  * released: rows_tail == rows_used, no reserved row unfilled, empty completed / failed logs — what agr_expire + agr_reclaim leave
