@@ -31,7 +31,7 @@ class AgrConfig(C.Structure):
     _fields_ = [("device", C.c_int32), ("flags", C.c_uint32), ("slab_rows", C.c_uint64), ("table_slots", C.c_uint64),
                 ("max_agents", C.c_uint32), ("max_batch", C.c_uint32), ("log_entries", C.c_uint64),
                 ("id_secret", C.c_uint64), ("vslab_bytes", C.c_uint64), ("resp_bytes", C.c_uint64),
-                ("k1_variant", C.c_uint32), ("reserved", C.c_uint32)]
+                ("k1_variant", C.c_uint32), ("max_record_bytes", C.c_uint32)]
 
 
 class AgrStats(C.Structure):
@@ -244,12 +244,13 @@ def comm_unique_id() -> bytes:
     return bytes(buf)
 
 
-def var_record_len(rec: np.ndarray) -> int:
+def var_record_len(rec: np.ndarray, cap: int = K.AGR_VAR_MAX_RECORD) -> int:
     """Stored length of the variable-length record whose 96-byte header starts rec (uint8): 96 + its payload rounded up to 16
-    bytes, capped at AGR_VAR_MAX_RECORD (include/agentainer_gpu.h)."""
+    bytes, capped at cap (AGR_VAR_MAX_RECORD: the single-request ring's rule, include/agentainer_gpu.h; an engine's
+    max_record_bytes: the longest record agr_ingest_var stores whole)."""
     h = np.frombuffer(np.ascontiguousarray(rec[: K.AGR_HEADER_BYTES]).tobytes(), dtype=header_dtype)[0]
     p = int(h["path_len"]) + int(h["hdr_len"]) + int(h["body_len"])
-    return min(K.AGR_VAR_MAX_RECORD, K.AGR_HEADER_BYTES + (p + 15) // 16 * 16)
+    return min(cap, K.AGR_HEADER_BYTES + (p + 15) // 16 * 16)
 
 
 def agent_hash(agent_id: str) -> int:
@@ -283,14 +284,15 @@ class Engine:
     """One shard (one GPU) of the request engine.  Thin wrapper: every method is one C-ABI call."""
 
     def __init__(self, *, device=-1, slab_rows=1 << 16, max_agents=1024, max_batch=0, flags=0, table_slots=0,
-                 log_entries=0, k1_variant=0, id_secret=0, vslab_bytes=0, resp_bytes=0, restore_from=None):
+                 log_entries=0, k1_variant=0, id_secret=0, vslab_bytes=0, resp_bytes=0, max_record_bytes=0, restore_from=None):
         """restore_from: agr_restore of that snapshot instead of agr_create.  slab_rows, vslab_bytes and resp_bytes may differ
         from the snapshot's (and AGR_CFG_RING may be added to an append-only one; into a ring, AGR_CFG_VARLEN may differ too,
         and the records are converted): the live window is then moved into the new capacities on the device, and op_time(4)
-        is that move's device time (DESIGN.md section 5)."""
+        is that move's device time (DESIGN.md section 5).  max_record_bytes (AGR_CFG_VARLEN): the longest record ingest_var
+        accepts, 0 = AGR_VAR_MAX_RECORD; a restore takes it from here, not from the file."""
         self.lib = load_library()
         cfg = AgrConfig(device, flags, slab_rows, table_slots, max_agents, max_batch or min(slab_rows, 1 << 20),
-                        log_entries, id_secret, vslab_bytes, resp_bytes, k1_variant, 0)
+                        log_entries, id_secret, vslab_bytes, resp_bytes, k1_variant, max_record_bytes)
         self.mint = bool(flags & K.AGR_CFG_MINT_IDS)
         self.varlen = bool(flags & K.AGR_CFG_VARLEN)
         h = C.c_void_p()
@@ -479,13 +481,14 @@ class Engine:
             return disp[: n.value], blob[: nb.value], offs[: n.value + 1]
 
     def get_record_var(self, agent_id: str, request_id: bytes) -> Optional[np.ndarray]:
-        out = np.zeros(8192, dtype=np.uint8)
         rid = (C.c_uint8 * 16).from_buffer_copy(request_id)
         ln = C.c_uint32()
-        rc = self.lib.agr_get_record_var(self.h, agent_id.encode(), C.cast(rid, C.c_void_p), _ptr(out), 8192, C.byref(ln))
+        rc = self.lib.agr_get_record_var(self.h, agent_id.encode(), C.cast(rid, C.c_void_p), None, 0, C.byref(ln))
         if rc == K.AGR_ENOTFOUND:
             return None
         _check(self.lib, rc)
+        out = np.zeros(max(1, ln.value), dtype=np.uint8)
+        _check(self.lib, self.lib.agr_get_record_var(self.h, agent_id.encode(), C.cast(rid, C.c_void_p), _ptr(out), out.size, C.byref(ln)))
         return out[: ln.value]
 
     # ---- K4 (multi-GPU exchange)

@@ -178,6 +178,15 @@ static int create_impl(const agr_config* cfg_in, agr_handle* h) {
     if (c.log_entries == 0) c.log_entries = c.slab_rows * 3;   // a replayed request pushes twice (Q7), plus once per earlier retry
     if (c.k1_variant & ~(0x20u | 0xff0000u))
         return fail(AGR_EINVAL, "k1_variant: only bit 0x20 (K1v form) and bits 16..23 (timing stride) are defined; the A/B alternates of the fixed-stride K1 were retired");
+    if ((c.flags & AGR_CFG_VARLEN) && c.vslab_bytes == 0) c.vslab_bytes = 1024ull * c.slab_rows;
+    if (c.max_record_bytes != 0) {
+        if (!(c.flags & AGR_CFG_VARLEN)) return fail(AGR_EINVAL, "max_record_bytes needs AGR_CFG_VARLEN (fixed-stride records are 512 B)");
+        if ((c.max_record_bytes & 15u) || c.max_record_bytes < AGR_VAR_MAX_RECORD || c.max_record_bytes > AGR_VAR_MAX_RECORD_LIMIT)
+            return fail(AGR_EINVAL, "max_record_bytes must be a multiple of 16 in [8192, 2^26], or 0 for 8192");
+        if (c.max_record_bytes > c.vslab_bytes / 2)
+            return fail(AGR_EINVAL, "max_record_bytes must be at most vslab_bytes / 2 (" + std::to_string(c.vslab_bytes / 2) + "): a batch never takes more than half the byte slab");
+    }
+    if (c.max_record_bytes == 0) c.max_record_bytes = AGR_VAR_MAX_RECORD;
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return fail(AGR_ENODEV, "no CUDA device visible (this library has no CPU fallback)"); }
     int dev = c.device;
@@ -197,15 +206,15 @@ static int create_impl(const agr_config* cfg_in, agr_handle* h) {
     agr_dev& d = h->d;
     const bool varlen = (c.flags & AGR_CFG_VARLEN) != 0;
     if (varlen) {
-        if (c.vslab_bytes == 0) c.vslab_bytes = 1024ull * c.slab_rows;
-        h->cfg = c;
         h->vcap = c.vslab_bytes;
         TRY(dev_alloc(h, &d.slab, (size_t)c.vslab_bytes + AGR_VT_MAXREC, false));
         TRY(dev_alloc(h, &d.voff, c.slab_rows, true));
         TRY(dev_alloc(h, &d.vlen, c.slab_rows, true));
         TRY(dev_alloc(h, &h->d_voffsets, (size_t)c.max_batch + 1, false));
         TRY(host_alloc(h, &h->h_voffsets, (size_t)c.max_batch + 1));
-        TRY(dev_alloc(h, &h->d_tile_first, (size_t)(((size_t)c.max_batch * AGR_VT_MAXREC) / AGR_VT_TILE + 8), false));
+        // (a blob holds at most max_batch records and, with long records, at most vslab_bytes)
+        const size_t tile_bytes = (size_t)c.max_batch * AGR_VT_MAXREC + (c.max_record_bytes > AGR_VAR_MAX_RECORD ? c.vslab_bytes : 0);
+        TRY(dev_alloc(h, &h->d_tile_first, tile_bytes / AGR_VT_TILE + 8, false));
         // runs of 512-byte slots: up to 2 x max_batch (the exchange decides own + received rows), offsets below 2^32
         h->slot_off_max = (uint32_t)std::min<uint64_t>(2ull * c.max_batch, (0xffffffffull / AGR_REC) - 1);
         TRY(dev_alloc(h, &h->d_slot_off, (size_t)h->slot_off_max + 1, false));
@@ -706,17 +715,28 @@ int launch_k1_locked(agr_handle* h, uint64_t first, uint32_t n, agr_verdict* d_o
 
 // K1v and its post pass over rows [first, first + n) of a variable-length engine, whose records lie at physical byte `base` of
 // the byte slab, record i at d_off[i] .. d_off[i + 1] from there (`bytes` in all)
+// (nlong: the batch's long records, listed in h->long_list as agr_launch_k1v_long takes it)
 static int launch_k1v_locked(agr_handle* h, uint64_t first, uint32_t n, uint64_t base, const uint32_t* d_off, uint64_t bytes,
-                             agr_verdict* d_out, uint8_t* d_ids) {
+                             agr_verdict* d_out, uint8_t* d_ids, uint32_t nlong = 0) {
     cudaStream_t st = h->stream;
     sync_window(h);
     flip_batch_words(h);
+    const size_t words = 2 * (size_t)nlong + 1;                   // long records: the list, then two sums per record
+    if (nlong) {
+        if (words + 2 * (size_t)nlong > h->d_long.cap) TRY(regrow(h, h->d_long, std::max<size_t>(words + 2 * (size_t)nlong, 1024)));
+        CK(cudaMemcpyAsync(h->d_long.p, h->long_list.data(), words * 4, cudaMemcpyHostToDevice, st));
+    }
     cudaEvent_t e0 = nullptr, e1 = nullptr;
     if (h->cfg.flags & AGR_CFG_TIMING) {
         TRY(claim_k1_events(h, &e0, &e1));
         CK(cudaEventRecord(e0, st));
     }
     CK(agr_launch_k1_var(h->d, h->d.slab + base, d_off, n, bytes, h->d_tile_first, (uint32_t)phys_row(h, first), base, h->sm_count, st, h->cfg.k1_variant));
+    if (nlong) {
+        CK(agr_launch_k1v_long(h->d, h->d.slab + base, d_off, h->d_long.p, nlong, h->long_list[2 * nlong], h->d_long.p + words,
+                               (uint32_t)phys_row(h, first), st));
+        h->k1_launches += 2;
+    }
     if (e1) CK(cudaEventRecord(e1, st));
     agr_launch_k1_post(h->d, (uint32_t)phys_row(h, first), n, h->sm_count, st, d_out, d_ids);
     h->k1_launches += 3;
@@ -1213,10 +1233,23 @@ int agr_ingest_var(agr_handle* h, const uint8_t* blob, const uint32_t* offsets, 
     if (n == 0) { if (first_rid) *first_rid = h->rows_used; return 0; }
     const uint64_t bytes = offsets[n];
     if (offsets[0] != 0) return fail(AGR_EINVAL, "offsets[0] must be 0");
+    const uint32_t maxrec = h->cfg.max_record_bytes;
+    h->long_list.clear();
     for (uint32_t i = 0; i < n; ++i) {                           // host-side shape check (lengths are part of the wire format)
         const uint32_t len = offsets[i + 1] - offsets[i];
-        if (offsets[i + 1] < offsets[i] || (len & 15u) || len < AGR_HEADER_BYTES || len > AGR_VAR_MAX_RECORD)
-            return fail(AGR_EINVAL, "record " + std::to_string(i) + ": length must be a multiple of 16 in [96, 8192]");
+        if (offsets[i + 1] < offsets[i] || (len & 15u) || len < AGR_HEADER_BYTES || len > maxrec)
+            return fail(AGR_EINVAL, "record " + std::to_string(i) + ": length must be a multiple of 16 in [96, " + std::to_string(maxrec) + "]");
+        if (len > AGR_VAR_MAX_RECORD) h->long_list.push_back(i);
+    }
+    const uint32_t nlong = (uint32_t)h->long_list.size();
+    if (nlong) {                                                 // then each long record's first 8 KiB piece, and the total
+        uint32_t pieces = 0;
+        for (uint32_t k = 0; k < nlong; ++k) {
+            const uint32_t i = h->long_list[k];
+            h->long_list.push_back(pieces);
+            pieces += (offsets[i + 1] - offsets[i] + AGR_VT_TILE - 1) / AGR_VT_TILE;
+        }
+        h->long_list.push_back(pieces);
     }
     uint64_t vpad = 0;
     TRY(vbytes_fit(h, bytes, &vpad));                             // (byte ring: a blob never wraps either)
@@ -1226,7 +1259,7 @@ int agr_ingest_var(agr_handle* h, const uint8_t* blob, const uint32_t* offsets, 
     cudaStream_t st = h->stream;
     CK(cudaMemcpyAsync(h->d.slab + base, blob, bytes, cudaMemcpyHostToDevice, st));
     TRY(h2d_staged(h, h->d_voffsets, offsets, ((size_t)n + 1) * 4, h->h_voffsets));
-    TRY(launch_k1v_locked(h, first, n, base, h->d_voffsets, bytes, out ? h->d_verdicts : nullptr, ids ? h->d_ids : nullptr));
+    TRY(launch_k1v_locked(h, first, n, base, h->d_voffsets, bytes, out ? h->d_verdicts : nullptr, ids ? h->d_ids : nullptr, nlong));
     if (out) CK(cudaMemcpyAsync(h->h_verdicts, h->d_verdicts, (size_t)n * sizeof(agr_verdict), cudaMemcpyDeviceToHost, st));
     if (ids) CK(cudaMemcpyAsync(h->h_ids, h->d_ids, (size_t)n * 16, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
@@ -1287,13 +1320,11 @@ int agr_get_record_var(agr_handle* h, const char* agent_id, const uint8_t reques
     TRY(ensure_out(h, 1));
     CK(cudaMemcpyAsync(h->d_out_rid.p, h->d_hrid, 4, cudaMemcpyDeviceToDevice, h->stream));
     uint64_t bytes = 0;
-    std::vector<uint8_t> tmp(AGR_VAR_MAX_RECORD);
     uint64_t offs[2];
-    TRY(gather_var_locked(h, 1, tmp.data(), tmp.size(), offs, &bytes));
+    TRY(gather_var_locked(h, 1, nullptr, 0, offs, &bytes));      // the record's length, then the record itself
     *len = (uint32_t)bytes;
     if (bytes > cap || !out) return out ? fail(AGR_ECAP, "output buffer too small") : 0;
-    memcpy(out, tmp.data(), bytes);
-    return 0;
+    return gather_var_locked(h, 1, out, cap, offs, &bytes);
 }
 
 // ------------------------------------------------------------------------------------------ stored responses

@@ -189,6 +189,10 @@ struct agr_handle {
     uint32_t* d_slot_off = nullptr;            // 512 i for i = 0 .. slot_off_max: the offsets of a run of 512-byte slots (K1v)
     uint32_t slot_off_max = 0;
     scratch<uint32_t> d_lens; scratch<unsigned long long> d_goffs;      // gather scratch
+    // long records (stored length over AGR_VAR_MAX_RECORD, up to cfg.max_record_bytes): the batch's list for K1v's checksum
+    // pass (agr_launch_k1v_long: batch indices, then first pieces) and, on the device, the list followed by two sums per record
+    std::vector<uint32_t> long_list;
+    scratch<uint32_t> d_long;
     // multi-GPU exchange (K4)
     ncclComm_t comm = nullptr; int rank = 0, world = 1;
     uint8_t* d_stage = nullptr;                // incoming batch before binning [max_batch * 512]

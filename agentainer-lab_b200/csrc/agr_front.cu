@@ -380,6 +380,12 @@ static int submit_one(agr_handle* h, uint32_t kind, const void* item, size_t byt
 }
 int agr_submit_ingest(agr_handle* h, const agr_record* rec, agr_ticket* ticket) {
     if (!h || !rec || !ticket || !h->svc || !(h->cfg.flags & AGR_CFG_VARLEN)) return submit_one(h, SVC_OP_RECORD, rec, sizeof(agr_record), ticket);
+    if (h->cfg.max_record_bytes > AGR_VAR_MAX_RECORD) {         // a long record would be stored whole by agr_ingest_var: refuse, do not cut it
+        uint32_t w[2];
+        memcpy(w, reinterpret_cast<const uint8_t*>(rec) + 76, 8);   // path_len, hdr_len | body_len (as svc_rec_len_at)
+        if ((uint64_t)(w[0] & 0xffffu) + (w[0] >> 16) + w[1] > AGR_VAR_MAX_RECORD - AGR_HEADER_BYTES)
+            return fail(AGR_EINVAL, "record longer than AGR_VAR_MAX_RECORD: a ticket carries at most 8192 B, agr_ingest_var takes longer records");
+    }
     uint64_t a = 0;                                              // a variable-length record: a record span of its stored length
     if (!svc_submit_record(h->svc, reinterpret_cast<const uint8_t*>(rec), &a)) return AGR_EAGAIN;
     *ticket = a;

@@ -8,11 +8,16 @@
 // an mbarrier; a warp-cooperative, position-weighted checksum per record (lane = 16 B chunk, REDUX per record); then
 // the decisions thread-per-record with the same staged functions as the fixed-stride kernel (agr_device.cuh).
 // Algorithmic bytes per record: its stored length (96 + 16-rounded payload) + 8 (SURVEY 8d).
+//
+// A LONG record (stored length over VT_MAXREC, on an engine whose max_record_bytes allows it) is always the last record its
+// tile owns, since nothing else can start before it ends.  K1v stages and decides only its 96-byte header; its checksum comes
+// from k1v_long_sums below, 8 KiB per warp, so that one warp never streams a megabyte alone while the tiles inside the record
+// own nothing.  Records up to VT_MAXREC take the same path as before.
 #include "agr_device.cuh"
 
 #define VT_TILE 8192u                 // bytes of blob per tile
 #define VT_WARPS 16
-#define VT_MAXREC 8192u               // longest legal record (header + payload)
+#define VT_MAXREC 8192u               // longest record K1v sums itself (header + payload); longer ones are long records
 #define VT_TAIL 4608u                 // stage room behind the tile for the last owned record (a 4 KB body fits); a record that
                                       // ends beyond the stage (> 4.5 KiB and badly placed: rare) is read from global memory
 #define VT_STAGE (VT_TILE + VT_TAIL)  // 12800 B = 100 x 128
@@ -74,10 +79,15 @@ k1_ingest_var(const agr_dev d, const uint8_t* __restrict__ blob, const uint32_t*
     // Tile metadata is software-pipelined two tiles deep so that no global-load latency sits on the warp's critical path:
     // while tile T is processed, the record offsets of T+1 are in flight into registers (their range [a1, b1) was read one
     // iteration earlier) and the range of T+2 is being read.  A tile inside one long record owns nothing (cnt == 0).
+    // bytes staged for a tile: its records, of a long last record only the header
+    auto stage_bytes = [](const uint32_t* so, uint32_t cnt) {
+        const uint32_t end = (so[cnt] - so[cnt - 1] > VT_MAXREC) ? so[cnt - 1] + AGR_OFF_PAYLOAD : so[cnt];
+        return min(end - so[0], VT_STAGE);
+    };
     auto issue = [&](int buf, uint32_t cnt) {
         if (lane == 0) {
             const uint32_t start = s_off[warp][buf][0];
-            const uint32_t bytes = min(s_off[warp][buf][cnt] - start, VT_STAGE);
+            const uint32_t bytes = stage_bytes(s_off[warp][buf], cnt);
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
             asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
             asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
@@ -127,12 +137,13 @@ k1_ingest_var(const agr_dev d, const uint8_t* __restrict__ blob, const uint32_t*
             continue;
         }
         const uint32_t* so = s_off[warp][cur];
-        const uint32_t start = so[0], bytes = min(so[cnt] - start, VT_STAGE);
+        const uint32_t start = so[0], bytes = stage_bytes(so, cnt);
         asm volatile("{\n\t.reg .pred p;\n\tW_%=:\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t@p bra D_%=;\n\tbra W_%=;\n\tD_%=:\n\t}"
                      ::"r"(bar), "r"(phase) : "memory");
         phase ^= 1u;
         // ---- checksum: one record at a time, lanes sweep its 16 B chunks (conflict-free), REDUX per record
         for (uint32_t r = 0; r < cnt; ++r) {
+            if (so[r + 1] - so[r] > VT_MAXREC) break;                           // a long last record: k1v_long_sums
             const uint32_t lo = so[r] - start, chunks = (so[r + 1] - so[r]) >> 4;
             const bool in_stage = (so[r + 1] - start) <= bytes;                    // warp-uniform
             const uint8_t* g = blob + so[r];
@@ -166,7 +177,7 @@ k1_ingest_var(const agr_dev d, const uint8_t* __restrict__ blob, const uint32_t*
             k1v_note_time(d, rid, res.state, h4);
             d.state[rid] = res.state;
             d.route[rid] = res.route;
-            d.cksum[rid] = s_ck[warp][r];
+            if (so[r + 1] - so[r] <= VT_MAXREC) d.cksum[rid] = s_ck[warp][r];
             d.voff[rid] = blob_base + so[r];
             d.vlen[rid] = so[r + 1] - so[r];
         };
@@ -195,7 +206,8 @@ k1_ingest_var(const agr_dev d, const uint8_t* __restrict__ blob, const uint32_t*
 // s0 = sum w and s1 = sum (g + 1) w of the chunks it meets and a record's pair is (S0, S1 - 4 lo S0) over the chunks between
 // two record starts.  A bitmap of record-start chunks tells each 32-chunk row where records begin: rows without a start
 // cost a load and a dozen integer ops; a row with a start closes the running record with two REDUX; records that lie
-// entirely inside one row are summed by a segmented shuffle reduction.
+// entirely inside one row are summed by a segmented shuffle reduction.  The sweep stops at the start of a long last record
+// (k1v_long_sums sums it), so it never spans more than the tile and one record of at most VT_MAXREC.
 #define VL_WARPS 8
 #define VL_MAXCH ((VT_TILE + VT_MAXREC) / 16u)         // chunks a tile's sweep can span (1024)
 #define VL_HWORDS (VL_MAXCH / 32u)
@@ -232,8 +244,9 @@ k1_ingest_var_lsu(const agr_dev d, const uint8_t* __restrict__ blob, const uint3
             for (uint32_t k = lane; k <= cnt; k += 32) so[k] = __ldg(&off[a + k]);
             if (lane < (int)VL_HWORDS) hb[lane] = 0;
             __syncwarp();
-            const uint32_t start = so[0], nch = (so[cnt] - start) >> 4;
-            for (uint32_t r = lane; r < cnt; r += 32) { const uint32_t c = (so[r] - start) >> 4; atomicOr(&hb[c >> 5], 1u << (c & 31u)); }
+            const uint32_t swept = cnt - (so[cnt] - so[cnt - 1] > VT_MAXREC ? 1u : 0u);   // records the sweep sums
+            const uint32_t start = so[0], nch = (so[swept] - start) >> 4;
+            for (uint32_t r = lane; r < swept; r += 32) { const uint32_t c = (so[r] - start) >> 4; atomicOr(&hb[c >> 5], 1u << (c & 31u)); }
             __syncwarp();
             const uint8_t* base = blob + start;
             uint32_t a0 = 0, a1s = 0, base_r = 0, cur_r = 0xffffffffu, cur_lo = 0;
@@ -296,7 +309,7 @@ k1_ingest_var_lsu(const agr_dev d, const uint8_t* __restrict__ blob, const uint3
                 k1v_note_time(d, rid, res.state, h4);
                 d.state[rid] = res.state;
                 d.route[rid] = res.route;
-                d.cksum[rid] = s_ck[warp][r];
+                if (r < swept) d.cksum[rid] = s_ck[warp][r];
                 d.voff[rid] = blob_base + so[r];
                 d.vlen[rid] = so[r + 1] - so[r];
             }
@@ -305,6 +318,56 @@ k1_ingest_var_lsu(const agr_dev d, const uint8_t* __restrict__ blob, const uint3
         a = a1; b = b1; a1 = a2; b1 = b2;
     }
     k1_flush_counters(d, lc, s_ctr);
+}
+
+// ---- checksums of long records.  Piece p of a record covers its chunks [512 p, 512 p + 512): lanes on 16 B chunks, all
+// sixteen loads of a lane issued before any is summed.  Word k of the record (k = 4 c + j in chunk c) weighs k + 1 as in K1v,
+// so the pieces' (s0, s1) add up to the record's exactly (mod 2^32 in any order): two atomics per piece, then one pack.
+#define VL_PIECE_CH (VT_TILE / 16u)                    // chunks per piece (512: 16 per lane)
+#define VL_LONG_WARPS 8
+__global__ void __launch_bounds__(VL_LONG_WARPS * 32) k1v_long_sums(const uint8_t* __restrict__ blob, const uint32_t* __restrict__ off,
+                                                                    const uint32_t* __restrict__ list, const uint32_t nl,
+                                                                    const uint32_t npieces, uint32_t* __restrict__ acc) {
+    const uint32_t w = blockIdx.x * VL_LONG_WARPS + (threadIdx.x >> 5);
+    const uint32_t lane = threadIdx.x & 31u;
+    if (w >= npieces) return;
+    const uint32_t* first = list + nl;                  // first[k] = first piece of long record k, first[nl] = npieces
+    uint32_t lo = 0, hi = nl;                           // the k with first[k] <= w < first[k + 1]
+    while (hi - lo > 1u) { const uint32_t m = (lo + hi) >> 1; if (__ldg(&first[m]) <= w) lo = m; else hi = m; }
+    const uint32_t i = __ldg(&list[lo]);
+    const uint32_t o = __ldg(&off[i]), chunks = (__ldg(&off[i + 1]) - o) >> 4;
+    const uint32_t c0 = (w - __ldg(&first[lo])) * VL_PIECE_CH;
+    const uint8_t* g = blob + o;
+    uint4 v[VL_PIECE_CH / 32u];
+#pragma unroll
+    for (uint32_t j = 0; j < VL_PIECE_CH / 32u; ++j) {
+        const uint32_t c = c0 + lane + 32u * j;
+        v[j] = c < chunks ? ldg_nc_v4(g + ((size_t)c << 4)) : make_uint4(0, 0, 0, 0);
+    }
+    uint32_t s0 = 0, s1 = 0;
+#pragma unroll
+    for (uint32_t j = 0; j < VL_PIECE_CH / 32u; ++j) {
+        const uint32_t c = c0 + lane + 32u * j;
+        s0 += v[j].x + v[j].y + v[j].z + v[j].w;
+        s1 += (4u * c + 1u) * v[j].x + (4u * c + 2u) * v[j].y + (4u * c + 3u) * v[j].z + (4u * c + 4u) * v[j].w;
+    }
+    s0 = __reduce_add_sync(FULL, s0);
+    s1 = __reduce_add_sync(FULL, s1);
+    if (lane == 0) { atomicAdd(&acc[2u * lo], s0); atomicAdd(&acc[2u * lo + 1u], s1); }
+}
+__global__ void __launch_bounds__(256) k1v_long_pack(const agr_dev d, const uint32_t* __restrict__ list, const uint32_t nl,
+                                                     const uint32_t* __restrict__ acc, const uint32_t first_rid) {
+    const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k < nl) d.cksum[first_rid + list[k]] = agr_cksum_pack(acc[2u * k], acc[2u * k + 1u]);
+}
+cudaError_t agr_launch_k1v_long(const agr_dev& d, const uint8_t* blob, const uint32_t* off, const uint32_t* list, uint32_t nl,
+                                uint32_t npieces, uint32_t* acc, uint32_t first_rid, cudaStream_t st) {
+    if (nl == 0) return cudaSuccess;
+    const cudaError_t e = cudaMemsetAsync(acc, 0, (size_t)nl * 2u * sizeof(uint32_t), st);
+    if (e != cudaSuccess) return e;
+    k1v_long_sums<<<(npieces + VL_LONG_WARPS - 1u) / VL_LONG_WARPS, VL_LONG_WARPS * 32, 0, st>>>(blob, off, list, nl, npieces, acc);
+    k1v_long_pack<<<(nl + 255u) / 256u, 256, 0, st>>>(d, list, nl, acc, first_rid);
+    return cudaGetLastError();
 }
 
 // gather of variable-length rows: lens pass, then copy pass (offsets are scanned on the host: a per-tick operation)

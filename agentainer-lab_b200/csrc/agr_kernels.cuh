@@ -130,6 +130,11 @@ struct agr_k3_params {
 cudaError_t agr_launch_k1_var(const agr_dev& d, const uint8_t* blob, const uint32_t* off, uint32_t n, unsigned long long blob_bytes,
                               uint32_t* tile_first, uint32_t first_rid, unsigned long long blob_base, int sm_count, cudaStream_t st,
                               uint32_t variant = 0 /* k1_variant: bit 0x20 = LSU form */);
+// The checksums of the batch's LONG records (stored length over AGR_VT_MAXREC), which K1v decides but does not sum: list[0..nl)
+// = their batch indices, list[nl..2 nl] = the index of each one's first 8 KiB piece (list[2 nl] = all pieces); acc = 2 nl
+// scratch words.  One warp per piece, the pieces' sums added per record, then packed into cksum[first_rid + index].
+cudaError_t agr_launch_k1v_long(const agr_dev& d, const uint8_t* blob, const uint32_t* off, const uint32_t* list, uint32_t nl,
+                                uint32_t npieces, uint32_t* acc, uint32_t first_rid, cudaStream_t st);
 // off[i] = 512 i for i = 0 .. n: the offsets K1v reads a run of 512-byte slots by
 void agr_launch_slot_offsets(uint32_t* off, uint32_t n, cudaStream_t st);
 void agr_launch_var_lens(const agr_dev& d, const uint32_t* rids, uint32_t n, uint32_t* lens, cudaStream_t st);

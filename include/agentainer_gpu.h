@@ -110,7 +110,8 @@ typedef struct agr_record {
                                        A batch never wraps: rows left before the end of the slab are skipped (<= max_batch per lap;
                                        max_batch is clamped to slab_rows / 2).  With caller-supplied ids every agr_reclaim rebuilds the dedupe
                                        index from the live rows.  Without the flag the slab is append-only. */
-#define AGR_CFG_VARLEN        0x10u /* variable-length records (BASELINE config 5): byte-addressed slab, agr_ingest_var / *_var reads */
+#define AGR_CFG_VARLEN        0x10u /* variable-length records (BASELINE config 5): byte-addressed slab, agr_ingest_var / *_var reads;
+                                       records up to agr_config.max_record_bytes (default AGR_VAR_MAX_RECORD) */
 #define AGR_CFG_ONLINE_SNAPSHOT 0x80u /* agr_snapshot stops the engine only for a short device-side cut and writes the file while every
                                        other call goes on (see agr_snapshot).  Costs HBM for the cut's shadow: 64 B per slab row
                                        (+ 12 B with AGR_CFG_VARLEN) and 8 B per log_entries, about 88 B per row with the defaults;
@@ -138,7 +139,9 @@ typedef struct agr_config {
     uint32_t k1_variant;     /* | 0x20 = LSU form of the variable-length kernel (AGR_CFG_VARLEN; default: TMA form);
                                 bits 16..23 = k: AGR_CFG_TIMING times every k-th K1 launch (0, 1 = every launch);
                                 every other bit must be 0 (AGR_EINVAL) */
-    uint32_t reserved;
+    uint32_t max_record_bytes; /* AGR_CFG_VARLEN: longest stored length agr_ingest_var accepts; 0 = AGR_VAR_MAX_RECORD.  Otherwise
+                                a multiple of 16 in [AGR_VAR_MAX_RECORD, AGR_VAR_MAX_RECORD_LIMIT] and at most vslab_bytes / 2
+                                (after its default), else AGR_EINVAL.  An ingest rule, not state: snapshots do not carry it */
 } agr_config;
 
 typedef struct agr_handle agr_handle;
@@ -281,7 +284,9 @@ typedef struct agr_result {
  * headers | body) and the call reads its stored length L = 96 + round16(path_len + hdr_len + body_len), capped at
  * AGR_VAR_MAX_RECORD, from rec.  The ticket's result is that of agr_ingest_var of those L bytes as a one-record blob (a header
  * whose lengths exceed AGR_VAR_MAX_RECORD - 96 is decided AGR_VF_BAD_LEN); AGR_ENOSPC when the rows or the record bytes found no
- * room, AGR_EINVAL when the record alone exceeds half a ring's byte slab. */
+ * room, AGR_EINVAL when the record alone exceeds half a ring's byte slab.  Tickets carry at most AGR_VAR_MAX_RECORD bytes: on
+ * an engine whose max_record_bytes is larger, a record whose header gives a stored length over AGR_VAR_MAX_RECORD is
+ * AGR_EINVAL at once (no ticket); agr_ingest_var takes it, as one locked batch that stops the service kernel while it runs. */
 int agr_submit_ingest(agr_handle* h, const agr_record* rec, agr_ticket* ticket);
 int agr_submit_complete(agr_handle* h, const agr_outcome* outcome, agr_ticket* ticket);
 /* agr_submit_complete with the outcome's bytes in the ticket (agr_complete_ex(n = 1) semantics): headers then body for a
@@ -333,12 +338,16 @@ int agr_list(agr_handle* h, const char* agent_id, int which, uint8_t (*ids)[16],
 /* ------------------------------------------------ variable-length records (AGR_CFG_VARLEN) */
 /* A variable-length record is the 96-byte header of agr_record (same fields, same offsets) followed by its payload
  * path | headers | body, zero padded to a multiple of 16 bytes; its stored length is 96 + round16(path_len + hdr_len +
- * body_len) <= AGR_VAR_MAX_RECORD.  A batch is one contiguous blob of such records plus offsets[0..n] (bytes from the
- * start of the blob, offsets[n] = blob length; every offset a multiple of 16).  Semantics are those of agr_ingest_ex.
+ * body_len) <= the engine's max_record_bytes (AGR_VAR_MAX_RECORD unless agr_config sets more).  A batch is one contiguous
+ * blob of such records plus offsets[0..n] (bytes from the start of the blob, offsets[n] = blob length; every offset a multiple
+ * of 16).  Semantics are those of agr_ingest_ex.  A record longer than AGR_VAR_MAX_RECORD (a LONG record) is decided like any
+ * other; its checksum is summed by a pass of its own, 8 KiB per warp, after the batch's decisions.
  * With AGR_CFG_COMBINE, 1 <= n <= 32 and every record in the COMPACT form (offsets[i+1] - offsets[i] = the stored length its
- * header gives), the call goes through the single-request ring like agr_ingest_ex(n <= 32) does, one record per ticket in
- * call order (first_rid: the row of record 0); otherwise it is one locked batch. */
+ * header gives, which is never over AGR_VAR_MAX_RECORD), the call goes through the single-request ring like agr_ingest_ex(n <=
+ * 32) does, one record per ticket in call order (first_rid: the row of record 0); otherwise it is one locked batch — so a long
+ * record always takes the locked path, and each such call stops the service kernel while it runs. */
 #define AGR_VAR_MAX_RECORD 8192u
+#define AGR_VAR_MAX_RECORD_LIMIT 67108864u   /* largest max_record_bytes (2^26) */
 int agr_ingest_var(agr_handle* h, const uint8_t* blob, const uint32_t* offsets, uint32_t n, agr_verdict* out,
                    uint8_t (*ids)[16], uint64_t* first_rid);
 /* agr_replay_scan for variable-length records: dispatch entries as usual; if blob != NULL the stored records are packed
@@ -346,7 +355,8 @@ int agr_ingest_var(agr_handle* h, const uint8_t* blob, const uint32_t* offsets, 
  * AGR_ECAP if either capacity is too small (*n and *blob_bytes hold what is needed). */
 int agr_replay_scan_var(agr_handle* h, agr_dispatch* out, uint8_t* blob, uint64_t blob_cap, uint64_t* offsets, uint32_t cap,
                         uint32_t* n, uint64_t* blob_bytes);
-/* storage.Get for a variable-length record: copies it into out (cap bytes), *len = stored length. */
+/* storage.Get for a variable-length record: copies it into out (cap bytes), *len = stored length (up to the max_record_bytes
+ * of the engine that stored it).  AGR_ECAP when cap is smaller (*len is set); out == NULL asks for *len only. */
 int agr_get_record_var(agr_handle* h, const char* agent_id, const uint8_t request_id[16], uint8_t* out, uint32_t cap, uint32_t* len);
 
 /* ------------------------------------------------- stored responses (requests.go:142-147,165) */
